@@ -21,7 +21,8 @@ Numbers in the JSON line (all: max over ranks, throughput = workers x K / max el
              ps acknowledgement of the last push. `input_feed` in the e2e object says which path fed the timed steps.
   parity   : the reference's worker semantics — one step at a time per worker (`--lanes 1`), host-fed — and the same
              with `--strict_steps` (the next pull waits for the acknowledgement of the previous push).
-  roofline : achieved fraction of the NVLink / HBM / tensor-core rooflines from MEASURED_PEAKS.json.
+  roofline : achieved fraction of the NVLink / HBM / tensor-core rooflines (MEASURED_PEAKS.json when present, else
+             the H100 SXM data sheet).
 
 Steps in flight: a worker keeps `--lanes` (default 12, the CLI's default too) steps in flight on its GPU — bounded-
 staleness asynchronous SGD: every step still pulls, computes, pushes and is applied on the ps individually.
@@ -38,11 +39,9 @@ import time
 import torch
 
 REFERENCE_UNAVAILABLE = (
-    "reference needs TensorFlow 1.x (tf.contrib, tf.app.flags, tf.train.Server); no tensorflow wheel in "
-    "/opt/wheelhouse, none for Python 3.12, no network; /root/reference has no setup.py/pyproject so "
-    "`pip install --target baseline/_ref /root/reference` fails with 'not installable'"
+    "reference needs TensorFlow 1.x (tf.contrib, tf.app.flags, tf.train.Server), which has no build for Python 3.12"
 )
-NVLINK_GBS = 770.0   # measured peer-copy bandwidth per direction per GPU (profiling recipe)
+NVLINK_GBS = 450.0   # H100 SXM NVLink 4 data sheet: 900 GB/s per GPU, i.e. 450 GB/s per direction (not measured)
 
 
 def parse_args(argv=None):
@@ -71,6 +70,12 @@ def parse_args(argv=None):
     p.add_argument("--ps_row_blocks", type=int, default=4)
     p.add_argument("--skip_e2e", action="store_true")
     p.add_argument("--skip_parity", action="store_true")
+    p.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                   help="right after the device-timed steps (before the e2e / parity regions), write the model "
+                        "variables they left on the ps as DIR/<variable>.npy (float32). Inputs and initial values are "
+                        "seeded. With several lanes in flight the ps applies pushes in arrival order, so the values "
+                        "vary from run to run; `--lanes 1 --strict_steps` (each pull waits for the previous push to be "
+                        "applied) makes them repeatable, for comparing two builds output for output")
     return p.parse_args(argv)
 
 
@@ -101,7 +106,8 @@ def load_peaks() -> dict:
             d = json.load(f)
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]), "source": "MEASURED_PEAKS.json"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "source": "fallback (profiling recipe)"}
+        # NVIDIA's H100 SXM data sheet (700 W part): HBM3 bandwidth and dense BF16 rate, not measured figures
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet"}
 
 
 def main(argv=None) -> int:
@@ -131,7 +137,7 @@ def main(argv=None) -> int:
     from dist_mnist_b200.utils.metrics import ClockSampler, StreamTimer
 
     if not torch.cuda.is_available():
-        print(json.dumps({"error": "bench.py needs a CUDA device (B200); none visible"}))
+        print(json.dumps({"error": "bench.py needs a CUDA device (H100); none visible"}))
         return 1
     N.lib()  # fail loudly if the native library is missing: there is no eager fallback for the hot path
 
@@ -165,7 +171,7 @@ def main(argv=None) -> int:
     if is_worker_rank:
         dev = torch.device("cuda", local_rank)
         tdtype = torch.float32 if args.dtype == "fp32" else torch.bfloat16
-        dev_x = ds.images.to(tdtype).to(dev).contiguous()      # 55000 x 784: 172 MB fp32 (> 126 MB L2)
+        dev_x = ds.images.to(tdtype).to(dev).contiguous()      # 55000 x 784: 172 MB fp32 (> 50 MB L2)
         dev_y = ds.labels.to(dev).contiguous()
         torch.cuda.synchronize()
 
@@ -220,7 +226,7 @@ def main(argv=None) -> int:
     phase = [0]
     sync_ms = []
 
-    def full_sync(restart: bool = True):
+    def full_sync(restart: bool = True, while_stopped=None):
         """barrier + torch.cuda.synchronize() on every rank.
 
         A resident persistent PS kernel makes a device synchronise hang, and — because CUDA loads kernels lazily —
@@ -229,7 +235,7 @@ def main(argv=None) -> int:
         then stop their serve kernel (all shard state stays in HBM); only then does every rank run the NCCL
         barrier + synchronise; finally the ps tasks relaunch the kernel and announce it through the store."""
         # (Kept short on purpose: NVLink sublinks drop into a low-power state after tens of milliseconds without
-        # traffic and the first pull after that costs ~200 us — measured, profiles/r2/nvlink_idle_probe.log — so the
+        # traffic and the first pull after that is much slower — so the
         # store polls below spin at 0.2 ms instead of sleeping 10 ms.)
         phase[0] += 1
         ph = phase[0]
@@ -249,6 +255,9 @@ def main(argv=None) -> int:
                     print(f"[ps_stats] sync {ph} rank={rank} shard={ps.task_index} {json.dumps(st)}", file=sys.stderr, flush=True)
         barrier()
         torch.cuda.synchronize()
+        if while_stopped is not None:
+            while_stopped()   # every rank is quiet and no serve kernel is resident
+            barrier()
         if restart:
             for ps in ps_list:
                 ps.restart()
@@ -317,12 +326,23 @@ def main(argv=None) -> int:
         resident_steps(W)
     full_sync()
 
+    def dump_outputs():
+        """What the timed steps computed: the variables their pushes left on the ps, read back as a caller reads them
+        (Worker.read_variables) right after timed region 1, before any other region trains them further."""
+        if worker is None or not worker.is_chief:
+            return
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in worker.read_variables().items():
+            np.save(os.path.join(args.dump_outputs, f"{name.replace('/', '_')}.npy"),
+                    t.detach().to(torch.float32).cpu().numpy())
+
     # ---------------- timed region 1: device-timed steps ----------------
     if worker is not None:
         launches_before = worker.kernel_launches()
         elapsed_ms, host_enqueue_ms = device_timed(K)
         launches = worker.kernel_launches() - launches_before + (0 if engine == "fused" else 1)   # (+ wait_ack kernel)
-    full_sync()
+    full_sync(while_stopped=dump_outputs if args.dump_outputs else None)
     if os.environ.get("DM_FUSED_DEBUG_TS") == "1" and worker is not None and getattr(worker, "_fx_dbg", None) is not None:
         from bench_tools.fused_phases import print_stamps   # in-kernel phase stamps of the timed launch (stderr)
         import contextlib
@@ -402,11 +422,13 @@ def main(argv=None) -> int:
         per_worker = value / n_workers
         roof = {
             "nvlink_frac": (round(value * pbytes / (NVLINK_GBS * 1e9), 4) if world > 1 else None),
-            "nvlink_note": "ps port, each direction: value x param bytes / 770 GB/s (measured peer copy)",
+            "nvlink_note": f"ps port, each direction: value x param bytes / {NVLINK_GBS:g} GB/s (H100 SXM NVLink data sheet)",
             "hbm_frac": round(value * 7 * pbytes / (peaks["hbm_gbs"] * 1e9), 4),
-            "hbm_note": "ps GPU: value x 7 x param bytes (g read, p/m/v read+write) / measured HBM copy bandwidth",
+            "hbm_note": f"ps GPU: value x 7 x param bytes (g read, p/m/v read+write) / {peaks['hbm_gbs']:g} GB/s HBM "
+                        f"bandwidth ({peaks['source']})",
             "tensor_frac": round(per_worker * flops_step / (peaks["bf16_tflops"] * 0.5 * 1e12), 6),
-            "tensor_note": "per worker GPU: steps/s x FLOPs/step / (0.5 x measured bf16 peak = tf32 rate)",
+            "tensor_note": f"per worker GPU: steps/s x FLOPs/step / (0.5 x {peaks['bf16_tflops']:g} TFLOP/s bf16 = tf32 rate; "
+                           f"{peaks['source']})",
             "peaks": peaks,
             "bound": "latency (dependent phases of a 10 MFLOP / 0.64 MB step), not bytes or FLOPs",
         }
@@ -438,7 +460,7 @@ def main(argv=None) -> int:
                 "strict_steps": bool(args.strict_steps),
                 "mailbox_slots": cfg.nslots,
                 "host_enqueue_us_per_step": round(float(mx[7]) * 1e3 / K, 2),
-                "l2_policy": "inputs stream from a 55000x784 device-resident dataset (172 MB fp32 > 126 MB L2); "
+                "l2_policy": "inputs stream from a 55000x784 device-resident dataset (172 MB fp32 > 50 MB L2); "
                              "parameters (0.3 MB) stay L2-resident as in real training",
                 "global_step_after_run": int(mx[5]),
                 "barrier_sync_ms": [round(v, 2) for v in sync_ms[:3]],

@@ -14,20 +14,21 @@ from dist_mnist_b200.utils import data
 NAMES = ["start", "acc1", "rs_bar", "head_in", "softmax", "grads_sent", "ag_bar", "acc2", "staged", "bar3",
          "tile_published(w0)", "result(w0)"]
 KTS = 16
+SM_MHZ = 1980   # H100 SXM maximum SM clock: cycle counts are converted at this rate (a power-limited card runs slower)
 
 
 def print_stamps(buf, tag):
     """Epilogue thread 0 of cluster 0 / CTA 0 stamps 0..9, warp 0 (publisher) stamps 10, 11; first 4 steps."""
     ts = buf.view(4, KTS)
     t0 = int(ts[0, 0])
-    print(f"{tag}: cluster 0, SM cycles (1965 MHz -> /1965 = us); deltas to the previous stamp")
+    print(f"{tag}: cluster 0, SM cycles ({SM_MHZ} MHz -> /{SM_MHZ} = us); deltas to the previous stamp")
     for j in range(4):
         row = [int(ts[j, k]) - t0 for k in range(12)]
         d = [row[k] - row[k - 1] if k else 0 for k in range(10)]
         nxt = (int(ts[j + 1, 0]) - t0 - row[0]) if j + 1 < 4 else None
         print(f"  step {j}: " + " ".join(f"{NAMES[k]}=+{d[k]}" for k in range(1, 10)) +
               f" | publisher: tile at +{row[10] - row[9]} after bar3, result at +{row[11] - row[9]}"
-              f" | step {row[9] - row[0]} cyc = {(row[9] - row[0]) / 1965:.2f} us"
+              f" | step {row[9] - row[0]} cyc = {(row[9] - row[0]) / SM_MHZ:.2f} us"
               + (f", next step starts {nxt} cyc after this one" if nxt is not None else ""))
 
 

@@ -1,4 +1,4 @@
-"""Bring-up checks for the sm_100a kernels against plain PyTorch fp32 references.
+"""Bring-up checks for the sm_90a kernels against plain PyTorch fp32 references.
 
 Each group runs in its own process (a kernel trap poisons the CUDA context) and keeps going after a
 mismatch so one GPU call yields the full picture:

@@ -1,4 +1,4 @@
-// Standalone driver of dm_nvls_probe (dist_mnist_b200/csrc/nvls_sm100.cu): no Python, no torch import, so a run on a
+// Standalone driver of dm_nvls_probe (dist_mnist_b200/csrc/nvls_sm90.cu): no Python, no torch import, so a run on a
 // fresh GPU box costs seconds. Built by bench_tools/build_nvls_probe.sh into bench_tools/bin/nvls_probe.
 //   nvls_probe [n_dev] -> probes the 318 KB parameter set of the 784-100-10 MLP and a 64 MiB buffer.
 #include <cstdio>

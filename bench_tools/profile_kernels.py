@@ -4,14 +4,14 @@ The persistent PS kernel cannot run under ncu (ncu serialises and replays kernel
 another kernel's flags would never finish), so this script launches the *same* kernels with the same launch
 plans against local buffers standing in for the PS shard:
 
-    fwd0   tcgen05 forward GEMM   (W "pulled" by TMA, +bias, relu)
+    fwd0   wgmma forward GEMM     (W "pulled" by TMA, +bias, relu)
     head   fused softmax-CE head  (mailbox push of dW_last / db)
-    dw0    tcgen05 dW GEMM        (epilogue = mailbox push + per-tile flags)
+    dw0    wgmma dW GEMM          (epilogue = mailbox push + per-tile flags)
     ps     ps_serve_kernel        (flags pre-staged by the step above; exits after applying that one push)
 
-    ncu --metrics gpu__time_duration.sum --clock-control none -s 20 -c 40 --csv --log-file gpurun_out/launches.csv \
+    ncu --metrics gpu__time_duration.sum --clock-control none -s 20 -c 40 --csv --log-file profiles/launches.csv \
         python -m bench_tools.profile_kernels --model book --iters 15
-    ncu --set full --clock-control none --import-source on -k regex:gemm_tcgen05 -s 6 -c 3 -o gpurun_out/prof_gemm \
+    ncu --set full --clock-control none --import-source on -k regex:gemm_wgmma -s 6 -c 3 -o profiles/prof_gemm \
         python -m bench_tools.profile_kernels --model book --iters 6
 """
 from __future__ import annotations

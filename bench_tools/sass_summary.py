@@ -1,6 +1,6 @@
 """Per-kernel SASS evidence of the in-tree library (no GPU needed): `python -m bench_tools.sass_summary` rewrites
 profiles/sass/mnemonic_summary.txt (mnemonic histogram per kernel) and profiles/sass/listings/<kernel>.sass (the full
-`cuobjdump -sass` listing of every kernel, one file each) from dist_mnist_b200/libdmnist_sm100a.so."""
+`cuobjdump -sass` listing of every kernel, one file each) from dist_mnist_b200/libdmnist_sm90a.so."""
 import collections
 import re
 import subprocess
@@ -11,18 +11,18 @@ ROOT = Path(__file__).resolve().parent.parent
 KEEP = re.compile(r"^(UTC|LDTM|STTM|UTMA|UBLKCP|SYNCS|RED|ATOM|MEMBAR|CCTL|UCGABAR|ACQBULK|PREEXIT|MUFU\.(RCP|SQRT|RSQ|EX2|LG2)|"
                   r"ERRBAR|FENCE|LDGMC|LDG\.E\.(\d+\.)?STRONG|STG\.E\.(\d+\.)?STRONG|LD\.E\.STRONG|ST\.E\.STRONG|STS\..*CLUSTER|ST\.E.*CLUSTER|MAPA|"
                   r"UMOV.*SR_CgaCtaId|S2UR)")
-HEADER = """SASS mnemonic evidence per kernel of libdmnist_sm100a.so (cuobjdump -sass, sm_100a); regenerate with
+HEADER = """SASS mnemonic evidence per kernel of libdmnist_sm90a.so (cuobjdump -sass, sm_90a); regenerate with
 `python -m bench_tools.sass_summary`.
-UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, UTMALDG = cp.async.bulk.tensor (TMA), UBLKCP = cp.async.bulk,
+HGMMA = wgmma.mma_async, UTMALDG = cp.async.bulk.tensor (TMA), UBLKCP = cp.async.bulk,
 SYNCS = mbarrier, UCGABAR = barrier.cluster, ACQBULK / PREEXIT = griddepcontrol.wait / launch_dependents (PDL),
 RED/REDG = red.global (atomic push, monotone acks), *.STRONG.SYS = system-scope flag ld/st, MUFU.RCP/SQRT = Adam fast path,
 LDGMC.E.ADD.F32x4 = multimem.ld_reduce (in-switch sum over an NVLS multicast team); multimem.st is an STG.E.128.STRONG.SYS whose
-address is a multicast mapping (nvls_sm100.cu)
+address is a multicast mapping (nvls_sm90.cu)
 """
 
 
 def main() -> int:
-    lib = ROOT / "dist_mnist_b200" / "libdmnist_sm100a.so"
+    lib = ROOT / "dist_mnist_b200" / "libdmnist_sm90a.so"
     txt = subprocess.run(["cuobjdump", "-sass", str(lib)], capture_output=True, text=True, check=True).stdout
     out = [HEADER]
     name, counts, n = None, None, 0
@@ -39,7 +39,7 @@ def main() -> int:
             dem = subprocess.run(["c++filt", cur_name], capture_output=True, text=True).stdout.strip() or cur_name
             short = re.sub(r"[^A-Za-z0-9_]+", "_", dem.split("(")[0])[:120]
             body = "\n".join(cur_lines)
-            (ldir / f"{short}.sass").write_text(f"// {dem}\n// {cur_name}  (sm_100a, cuobjdump -sass)\n{body}\n")
+            (ldir / f"{short}.sass").write_text(f"// {dem}\n// {cur_name}  (sm_90a, cuobjdump -sass)\n{body}\n")
             n_files += 1
 
     for line in txt.splitlines():

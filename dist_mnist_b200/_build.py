@@ -1,9 +1,9 @@
-"""In-tree build of the native runtime (`libdmnist_sm100a.so`).
+"""In-tree build of the native runtime (`libdmnist_sm90a.so`).
 
-Every CUDA source is compiled for sm_100a only
-(`-gencode arch=compute_100a,code=sm_100a -lineinfo`); nvcc cross-compiles without a GPU, so this
-runs on the CPU build box. The shared object lands next to this file so it travels to GPU boxes
-with the source snapshot (a JIT cache under ~/.cache would not).
+Every CUDA source is compiled for sm_90a (H100) only
+(`-gencode arch=compute_90a,code=sm_90a -lineinfo`); nvcc cross-compiles without a GPU, so this
+runs on a machine without one. The shared object lands next to this file, so a built tree can be
+copied to a GPU machine as it is (a JIT cache under ~/.cache would not travel with it).
 
     python -m dist_mnist_b200._build [--force] [--verbose]
 """
@@ -19,16 +19,16 @@ from pathlib import Path
 PKG_DIR = Path(__file__).resolve().parent
 CSRC = PKG_DIR / "csrc"
 BUILD_DIR = PKG_DIR.parent / "build" / "native"
-LIB_NAME = "libdmnist_sm100a.so"
+LIB_NAME = "libdmnist_sm90a.so"
 LIB_PATH = PKG_DIR / LIB_NAME
 
-CUDA_SOURCES = ["gemm_sm100.cu", "head_sm100.cu", "ps_apply_sm100.cu", "p2p_sm100.cu", "fused_step_sm100.cu",
-                "nvls_sm100.cu", "executor.cu", "fused_exec.cu", "api.cu"]
+CUDA_SOURCES = ["gemm_sm90.cu", "head_sm90.cu", "ps_apply_sm90.cu", "p2p_sm90.cu", "fused_step_sm90.cu",
+                "nvls_sm90.cu", "executor.cu", "fused_exec.cu", "api.cu"]
 CXX_SOURCES = ["host_runtime.cpp", "loader_api.cpp"]
 HEADERS = ["common.cuh", "protocol.h", "fused.h", "loader.h", "trace.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

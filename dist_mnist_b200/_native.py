@@ -1,4 +1,4 @@
-"""ctypes binding of the native runtime (`libdmnist_sm100a.so`, built in-tree by `_build.py`).
+"""ctypes binding of the native runtime (`libdmnist_sm90a.so`, built in-tree by `_build.py`).
 
 The C ABI is flat (see csrc/api.cu): kernel parameter blocks are ctypes mirrors of the structs in
 csrc/protocol.h and are passed by address; `sizeof` of every mirror is checked against the library
@@ -151,7 +151,7 @@ class FusedParams(C.Structure):
 
 
 class FusedMaps(C.Structure):
-    _fields_ = [("w", (C.c_uint8 * 128) * FUSED_CLUSTER), ("xk", C.c_uint8 * 128), ("xmn", C.c_uint8 * 128),
+    _fields_ = [("w", (C.c_uint8 * 128) * FUSED_CLUSTER), ("xk", C.c_uint8 * 128),
                 ("push", (C.c_uint8 * 128) * FUSED_CLUSTER)]
 
 
@@ -203,7 +203,7 @@ def _declare(l: C.CDLL) -> None:
         "dm_stream_sync": (i, [vp]),
         "dm_stream_query": (i, [vp]),
         "dm_stream_wait_stream": (i, [vp, vp]),
-        "dm_make_tensor_map_2d": (i, [vp, vp, i, u64, u64, u64, u32, u32, i]),
+        "dm_make_tensor_map_2d": (i, [vp, vp, i, u64, u64, u64, u32, u32]),
         "dm_make_tensor_map_3d": (i, [vp, vp, u64, u64, u64, u64, u64, u32, u32]),
         "dm_gemm_smem_bytes": (i, [i, i, i]),
         "dm_launch_gemm": (i, [vp, vp, vp, i, i, i, i, vp]),
@@ -373,25 +373,22 @@ def make_tensor_map_3d(ptr: int, dim0: int, dim1: int, dim2: int, stride1_bytes:
     return buf
 
 
-def make_tensor_map(ptr: int, dtype: int, dim0: int, dim1: int, stride1_bytes: int, box0: int, box1: int,
-                    mn_major: bool = False):
-    """2-D 128-byte-swizzled tensor map over a row-major [dim1][dim0] tensor (dim0 contiguous).
+def make_tensor_map(ptr: int, dtype: int, dim0: int, dim1: int, stride1_bytes: int, box0: int, box1: int):
+    """2-D 128-byte-swizzled (SWIZZLE_128B) tensor map over a row-major [dim1][dim0] tensor (dim0 contiguous).
 
-    MN-major fp32 (tf32) operands need the 32-byte-chunk swizzle variant; everything else uses SWIZZLE_128B.
-    """
+    K-major and MN-major operand tiles use the same swizzle; the kernels address either layout themselves."""
     if stride1_bytes % 16 != 0:
         raise NativeError(f"TMA row stride must be a multiple of 16 bytes, got {stride1_bytes}")
     buf = (C.c_uint8 * TENSOR_MAP_BYTES)()
-    swz = 1 if (mn_major and dtype == DT_F32) else 0
     check(
-        lib().dm_make_tensor_map_2d(C.addressof(buf), ptr, dtype, dim0, dim1, stride1_bytes, box0, box1, swz),
+        lib().dm_make_tensor_map_2d(C.addressof(buf), ptr, dtype, dim0, dim1, stride1_bytes, box0, box1),
         "cuTensorMapEncodeTiled",
     )
     return buf
 
 
 def nvls_probe(n_dev: int, nbytes: int, iters: int = 50) -> tuple[bool, str]:
-    """NVSwitch multicast probe (csrc/nvls_sm100.cu): builds a multicast team over the first ``n_dev`` GPUs of this
+    """NVSwitch multicast probe (csrc/nvls_sm90.cu): builds a multicast team over the first ``n_dev`` GPUs of this
     process, publishes ``nbytes`` from GPU 0 with ``multimem.st``, aggregates with ``multimem.ld_reduce`` and times both
     against unicast peer stores / loads. Returns ``(ok, log)``; never raises on a box without GPUs or NVLS."""
     buf = C.create_string_buffer(1 << 16)

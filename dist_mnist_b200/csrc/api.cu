@@ -172,9 +172,8 @@ int dm_stream_query(void* s) {  // 0 = idle, 1 = busy, <0 error
 // The global address may be a peer-mapped (cudaIpcOpenMemHandle) pointer: the resulting TMA loads
 // then travel over NVLink from the PS shard straight into the consumer's shared memory.
 // ------------------------------------------------------------------------------------------
-// swizzle: 0 = SWIZZLE_128B (16-byte chunks), 1 = SWIZZLE_128B_ATOM_32B (32-byte chunks; MN-major tf32 operands)
 int dm_make_tensor_map_2d(void* out, void* gptr, int dtype, uint64_t dim0, uint64_t dim1, uint64_t stride1_bytes,
-                          uint32_t box0, uint32_t box1, int swizzle) {
+                          uint32_t box0, uint32_t box1) {
   static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
   if (!encode) {
     void* fn = nullptr;
@@ -193,15 +192,15 @@ int dm_make_tensor_map_2d(void* out, void* gptr, int dtype, uint64_t dim0, uint6
   cuuint32_t estr[2] = {1, 1};
   CUtensorMapDataType dt = dtype == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUresult r = encode(&tm, dt, 2, gptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                      CU_TENSOR_MAP_SWIZZLE_128B,
                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[256];
     snprintf(buf, sizeof(buf),
-             "cuTensorMapEncodeTiled failed: CUresult %d (ptr=%p dims=%llu,%llu stride=%llu box=%u,%u swz=%d); "
+             "cuTensorMapEncodeTiled failed: CUresult %d (ptr=%p dims=%llu,%llu stride=%llu box=%u,%u); "
              "row strides must be multiples of 16 bytes", int(r), gptr,
-             (unsigned long long)dim0, (unsigned long long)dim1, (unsigned long long)stride1_bytes, box0, box1, swizzle);
+             (unsigned long long)dim0, (unsigned long long)dim1, (unsigned long long)stride1_bytes, box0, box1);
     g_err = buf;
     return -1;
   }
@@ -265,7 +264,7 @@ int dm_prepare_kernels(int dev) {
   return 0;
 }
 
-// Fused worker-step kernel (fused_step_sm100.cu): direct launch (tests / tools; the engine goes through fused_exec.cu)
+// Fused worker-step kernel (fused_step_sm90.cu): direct launch (tests / tools; the engine goes through fused_exec.cu)
 int dm_launch_fused(const void* maps, const void* params, int lanes, void* stream) {
   dm::FusedMaps m;
   dm::FusedParams p;

@@ -1,9 +1,9 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM,
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA, wgmma,
 // system-scope flag loads/stores for the NVLink peer-memory protocol.
 //
-// Everything here is raw PTX for sm_100a (compile with -gencode arch=compute_100a,code=sm_100a).
-// No CUTLASS/CuTe dependency: the descriptor encodings below follow the PTX ISA tables
-// (smem matrix descriptor, instruction descriptor) for tcgen05.mma kind::tf32 / kind::f16.
+// Everything here is raw PTX for sm_90a (compile with -gencode arch=compute_90a,code=sm_90a).
+// No CUTLASS/CuTe dependency: the descriptor encoding below follows the PTX ISA table of the
+// wgmma shared-memory matrix descriptor.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -26,11 +26,21 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 
-// Spin-wait guard: a kernel that waits longer than this traps instead of hanging the GPU.
-// (A hung GPU costs a gpurun strike; a trap is just a failed test.)
+// Spin-wait guard: a kernel that waits longer than this traps instead of hanging the GPU
+// (a trap is a failed call the host can report; a hang is not).
 #ifndef DM_SPIN_TIMEOUT_NS
 #define DM_SPIN_TIMEOUT_NS (4000000000ull)
 #endif
+
+// SM count of the current device: grid-stride kernels cap their grid at a few CTAs per SM (132 on an H100 SXM, the
+// fallback if the query fails).
+inline int device_sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      n <= 0)
+    return 132;
+  return n;
+}
 
 // ------------------------------------------------------------------------------------------
 // mbarrier
@@ -120,117 +130,63 @@ __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA, sm_90a): D[64 x N] (fp32, registers of the 128 threads of one aligned warpgroup)
+//   += A[64 x K] * B[N x K]^T, B from a shared-memory matrix descriptor (K-major), A from registers.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, sm_100 "version 1".
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-//                (1 = SWIZZLE_128B_BASE32B: 32-byte swizzle chunks, required for MN-major 32-bit operands)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                         uint32_t layout_type = 2) {
+// Shared-memory matrix descriptor, SWIZZLE_128B, K-major (sm_90 layout):
+//   bits [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major)
+//   bits [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024)   [62,64) layout type (1 = SWIZZLE_128B)
+// The tile base is 1024-byte aligned; a k-step inside the 128-byte swizzle atom advances the start address by
+// its byte offset (32 B per k8 tf32 / k16 bf16 step).
+__device__ __forceinline__ uint64_t make_wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout_type & 7u) << 61;
+  d |= static_cast<uint64_t>(1u) << 16;
+  d |= static_cast<uint64_t>(1024u >> 4) << 32;
+  d |= static_cast<uint64_t>(1u) << 62;
   return d;
 }
-
-// Instruction descriptor for kind::tf32 / kind::f16 with fp32 accumulation.
-//   [4,6) c_format (1 = F32)   [7,10) a_format   [10,13) b_format  (0 F16, 1 BF16, 2 TF32)
-//   [15] a_major  [16] b_major (0 = K-major, 1 = MN-major)   [17,23) N>>3   [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t make_idesc(uint32_t fmt, bool a_mn, bool b_mn, uint32_t M,
-                                                         uint32_t N) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (fmt & 7u) << 7;
-  d |= (fmt & 7u) << 10;
-  d |= (a_mn ? 1u : 0u) << 15;
-  d |= (b_mn ? 1u : 0u) << 16;
-  d |= ((N >> 3) & 0x3Fu) << 17;
-  d |= ((M >> 4) & 0x1Fu) << 24;
-  return d;
+// Byte offset of element `c` (element size `es`) of row `r` in a 128-byte-swizzled tile (TMA SWIZZLE_128B,
+// 1024-byte aligned base): the 16-byte chunk j of row r sits at chunk position j ^ (r & 7).
+__device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t c, uint32_t es) {
+  const uint32_t b = c * es;
+  return r * 128u + ((((b >> 4) ^ (r & 7u)) << 4) | (b & 15u));
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keep the accumulator registers of an asynchronous wgmma live across the fence / wait
+__device__ __forceinline__ void wgmma_reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
 template <typename T>
-struct MmaKind;
+struct Wgmma;
 template <>
-struct MmaKind<float> {  // fp32 storage consumed as tf32
-  static constexpr uint32_t kFormat = 2;
-  __device__ static __forceinline__ void mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+struct Wgmma<float> {  // fp32 storage consumed as tf32: k = 8 per instruction
+  static constexpr int kK = 8;
+  // A fragment (m64 x k8, per warp 16 rows): a0 (r, c), a1 (r + 8, c), a2 (r, c + 4), a3 (r + 8, c + 4)
+  // with r = 16 * warp + lane / 4, c = lane % 4
+  __device__ static __forceinline__ void mma(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
   }
 };
 template <>
-struct MmaKind<__nv_bfloat16> {
-  static constexpr uint32_t kFormat = 1;
-  __device__ static __forceinline__ void mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+struct Wgmma<__nv_bfloat16> {  // k = 16 per instruction
+  static constexpr int kK = 16;
+  // A fragment: pairs of consecutive k; a0 (r, 2c..2c+1), a1 (r + 8, 2c..), a2 (r, 2c + 8..), a3 (r + 8, 2c + 8..)
+  __device__ static __forceinline__ void mma(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
   }
 };
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// The same without the implicit wait: several loads can be in flight before one tmem_ld_wait().
-__device__ __forceinline__ void tmem_ld_32x32b_x32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
 // system-scope flags (NVLink peer-memory protocol)
@@ -318,6 +274,9 @@ __device__ __forceinline__ void st_shared_cluster_f32(uint32_t cluster_addr, flo
 __device__ __forceinline__ void st_shared_cluster_v4f32(uint32_t cluster_addr, float a, float b, float c, float d) {
   asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(cluster_addr), "f"(a), "f"(b), "f"(c), "f"(d)
                : "memory");
+}
+__device__ __forceinline__ void st_shared_cluster_v2f32(uint32_t cluster_addr, float a, float b) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void st_shared_cluster_u32(uint32_t cluster_addr, uint32_t v) {
   asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");

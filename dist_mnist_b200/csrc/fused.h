@@ -1,4 +1,4 @@
-// Host-visible interface of the fused worker-step kernel (fused_step_sm100.cu).
+// Host-visible interface of the fused worker-step kernel (fused_step_sm90.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -9,8 +9,7 @@ namespace dm {
 
 struct FusedMaps {
   CUtensorMap w[kFusedCluster];  // hidden weight [H][I] on the shard that owns CTA r's slice (box 32 x 128)
-  CUtensorMap xk;                // x, K-major view for the forward GEMM (box 32 features x 32 rows, SWIZZLE_128B)
-  CUtensorMap xmn;               // x, MN-major view for the dW GEMM (same box, SWIZZLE_128B_ATOM_32B)
+  CUtensorMap xk;                // x (box 32 features x 32 rows, SWIZZLE_128B): forward B operand and dW A operand
   CUtensorMap push[kFusedCluster];  // where CTA r's dW tile goes: [slot][H][I] view of this worker's mailbox for the
                                     // hidden weight on the owning shard (mailbox mode) or of the master copy (atomic
                                     // mode, 1 slot); box 32 x 128 x 1, SWIZZLE_128B — destination of the TMA store

@@ -1,4 +1,4 @@
-// Native worker-side executor for the fused step kernel (fused_step_sm100.cu).
+// Native worker-side executor for the fused step kernel (fused_step_sm90.cu).
 //
 // The reference worker loop is `next_batch(32)` -> `sess.run(train_op, feed_dict)` -> read loss / global_step
 // (/root/reference/distributed_server-basic.py:110-116). Here the steps themselves run inside one persistent

@@ -4,7 +4,7 @@
 // The CPU backend (BASELINE.json config 1: 1 ps + 1 worker on CPU) runs the *same* shard protocol as the
 // GPU path — arena / mailbox / per-item flags / inbox acks (protocol.h) — with POSIX shm standing in for
 // NVLink peer memory and a native thread standing in for the persistent PS kernel. It mirrors
-// ps_serve_kernel in ps_apply_sm100.cu line for line so the protocol logic can be tested without a GPU.
+// ps_serve_kernel in ps_apply_sm90.cu line for line so the protocol logic can be tested without a GPU.
 //
 // Reference parity: tf.train.Server(...).join() serving variable reads / ApplyAdam on the ps task
 // (/root/reference/distributed_server-basic.py:80-83, 102-103).

@@ -40,7 +40,7 @@ struct PushTarget {
   const uint32_t* seq_ptr;  // device-local current push sequence number (1-based); null => seq 1 / slot 0
 };
 
-// Epilogue selection for the tcgen05 GEMM  D[M,N] = A[M,K] * B[N,K]^T  (fp32 accumulators in TMEM)
+// Epilogue selection for the wgmma GEMM  D[M,N] = A[M,K] * B[N,K]^T  (fp32 accumulators)
 enum GemmEpilogue : int {
   // out[n * ldo + m] = f(acc[m][n]) — lanes write consecutive m (coalesced). Forward and dX GEMMs.
   //   f = (+bias[m]) -> (relu) -> (* (mask[n*ldmask+m] > 0)), optional sums over n (bias grads).
@@ -84,7 +84,7 @@ struct GemmParams {
   int pad2_, pad3_;
 };
 
-// Softmax-cross-entropy head (last dense layer + loss + its gradients), see head_sm100.cu
+// Softmax-cross-entropy head (last dense layer + loss + its gradients), see head_sm90.cu
 enum LossKind : int {
   LOSS_BOOK = 0,  // -mean over B x C of labels * log(clip(softmax, 1e-10, 1))   (reference DS:52-53)
   LOSS_XENT = 1,  // mean over B of softmax_cross_entropy_with_logits               (reference DS:35)
@@ -190,10 +190,10 @@ struct PsServeParams {
 };
 
 // ------------------------------------------------------------------------------------------------
-// Fused worker step (fused_step_sm100.cu): one 8-CTA thread-block cluster runs whole training steps of the
+// Fused worker step (fused_step_sm90.cu): one 8-CTA thread-block cluster runs whole training steps of the
 // 784-H-10 MLP (H <= 128, batch <= 32) back to back inside one launch: TMA pull of its K-slice of W from the ps
-// shard, tcgen05 forward (split-K over the cluster, DSMEM reduce-scatter), classifier head, DSMEM all-gather of
-// the pre-activation gradient, tcgen05 dW of its own column slice, gradient push + flag. `lanes` clusters of one
+// shard, wgmma forward (split-K over the cluster, DSMEM reduce-scatter), classifier head, DSMEM all-gather of
+// the pre-activation gradient, wgmma dW of its own column slice, gradient push + flag. `lanes` clusters of one
 // launch work on different steps concurrently.
 // ------------------------------------------------------------------------------------------------
 constexpr int kFusedCluster = 8;

@@ -10,7 +10,7 @@ Two models exist in the reference (`/root/reference/distributed_server-basic.py`
 
 plus the bf16 784-1024-1024-10 configuration named in BASELINE.json. Everything here is generic over the
 hidden-layer list. Weights are stored `[out_features, in_features]` (row-major, `in` contiguous) — the
-K-major operand layout of the forward tcgen05 GEMM — i.e. the transpose of the reference's `[in, out]`
+K-major operand layout of the forward wgmma GEMM — i.e. the transpose of the reference's `[in, out]`
 variables; `to_reference_layout` converts for checkpoints that want TF's orientation.
 
 The torch implementation in this file is the numerical reference for every CUDA kernel test and the compute

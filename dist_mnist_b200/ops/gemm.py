@@ -1,4 +1,4 @@
-"""Python launch plans for the tcgen05 dense-layer GEMM (csrc/gemm_sm100.cu).
+"""Python launch plans for the wgmma dense-layer GEMM (csrc/gemm_sm90.cu).
 
 A `GemmPlan` freezes the TMA tensor maps and the parameter block of one launch; `plan.launch()` enqueues
 it on the current CUDA stream, so plans can be replayed inside a CUDA graph. The three constructors map
@@ -91,16 +91,16 @@ class GemmPlan:
         return N.lib().dm_gemm_smem_bytes(self.params.bn, self.params.stages, int(self.params.splitk_cluster))
 
 
-def _pick_stages(bn: int, kc: int) -> int:
+def _pick_stages(bn: int, kc: int, budget: int = SMEM_BUDGET) -> int:
     stage = TILE_M * 128 + bn * 128
-    return max(1, min(MAX_STAGES, kc, SMEM_BUDGET // stage))
+    return max(1, min(MAX_STAGES, kc, budget // stage))
 
 
 def auto_splits(K: int, dtype: int, mtiles: int) -> int:
-    """Split-K factor for the K-loop GEMMs (forward, dX). Measured on B200 (profiles/gemm_phase_timestamps_*):
-    one CTA streams a 20 KB k-chunk (128-byte-wide TMA boxes) every ~730 cycles, so a 25-chunk K loop costs
-    ~9 us on one SM. The loop is therefore spread over up to 8 CTAs (~3-4 k-chunks each) whose fp32 partial
-    tiles are summed by the last-arriving CTA in a single round of independent L2 loads."""
+    """Split-K factor for the K-loop GEMMs (forward, dX). One CTA streams its K loop one 128-byte-wide TMA box
+    per operand and k-chunk, so a long K loop on one SM is latency bound. The loop is therefore spread over up
+    to 8 CTAs (~3-4 k-chunks each) whose fp32 partial tiles are summed by the last-arriving CTA in a single
+    round of independent L2 loads."""
     kc = ceil_div(K, bke(dtype))
     return max(1, min(8, ceil_div(kc, 3), max(1, 96 // max(1, mtiles))))
 
@@ -193,9 +193,11 @@ def dw_plan(*, dy_ptr: int, x_ptr: int, O: int, I: int, B_pad: int, dtype: int, 
     assert bn % k == 0 and bn <= 256, "MN-major B tile must be whole 128-byte slabs"
     lddy = O if lddy is None else lddy
     ldx = I if ldx is None else ldx
-    tm_a = N.make_tensor_map(dy_ptr, dtype, O, B_pad, lddy * es, k, k, mn_major=True)
-    tm_b = N.make_tensor_map(x_ptr, dtype, I, B_pad, ldx * es, k, k, mn_major=True)
+    tm_a = N.make_tensor_map(dy_ptr, dtype, O, B_pad, lddy * es, k, k)
+    tm_b = N.make_tensor_map(x_ptr, dtype, I, B_pad, ldx * es, k, k)
     p = _base_params(O, I, B_pad, bn, dtype, 1)
+    # the kernel keeps a K-major copy of the MN-major B tile (bn rows x 128 B, + 1 KB alignment) beside the ring
+    p.stages = _pick_stages(bn, p.kc_per_split, SMEM_BUDGET - (bn * 128 + 1024))
     p.epi = N.EPI_ROWMAJOR_PUSH
     p.ldo = I if ldw is None else ldw
     p.push = push
@@ -226,7 +228,7 @@ def dx_plan(*, w_ptr: int, dy_ptr: int, out_ptr: int, mask_ptr: int, O: int, I: 
     ldw = I if ldw is None else ldw
     lddy = O if lddy is None else lddy
     ldo = I if ldo is None else ldo
-    tm_a = N.make_tensor_map(w_ptr, dtype, I, O, ldw * es, k, k, mn_major=True)
+    tm_a = N.make_tensor_map(w_ptr, dtype, I, O, ldw * es, k, k)
     tm_b = N.make_tensor_map(dy_ptr, dtype, O, B_pad, lddy * es, k, B_pad)
     mtiles = ceil_div(I, TILE_M)
     cluster = splitk_mode(B_pad) == "cluster"

@@ -1,4 +1,4 @@
-"""Launch plan for the fused classifier head (csrc/head_sm100.cu): last dense layer + softmax + loss +
+"""Launch plan for the fused classifier head (csrc/head_sm90.cu): last dense layer + softmax + loss +
 accuracy + small-variable gradients + their parameter-server push.
 
 Reference parity: /root/reference/distributed_server-basic.py:52-53 (book loss), :35 (xent loss),

@@ -43,7 +43,7 @@ class OptimizerConfig:
 
 @dataclass(frozen=True)
 class EngineConfig:
-    backend: str = "cuda"            # "cuda" (sm_100a kernels over NVLink peer memory) | "cpu" (shm plumbing backend)
+    backend: str = "cuda"            # "cuda" (sm_90a kernels over NVLink peer memory) | "cpu" (shm plumbing backend)
     dtype: str = "fp32"              # compute dtype of the dense layers: "fp32" (tf32 tensor cores) | "bf16"
     nslots: int = 2                  # mailbox slots per worker (pushes in flight before the worker waits for an ack)
     apply_mode: str = "per_push"     # "per_push" (reference semantics) | "merged"

@@ -6,7 +6,7 @@ Reference parity (`/root/reference/distributed_server-basic.py`):
                optimizer apply ops the workers' sessions dispatch to it. It never exits on its own.
 
 Here the shard lives in one GPU's HBM (or in POSIX shm for the CPU backend); a *persistent kernel*
-(`ps_serve_kernel`, csrc/ps_apply_sm100.cu) — or the native host loop for the CPU backend — polls the
+(`ps_serve_kernel`, csrc/ps_apply_sm90.cu) — or the native host loop for the CPU backend — polls the
 workers' mailbox flags and applies. The Python object only allocates, publishes the peer-memory descriptor,
 attaches workers as they register, and blocks in `join()`.
 """
@@ -204,7 +204,7 @@ class ParameterServer:
     @nvtx_annotate("dm.ps.serve_once")
     def serve_once(self, after_stream: Optional[int] = None, wait: bool = True) -> None:
         """One-shot mode: launch the serve kernel once; it applies every push that is complete in memory and exits
-        after the first sweep that finds nothing (csrc/ps_apply_sm100.cu, PsServeParams::oneshot). `after_stream`:
+        after the first sweep that finds nothing (csrc/ps_apply_sm90.cu, PsServeParams::oneshot). `after_stream`:
         a CUDA stream whose enqueued work (the worker's step kernels) must finish first — the launch is ordered
         behind it with an event, so nothing ever waits for a kernel that has not been launched: safe under
         profilers and sanitizers that serialise kernels."""
@@ -498,6 +498,20 @@ class ParameterServer:
                 self.serve_once()      # one-shot mode as a stand-alone task: apply whatever has arrived
             time.sleep(poll_s)
         self.stop()
+        self._leave_rendezvous()
+
+    def _leave_rendezvous(self, timeout_s: float = 30.0) -> None:
+        """The rendezvous store is served from ps task 0's process: the other ps tasks poll it until they leave `join`,
+        so task 0 returns only after each of them has said it is done with the store (or after `timeout_s`, in case one
+        of them died)."""
+        if self.cluster.num_ps < 2:
+            return
+        if self.task_index != 0:
+            self.rdv.add("session/ps_left", 1)
+            return
+        t0 = time.time()
+        while self.rdv.add("session/ps_left", 0) < self.cluster.num_ps - 1 and time.time() - t0 < timeout_s:
+            time.sleep(0.01)
 
     def close(self) -> None:
         self.stop()

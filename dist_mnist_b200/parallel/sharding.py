@@ -9,7 +9,7 @@ hid_b->ps0, sm_w->ps1, sm_b->ps0); `strategy="byte_balanced"` is the better shar
 
 `strategy="row_split"` additionally splits the hidden weight *inside* the variable: TF stores it `[in, out]`, so a
 TF row split is a split along the input features — exactly the K-slices the CTAs of the fused step kernel own
-(csrc/fused_step_sm100.cu). Slice r of the 8 goes to ps task r % num_ps: every ps shard then serves 1/num_ps of the
+(csrc/fused_step_sm90.cu). Slice r of the 8 goes to ps task r % num_ps: every ps shard then serves 1/num_ps of the
 pull and push bytes of the big variable (the reference's `--ps_hosts` list, DS:73-77, finally balances the flagship
 model); the small variables stay round-robin.
 
@@ -185,7 +185,7 @@ def _items_for(role: str, offset: int, rows: int, cols: int, ld: int, dw_tile_n:
 
 
 def fused_eligible(spec: MLPSpec, batch_size: int, dtype: str = "fp32") -> bool:
-    """Can the fused step kernel (csrc/fused_step_sm100.cu) run this model? One hidden layer of <= 128 units, <= 11
+    """Can the fused step kernel (csrc/fused_step_sm90.cu) run this model? One hidden layer of <= 128 units, <= 11
     classes, batch <= 32, fp32 storage (tf32 MMA), 8 <= ceil(in / 32) <= 32 and in % 4 == 0."""
     sizes = spec.layer_sizes
     if len(sizes) != 2 or dtype != "fp32":

@@ -9,12 +9,12 @@ Reference parity (`/root/reference/distributed_server-basic.py`):
 
 GPU backend, two step engines (`EngineConfig.engine`, resolved by `EngineConfig.resolve_engine`):
   * "fused" (784-H-10 models, H <= 128, batch <= 32, fp32 — the reference's live configuration): whole steps run
-    inside one persistent kernel (csrc/fused_step_sm100.cu): an 8-CTA cluster pulls its K-slices of W from the ps
-    shard(s) with TMA over NVLink, tcgen05 forward with a DSMEM reduce-scatter, head, DSMEM all-gather, tcgen05 dW
+    inside one persistent kernel (csrc/fused_step_sm90.cu): an 8-CTA cluster pulls its K-slices of W from the ps
+    shard(s) with TMA over NVLink, wgmma forward with a DSMEM reduce-scatter, head, DSMEM all-gather, wgmma dW
     whose epilogue pushes into the ps mailbox; `cfg.lanes` clusters work on different steps concurrently. The
     native executor (csrc/fused_exec.cu) feeds it chunk by chunk: gather pool -> pinned staging -> H2D -> one launch.
   * "graph" (any depth / width / bf16): a PDL-linked chain of per-layer kernels inside a CUDA graph (`ops/`,
-    csrc/gemm_sm100.cu, csrc/head_sm100.cu) driven by csrc/executor.cu.
+    csrc/gemm_sm90.cu, csrc/head_sm90.cu) driven by csrc/executor.cu.
 
 CPU backend: same protocol over POSIX shm with torch CPU math (BASELINE.json config 1, plumbing tests).
 """
@@ -616,9 +616,7 @@ class Worker:
                 tp = N.make_tensor_map_3d(base, I, vl.rows, ns, vl.ld * 4, arena * 4, 32, 128)
             C.memmove(C.addressof(m.push[sl.rank]), C.addressof(tp), N.TENSOR_MAP_BYTES)
         xk = N.make_tensor_map(x_ptr, N.DT_F32, I, n_rows, I * 4, 32, 32)
-        xmn = N.make_tensor_map(x_ptr, N.DT_F32, I, n_rows, I * 4, 32, 32, mn_major=True)
         C.memmove(C.addressof(m.xk), C.addressof(xk), N.TENSOR_MAP_BYTES)
-        C.memmove(C.addressof(m.xmn), C.addressof(xmn), N.TENSOR_MAP_BYTES)
         return m
 
     def _build_fused(self) -> None:
@@ -1006,7 +1004,7 @@ class Worker:
                 correct += int(self._ev_cnt_pin.item())
             return loss, correct / max(1, images.shape[0])
         if self.cfg.backend == "cuda":
-            # forward tcgen05 GEMMs (weights pulled from the PS shards) + the head kernel in eval mode; whole
+            # forward wgmma GEMMs (weights pulled from the PS shards) + the head kernel in eval mode; whole
             # batches only (the step kernels are specialised for this worker's batch size).
             self.drain()
             stream = self.compute_stream

@@ -2,11 +2,11 @@
 
 The reference has no race detection of any kind (SURVEY §5 "Race detection / sanitizers": TF's runtime owns every
 queue); here the hand-off between a worker's step clusters and the persistent ps kernel is a hand-written lock-free
-protocol, so besides compute-sanitizer runs on the GPU (``profiles/r2/evidence``) its *design* is checked exhaustively:
+protocol, so besides compute-sanitizer runs on the GPU its *design* is checked exhaustively:
 this module enumerates every interleaving of a small configuration and verifies that none deadlocks, none overwrites a
 mailbox slot the ps has not consumed, and every push is applied exactly once and in order.
 
-What is modelled (csrc/fused_step_sm100.cu, csrc/ps_apply_sm100.cu):
+What is modelled (csrc/fused_step_sm90.cu, csrc/ps_apply_sm90.cu):
 
 * a launch runs ``lanes`` clusters; steps are claimed from one atomic counter (``claim()``, kernel line "first step of
   this cluster"), the *next* step of a lane is claimed in the prologue of its current one;

@@ -4,8 +4,7 @@ stream, sum the replicas inside the switch with `multimem.ld_reduce`, compare wi
     python examples/nvls_multicast_probe.py [n_gpus] [bytes]
 
 Needs >= 2 GPUs visible to one process and a driver / fabric with multicast support
-(CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED). Kernels and team set-up: dist_mnist_b200/csrc/nvls_sm100.cu; numbers measured
-on B200 x2 / x4: profiles/r2/nvls_probe.md. The reference has nothing comparable: its workers re-fetch every variable
+(CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED). Kernels and team set-up: dist_mnist_b200/csrc/nvls_sm90.cu. The reference has nothing comparable: its workers re-fetch every variable
 over gRPC on every step (/root/reference/distributed_server-basic.py:112)."""
 import os
 import sys

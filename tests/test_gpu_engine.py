@@ -1,4 +1,4 @@
-"""End-to-end engine on one B200 (ps + worker in one process): trajectories vs a PyTorch re-implementation."""
+"""End-to-end engine on one H100 (ps + worker in one process): trajectories vs a PyTorch re-implementation."""
 import pytest
 
 pytestmark = pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""Fused step engine on one B200: long-horizon parity with fp32 PyTorch, agreement with the per-layer graph engine,
+"""Fused step engine on one H100: long-horizon parity with fp32 PyTorch, agreement with the per-layer graph engine,
 checkpoint / resume, lane and strictness switching, StopAtStep semantics of the native loop."""
 import pytest
 import torch
@@ -57,8 +57,7 @@ def test_long_horizon_loss_and_accuracy_parity_with_fp32_torch(okind, lr, steps)
     perr = max(float((got[k] - ref_p[k]).norm() / (ref_p[k].norm() + 1e-9)) for k in got)
     print(f"[parity {okind}] {steps} steps: worst per-step loss rel err {worst:.2e}; checkpoints {checks}; "
           f"eval loss engine {loss_e:.5f} vs fp32 {loss_r:.5f}; accuracy {acc_e:.4f} vs {acc_r:.4f}; param rel err {perr:.2e}")
-    # measured on B200: worst per-step loss error 1.8e-3 (SGD, 4000 steps) / 3.3e-3 (Adam, 2000 steps), final parameter
-    # distance 1.1e-3 / 6.6e-3, identical accuracy (profiles/r2/parity_4000_steps.log)
+    # tf32 MMAs against fp32 PyTorch: the bounds leave room for tf32 rounding accumulated over these horizons
     assert abs(acc_e - acc_r) <= 0.005
     assert abs(loss_e - loss_r) <= 0.02 * abs(loss_r) + 1e-6
     assert worst < 1e-2

@@ -1,4 +1,4 @@
-"""sm_100a kernel numerics vs plain PyTorch fp32 references (runs on a B200: `pytest -m gpu`).
+"""sm_90a kernel numerics vs plain PyTorch fp32 references (runs on an H100: `pytest -m gpu`).
 The checks themselves live in bench_tools/gpu_check.py so they can also be run stand-alone."""
 import pytest
 
@@ -12,18 +12,18 @@ def test_native_library_is_loaded_not_a_fallback():
     lib = N.lib()
     assert lib is not None
     maps = open("/proc/self/maps").read()
-    assert "libdmnist_sm100a.so" in maps
+    assert "libdmnist_sm90a.so" in maps
 
 
-def test_tcgen05_forward_gemm():
+def test_wgmma_forward_gemm():
     assert gpu_check.check_gemm_fwd()
 
 
-def test_tcgen05_dw_gemm_with_push_epilogue():
+def test_wgmma_dw_gemm_with_push_epilogue():
     assert gpu_check.check_gemm_dw()
 
 
-def test_tcgen05_dx_gemm():
+def test_wgmma_dx_gemm():
     assert gpu_check.check_gemm_dx()
 
 

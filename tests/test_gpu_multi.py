@@ -1,4 +1,4 @@
-"""Multi-GPU tests (need >= 2 B200s on one box; skipped otherwise): separate OS processes exchange CUDA IPC
+"""Multi-GPU tests (need >= 2 H100s on one machine; skipped otherwise): separate OS processes exchange CUDA IPC
 handles through the rendezvous and train over NVLink peer memory."""
 import json
 import os
@@ -97,9 +97,9 @@ def test_documented_topology_one_process_per_gpu(n_ps, extra):
 
 
 def test_nvls_multicast_publish_and_in_switch_reduce():
-    """NVSwitch multicast over every visible GPU of this process (csrc/nvls_sm100.cu): `multimem.st` publish lands bit
+    """NVSwitch multicast over every visible GPU of this process (csrc/nvls_sm90.cu): `multimem.st` publish lands bit
     for bit in every replica, `multimem.ld_reduce` returns the exact sum over the replicas. Run in a fresh process
-    (the probe creates VMM mappings and enables peer access itself). Measured: profiles/r2/nvls_probe.md."""
+    (the probe creates VMM mappings and enables peer access itself)."""
     _need_gpus(2)
     n = min(torch.cuda.device_count(), 8)
     code = ("from dist_mnist_b200 import _native as N\n"

@@ -1,6 +1,6 @@
 """Exhaustive interleaving check of the fused engine's mailbox protocol (dist_mnist_b200/utils/protocol_model.py).
 
-The deferred-publish guard of csrc/fused_step_sm100.cu (`deferred = ... && (nxt - cur) < (nslots >> 1)`) exists because
+The deferred-publish guard of csrc/fused_step_sm90.cu (`deferred = ... && (nxt - cur) < (nslots >> 1)`) exists because
 the unguarded version deadlocked on the GPU; the model reproduces that deadlock and shows that the guarded protocol, the
 immediate-publish protocol and `--strict_steps` have none, never overwrite an unconsumed mailbox slot and apply every push
 exactly once, in order — for every interleaving of every small configuration."""

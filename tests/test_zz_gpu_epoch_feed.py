@@ -1,4 +1,4 @@
-"""Epoch feed of the fused executor on a real B200 (csrc/fused_exec.cu, csrc/loader.h): steps fed as contiguous slices of
+"""Epoch feed of the fused executor on a real H100 (csrc/fused_exec.cu, csrc/loader.h): steps fed as contiguous slices of
 the pinned epoch buffer must see exactly the `next_batch` sequence (/root/reference/distributed_server-basic.py:111).
 The host-side logic is covered on CPU by tests/test_fexec_emulated.py; this is the same check through the real DMA
 engine and the real kernel. (Sorted last on purpose: it is the newest GPU test.)"""
