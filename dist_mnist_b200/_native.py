@@ -116,7 +116,7 @@ class PsServeParams(C.Structure):
 FUSED_CLUSTER = 8
 FUSED_MAX_CHUNKS = 4
 FUSED_MAX_SHARDS = 8
-FUSED_ROWS_PER_SLOT = 32
+FUSED_ROW_TILE = 32   # rows of one row tile of the fused kernel; a batch occupies round_up(batch, 32) rows
 
 
 class FusedSlice(C.Structure):
@@ -262,8 +262,8 @@ def _declare(l: C.CDLL) -> None:
         "dm_exec_kernel_launches": (u64, [vp]),
         "dm_exec_destroy": (i, [vp]),
         "dm_launch_fused": (i, [vp, vp, i, vp]),
-        "dm_fused_max_lanes": (i, [i, C.POINTER(i)]),
-        "dm_fused_smem_bytes": (i, []),
+        "dm_fused_max_lanes": (i, [i, i, C.POINTER(i)]),
+        "dm_fused_smem_bytes": (i, [i]),
         "dm_nvls_probe": (i, [i, sz, i, C.c_char_p, sz]),
         "dm_fexec_last_error": (C.c_char_p, []),
         "dm_fexec_create": (i, [i, i, i, i, i, C.POINTER(vp)]),

@@ -77,8 +77,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="variable -> ps placement: round_robin = the reference's replica_device_setter; row_split also "
                         "splits the hidden weight along its input features over every ps task (fused engine)")
     p.add_argument("--engine", choices=["auto", "fused", "graph"], default="auto",
-                   help="fused: one persistent kernel runs whole steps (784-H-10, H <= 128, batch <= 32, fp32); "
-                        "graph: per-layer kernels in a CUDA graph (any model / dtype)")
+                   help="fused: one persistent kernel runs whole steps (784-H-10, H <= 128, batch <= 256, fp32); "
+                        "graph: per-layer kernels in a CUDA graph (any model / dtype); auto: fused for eligible "
+                        "models up to batch 32 (any eligible batch with --sharding row_split), graph otherwise")
     p.add_argument("--nslots", type=int, default=0, help="mailbox slots per worker (0 = max(4 x lanes, 8))")
     p.add_argument("--lanes", type=int, default=DEFAULT_LANES,
                    help="steps of this worker in flight at once: bounded-staleness asynchronous SGD inside one worker "

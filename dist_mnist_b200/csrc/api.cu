@@ -273,12 +273,12 @@ int dm_launch_fused(const void* maps, const void* params, int lanes, void* strea
   DM_CUDA(dm::launch_fused_step(m, p, lanes, static_cast<cudaStream_t>(stream)));
   return 0;
 }
-int dm_fused_max_lanes(int dev, int* out) {
+int dm_fused_max_lanes(int dev, int batch, int* out) {
   DM_CUDA(cudaSetDevice(dev));
-  DM_CUDA(dm::fused_max_lanes(out));
+  DM_CUDA(dm::fused_max_lanes(batch, out));
   return 0;
 }
-int dm_fused_smem_bytes() { return static_cast<int>(dm::fused_smem_bytes()); }
+int dm_fused_smem_bytes(int batch) { return static_cast<int>(dm::fused_smem_bytes(batch)); }
 
 int dm_launch_gemm(const void* tmA, const void* tmB, const void* params, int dtype, int a_mn, int b_mn, int splits,
                    void* stream) {

@@ -190,7 +190,8 @@ struct GatherPool {
 
 constexpr int kChunkMax = 16;   // steps per chunk buffer
 constexpr int kBuffers = 4;     // chunk buffers in rotation
-constexpr int kRowsPerSlot = 32;
+constexpr int kRowTile = 32;         // rows of one row tile of the fused kernel
+constexpr int kMaxBatch = 256;       // 8 row tiles
 constexpr int kRowsPerTask = 8;   // rows of a batch gathered by one pool task
 
 struct ChunkBuf {
@@ -205,6 +206,7 @@ struct ChunkBuf {
 struct FusedExec {
   int device = 0, lanes = 1, n_threads = 4;
   int I = 0, C = 0, batch = 0;
+  int rows = 0;                // rows of a ring slot: the batch rounded up to whole 32-row tiles (rows >= batch zero)
   size_t x_slot_bytes = 0, y_slot_bytes = 0;
   uint8_t *x_dev = nullptr, *y_dev = nullptr, *x_stage = nullptr, *y_stage = nullptr;
   dm::StepResult* res_chunks = nullptr;   // pinned [kBuffers][kChunkMax]
@@ -308,8 +310,8 @@ const char* dm_fexec_last_error() { return g_fx_err.c_str(); }
 
 int dm_fexec_create(int device, int lanes, int I, int C, int batch, void** out) {
   FX_CUDA(cudaSetDevice(device));
-  if (lanes < 1 || batch < 1 || batch > kRowsPerSlot || (I & 3) != 0) {
-    g_fx_err = "fused executor: need lanes >= 1, 1 <= batch <= 32, in_features % 4 == 0";
+  if (lanes < 1 || batch < 1 || batch > kMaxBatch || (I & 3) != 0) {
+    g_fx_err = "fused executor: need lanes >= 1, 1 <= batch <= 256, in_features % 4 == 0";
     return -1;
   }
   FusedExec* ex = new FusedExec();
@@ -318,8 +320,9 @@ int dm_fexec_create(int device, int lanes, int I, int C, int batch, void** out) 
   ex->I = I;
   ex->C = C;
   ex->batch = batch;
-  ex->x_slot_bytes = static_cast<size_t>(kRowsPerSlot) * I * 4;
-  ex->y_slot_bytes = static_cast<size_t>(kRowsPerSlot) * C * 4;
+  ex->rows = (batch + kRowTile - 1) / kRowTile * kRowTile;
+  ex->x_slot_bytes = static_cast<size_t>(ex->rows) * I * 4;
+  ex->y_slot_bytes = static_cast<size_t>(ex->rows) * C * 4;
   const size_t slots = static_cast<size_t>(kBuffers) * kChunkMax;
   FX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ex->x_dev), slots * ex->x_slot_bytes));
   FX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ex->y_dev), slots * ex->y_slot_bytes));
@@ -355,7 +358,8 @@ int dm_fexec_create(int device, int lanes, int I, int C, int batch, void** out) 
   return 0;
 }
 
-// Device / staging ring buffers: [kBuffers * kChunkMax slots][32 rows][I] fp32 and [..][32][C] fp32, and the control words.
+// Device / staging ring buffers: [kBuffers * kChunkMax slots][rows][I] fp32 and [..][rows][C] fp32 (rows: the batch
+// rounded up to a multiple of 32), and the control words.
 int dm_fexec_buffers(void* h, void** x_dev, void** y_dev, void** x_stage, void** y_stage, void** ctl_dev, int* slots) {
   FusedExec* ex = static_cast<FusedExec*>(h);
   *x_dev = ex->x_dev;
@@ -434,7 +438,7 @@ int dm_fexec_drain(void* h) {
   return 0;
 }
 
-// n steps (n <= kChunkMax) on host batches laid out like the staging ring (x [n][32][I], y [n][32][C]; rows >= batch
+// n steps (n <= kChunkMax) on host batches laid out like the staging ring (x [n][rows][I], y [n][rows][C]; rows >= batch
 // zero): H2D + one launch + wait. Results to out[n]. The `step()` / `submit` path of the public API.
 int dm_fexec_steps_host(void* h, const void* x_host, const void* y_host, uint32_t n, void* out, uint32_t* n_done) {
   FusedExec* ex = static_cast<FusedExec*>(h);
@@ -486,9 +490,10 @@ int dm_fexec_run(void* h, void* loader, uint64_t n_steps, void* out_results, uin
       sz = std::min<uint32_t>(sz * 2, kChunkMax);
     }
   }
-  // epoch feed usable with this executor's ring geometry: a slot is exactly one dense batch
-  bool feed_ok = ld->feed && !ex->feed_broken && ld->batch == kRowsPerSlot &&
-                 ld->x_row_bytes * kRowsPerSlot == ex->x_slot_bytes && ld->y_row_bytes * kRowsPerSlot == ex->y_slot_bytes;
+  // epoch feed usable with this executor's ring geometry: a slot is exactly one dense batch (the batch is a multiple of
+  // 32 rows, so no slot has padding rows)
+  bool feed_ok = ld->feed && !ex->feed_broken && ld->batch == ex->rows &&
+                 ld->x_row_bytes * ex->rows == ex->x_slot_bytes && ld->y_row_bytes * ex->rows == ex->y_slot_bytes;
   const size_t nchunks = sizes.size();
   std::vector<uint64_t> first(nchunks + 1, 0);
   for (size_t c = 0; c < nchunks; ++c) first[c + 1] = first[c] + sizes[c];
@@ -641,7 +646,7 @@ int dm_fexec_run(void* h, void* loader, uint64_t n_steps, void* out_results, uin
       if (e == cudaSuccess) e = cudaStreamWaitEvent(ex->compute, b.copied, 0);
       if (e != cudaSuccess) { rc = fxfail("chunk transfer", e); break; }
       dm::FusedParams p = ex->params;
-      p.row_start = static_cast<uint64_t>(slot0) * kRowsPerSlot;
+      p.row_start = static_cast<uint64_t>(slot0) * ex->rows;
       // seq_base of this chunk assumes every earlier chunk of the run completes all its steps; if one is cut short
       // by the stop condition the (persistent) stop word keeps every later chunk from claiming anything
       const uint64_t saved = ex->steps_done;
@@ -692,7 +697,8 @@ int dm_fexec_run(void* h, void* loader, uint64_t n_steps, void* out_results, uin
 }
 
 // One launch for n_steps over a device-resident dataset: `maps` are tensor maps over the dataset, the batch of step s
-// is rows [(row_start + s * row_stride) % row_wrap, +32). Asynchronous: returns after enqueueing (dm_fexec_drain /
+// is rows [(row_start + s * row_stride) % row_wrap, + batch); the kernel reads whole 32-row tiles, so the maps must
+// cover `rows` rows from there. Asynchronous: returns after enqueueing (dm_fexec_drain /
 // dm_fexec_resident_results complete it).
 // `timed` != 0: the launch is bracketed by two CUDA events recorded on the compute stream immediately before and after
 // it (no interpreter time in between); dm_fexec_last_elapsed_ms returns their distance.

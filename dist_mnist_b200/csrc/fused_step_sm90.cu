@@ -34,6 +34,14 @@
 // step's W / x loads are issued as soon as the forward MMAs of the current step have drained the buffers
 // (`strict` = 0), i.e. the pull of step s+1 overlaps the backward half of step s.
 //
+// Batches of 33..256 rows (fused_step_kernel<kFsMaxTiles>): a step is T = ceil(B / 32) row tiles of 32 rows. W and the
+// small variables are pulled once per step and stay resident for all T tiles (the next step's pull is issued after
+// barrier #1 of the last tile); each tile loads its own x rows (row0 + 32 t, same tensor map) and runs the phases above
+// with barriers #1 and #2, and #3 closes the step. The forward's x of tile t + 1 goes into Xk after barrier #1 of tile
+// t, the dW GEMM's copy into Xmn once tile t's dW MMAs are done (bar_xmn_empty). The dW staging tile and the small
+// gradients / loss / correct count add up over the tiles in shared memory and are pushed once per step, the loss
+// normalised by the whole batch. B <= 32 runs fused_step_kernel<1>, whose code is that of the one-tile kernel.
+//
 // SURVEY K1-K6, K12, X3-X5 for the flagship model; deeper / wider / bf16 models use the per-layer kernels
 // (gemm_sm90.cu, head_sm90.cu) chained in a CUDA graph.
 #include "common.cuh"
@@ -64,7 +72,7 @@ constexpr uint32_t kOffDbl = kOffDl + kFsRows * kFsMaxC * 4;         // [8][16] 
 constexpr uint32_t kOffScal = kOffDbl + 8 * kFsMaxC * 4;             // [8][2]      loss / correct partials (CTA 0)
 constexpr uint32_t kOffRedw = kOffScal + 8 * 2 * 4;                  // [8]         warp partials
 constexpr uint32_t kOffCtl = kOffRedw + 8 * 4;                       // next-step words [2]
-constexpr uint32_t kOffBar = kOffCtl + 32;                           // 2 mbarriers
+constexpr uint32_t kOffBar = kOffCtl + 32;                           // mbarriers (2; the multi-tile kernel: 4)
 constexpr uint32_t kOffRawWl = (kOffBar + 64 + 127) & ~127u;         // W_last as it sits in the arena [C][H] (bulk copy)
 constexpr uint32_t kOffRawB = kOffRawWl + (kFsPart - 1) * 128 * 4;   // hidden bias [H]
 constexpr uint32_t kOffRawBl = kOffRawB + 128 * 4;                   // b_last [C]
@@ -75,6 +83,16 @@ static_assert(kOffA % 1024 == 0 && kOffXk % 1024 == 0 && kOffXmn % 1024 == 0, "s
 static_assert(kOffBar % 8 == 0 && kOffRed % 16 == 0 && kOffSg % 16 == 0 && kOffRawWl % 16 == 0 && kOffRawB % 16 == 0 &&
               kOffRawBl % 16 == 0 && kOffStage % 1024 == 0, "alignment");
 static_assert(kFsSmemBytes <= 227 * 1024, "shared memory budget");
+// Batches of more than 32 rows run as several 32-row tiles per step (the multi-tile instantiation). Its running sums
+// of the small gradients over the tiles of a step live behind the one-tile layout, which is left exactly as it is.
+constexpr int kFsMaxTiles = 8;                                       // 256 rows
+constexpr uint32_t kOffAcc = kFsSmemUsed;                            // [12][128]   dW_last / db_hidden of unit et
+constexpr uint32_t kOffAccDbl = kOffAcc + kFsPart * 128 * 4;         // [16]        db_last of my rows
+constexpr uint32_t kOffAccScal = kOffAccDbl + kFsMaxC * 4;           // [2]         loss / correct of my rows
+constexpr uint32_t kFsMultiSmemBytes = kOffAccScal + 2 * 4 + 1024;
+static_assert(kFsMultiSmemBytes <= 227 * 1024, "shared memory budget (multi-tile)");
+template <int kMaxTiles>
+constexpr uint32_t fs_smem_bytes() { return kMaxTiles == 1 ? kFsSmemBytes : kFsMultiSmemBytes; }
 
 // pre^T block [64 x 32] += W [64 x k8] . x [32 x k8]^T, both operands from shared memory (tf32)
 __device__ __forceinline__ void fs_mma_m64n32(float (&d)[4][4], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
@@ -152,8 +170,11 @@ __device__ __forceinline__ void fs_wait_acks(const FusedParams& p, uint32_t need
   }
 }
 
+// kMaxTiles == 1: B <= 32, one row tile per step. kMaxTiles > 1: T = ceil(B / 32) row tiles per step (see the header).
+template <int kMaxTiles>
 __global__ void __launch_bounds__(kFsThreads, 1)
 fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant__ FusedParams p) {
+  constexpr bool kMulti = kMaxTiles > 1;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sbase = smem_u32(smem);
@@ -164,7 +185,9 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
   const int nkc = sl.kc_count;
 
   uint64_t* bar_w = reinterpret_cast<uint64_t*>(smem + kOffBar);   // W + x (K-major) of a step have landed
-  uint64_t* bar_xmn = bar_w + 1;                                    // the dW GEMM's copy of x of a step has landed
+  uint64_t* bar_xmn = bar_w + 1;                                    // the dW GEMM's copy of x of a tile has landed
+  uint64_t* bar_xk = bar_w + 2;          // multi-tile: the forward's x of tile t >= 1 has landed (W stays resident)
+  uint64_t* bar_xmn_empty = bar_w + 3;   // multi-tile: the dW MMAs of tile t < T - 1 are done with Xmn
   volatile uint32_t* ctl_next = reinterpret_cast<volatile uint32_t*>(smem + kOffCtl);
 
   if (p.debug_ts != nullptr && blockIdx.y == 0 && rank == 0 && threadIdx.x == 0)
@@ -174,6 +197,10 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
     prefetch_tensormap(&maps.xk);
     mbar_init(bar_w, 1);
     mbar_init(bar_xmn, 1);
+    if constexpr (kMulti) {
+      mbar_init(bar_xk, 1);
+      mbar_init(bar_xmn_empty, 128);
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -200,6 +227,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
   if (dbg && threadIdx.x == 0) p.debug_ts[61] = static_cast<long long>(globaltimer_ns());   // first step claimed
   const bool mailbox = p.shard[0].push.mode == PUSH_MAILBOX;
   const int H = p.H, C = p.C, B = p.B;
+  const int T = kMulti ? (B + 31) >> 5 : 1;   // row tiles per step
   const uint32_t wl_bytes = (static_cast<uint32_t>(C * H) * 4u + 15u) & ~15u;   // bulk copies move 16-byte multiples
   const uint32_t b_bytes = (static_cast<uint32_t>(H) * 4u + 15u) & ~15u;        // (the arena pads every variable)
   const uint32_t bl_bytes = (static_cast<uint32_t>(C) * 4u + 15u) & ~15u;
@@ -220,16 +248,19 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
       bulk_load_1d(smem + kOffRawB, p.bias_h, b_bytes, bar_w);
       bulk_load_1d(smem + kOffRawBl, p.b_last, bl_bytes, bar_w);
     };
-    auto issue_xmn = [&](uint32_t step) {
-      if (nkc == 0) { mbar_arrive(bar_xmn); return; }
-      const int row0 = static_cast<int>(fs_row0(p, step));
-      mbar_arrive_expect_tx(bar_xmn, static_cast<uint32_t>(nkc) * kFsXChunk);
+    // x rows of row tile t of a step into one of the two x buffers (Xmn: the dW GEMM's copy; Xk: the forward's copy
+    // of tiles t >= 1 — tile 0's rides on bar_w with W)
+    auto issue_x = [&](uint32_t step, int t, uint32_t off, uint64_t* bar) {
+      if (nkc == 0) { mbar_arrive(bar); return; }
+      const int row0 = static_cast<int>(fs_row0(p, step)) + 32 * t;
+      mbar_arrive_expect_tx(bar, static_cast<uint32_t>(nkc) * kFsXChunk);
       for (int i = 0; i < nkc; ++i)
-        tma_load_2d(smem + kOffXmn + i * kFsXChunk, &maps.xk, bar_xmn, (sl.kc_begin + i) * 32, row0);
+        tma_load_2d(smem + off + i * kFsXChunk, &maps.xk, bar, (sl.kc_begin + i) * 32, row0);
     };
+    auto issue_xmn = [&](uint32_t step, int t) { issue_x(step, t, kOffXmn, bar_xmn); };
     if (lane == 0 && cur != kFusedNoStep) {
       issue_wx(cur);
-      issue_xmn(cur);
+      issue_xmn(cur, 0);
     }
     __syncwarp();
     const float* scal = reinterpret_cast<const float*>(smem + kOffScal);
@@ -283,21 +314,38 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
     bool deferred = false;   // `pend` holds a finished step whose publishing was deferred into this step's head phase
     for (uint32_t jl = 0; cur != kFusedNoStep; ++jl) {
       const uint32_t seq = p.seq_base + cur + 1u;
-      if (!arrived1) cluster_barrier_arrive_release();
-      cluster_barrier_wait_acquire();                       // #1: the forward MMAs have drained the W / x tiles
-      const uint32_t nxt = ctl_next[(jl + 1) & 1];
-      if (lane == 0 && !p.strict && nxt != kFusedNoStep) issue_wx(nxt);   // W / x buffers are free: pull ahead
-      __syncwarp();
-      if (deferred) {
-        // EARLY ARRIVAL at barrier #2, then the previous step is published while the other warps run this step's
-        // head: nothing they do before their staging writes (which come after barrier #2) involves this warp.
-        cluster_barrier_arrive_release();                   // #2 (arrive)
-        if (lane == 0) publish(pend);
+      uint32_t nxt = kFusedNoStep;
+      // Row tiles: barriers #1 and #2 are passed once per tile (cluster barriers count every thread), #3 once per step.
+      for (int t = 0; t < T; ++t) {
+        const bool last = t == T - 1;
+        if (t > 0 || !arrived1) cluster_barrier_arrive_release();
+        cluster_barrier_wait_acquire();                     // #1: the forward MMAs have drained the W / x tiles
+        if (t == 0) nxt = ctl_next[(jl + 1) & 1];
+        if (!last) {
+          if (lane == 0) issue_x(cur, t + 1, kOffXk, bar_xk);   // x of the next tile (W stays for the whole step)
+        } else if (lane == 0 && !p.strict && nxt != kFusedNoStep) {
+          issue_wx(nxt);                                    // W / x buffers are free: pull ahead
+        }
         __syncwarp();
-        cluster_barrier_wait_acquire();                     // #2 (wait)
-        deferred = false;
-      } else {
-        cluster_sync_all();                                 // #2
+        if (t == 0 && deferred) {
+          // EARLY ARRIVAL at barrier #2, then the previous step is published while the other warps run this step's
+          // head: nothing they do before their staging writes (which come after barrier #2) involves this warp.
+          cluster_barrier_arrive_release();                 // #2 (arrive)
+          if (lane == 0) publish(pend);
+          __syncwarp();
+          cluster_barrier_wait_acquire();                   // #2 (wait)
+          deferred = false;
+        } else {
+          cluster_sync_all();                               // #2
+        }
+        if (!last) {
+          // the next tile's copy of x for the dW GEMM, once this tile's dW MMAs have read Xmn
+          if (lane == 0) {
+            if (nkc > 0) mbar_wait(bar_xmn_empty, (jl * static_cast<uint32_t>(T - 1) + static_cast<uint32_t>(t)) & 1u);
+            issue_xmn(cur, t + 1);
+          }
+          __syncwarp();
+        }
       }
       // ---- the gradient push: the epilogue warps have staged the dW tile (swizzled, fence.proxy.async'ed) ----
       named_bar_sync(2, 160);
@@ -327,7 +375,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 #pragma unroll
         for (int src = 0; src < kFusedCluster; ++src) { pend.loss += scal[src * 2]; pend.corr += scal[src * 2 + 1]; }
       }
-      if (lane == 0 && nxt != kFusedNoStep) issue_xmn(nxt);  // (the dW MMAs that read the second x tile are complete)
+      if (lane == 0 && nxt != kFusedNoStep) issue_xmn(nxt, 0);   // (the dW MMAs that read the second x tile are complete)
       // Publishing costs several memory round trips (an NVLink round trip when the ps is remote): store completion,
       // a system-scope fence, the flags, the step result. It is deferred into the next step's head phase (see above)
       // unless (a) strict mode wants the acknowledgement before the next pull, (b) this was the cluster's last step,
@@ -373,297 +421,337 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
     // head role of this thread: warp q handles batch row q of this CTA; lane -> (class hc, k-half kh)
     const int hc = lane >> 1, kh = lane & 1;
     const bool hc_ok = hc < C;
-    const int brow = static_cast<int>(rank) * kFsRows + q;
-    const bool hrow_ok = brow < B;
+    const int brow = static_cast<int>(rank) * kFsRows + q;   // row of the head role inside a 32-row tile
+    float* acc = reinterpret_cast<float*>(smem + kOffAcc);   // multi-tile running sums (see kOffAcc)
+    float* acc_dbl = reinterpret_cast<float*>(smem + kOffAccDbl);
+    float* acc_scal = reinterpret_cast<float*>(smem + kOffAccScal);
 
     for (uint32_t jl = 0; cur != kFusedNoStep; ++jl) {
       const uint32_t seq = p.seq_base + cur + 1u;
       if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 0] = clock64();
       // ---- step prologue ----
       if (is_claimer) broadcast_next((jl + 1) & 1, claim());
-      float ylab = 0.f;
-      if (hrow_ok && hc_ok) ylab = p.y_base[(fs_row0(p, cur) + static_cast<uint64_t>(brow)) * C + hc];
-      if (et == 127 && mailbox && seq > p.nslots) fs_wait_acks(p, seq - p.nslots, "flow control");
-
-      // ---- forward partial: pre^T [128 hidden x 32 batch] over my K-slice ----
-      mbar_wait(bar_w, jl & 1);      // this step's W / x / small variables have landed
-      float fa[2][4][4];             // [m64 block][n8 group][element]
-#pragma unroll
-      for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) fa[mb][g][e] = 0.f;
-      if (nkc > 0) {
-        wgmma_fence();
-        for (int i = 0; i < nkc; ++i) {
-          const uint32_t a_addr = sbase + kOffW + i * kFsWChunk;
-          const uint32_t b_addr = sbase + kOffXk + i * kFsXChunk;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)   // K-major: advance 32 B inside the 128 B swizzle atom; SBO = 8 rows x 128 B
-#pragma unroll
-            for (int mb = 0; mb < 2; ++mb)
-              fs_mma_m64n32(fa[mb], make_wgmma_desc_sw128(a_addr + mb * 64 * 128 + j * 32),
-                            make_wgmma_desc_sw128(b_addr + j * 32), (i > 0 || j > 0) ? 1u : 0u);
+      // ---- row tiles of the step (the debug stamps below record the last tile's phases) ----
+      for (int t = 0; t < T; ++t) {
+        const bool last = t == T - 1;
+        // Multi-tile: the step number is re-read from ctl_next[jl & 1], where it stays until barrier #3 of the step —
+        // one register fewer across the tile loop, which keeps the kernel free of spills.
+        uint32_t step = cur, push_seq = seq;
+        if constexpr (kMulti) {
+          step = ctl_next[jl & 1];
+          push_seq = p.seq_base + step + 1u;
         }
-        wgmma_commit();
-        wgmma_wait0();
+        const int trow = 32 * t + brow;
+        const bool hrow_ok = trow < B;
+        float ylab = 0.f;
+        if (hrow_ok && hc_ok) ylab = p.y_base[(fs_row0(p, step) + static_cast<uint64_t>(trow)) * C + hc];
+        if (t == 0 && et == 127 && mailbox && push_seq > p.nslots) fs_wait_acks(p, push_seq - p.nslots, "flow control");
+
+        // ---- forward partial: pre^T [128 hidden x 32 batch] over my K-slice ----
+        if (t == 0) mbar_wait(bar_w, jl & 1);      // this step's W / x of tile 0 / small variables have landed
+        else mbar_wait(bar_xk, (jl * static_cast<uint32_t>(T - 1) + static_cast<uint32_t>(t - 1)) & 1u);   // x of tile t
+        float fa[2][4][4];             // [m64 block][n8 group][element]
 #pragma unroll
         for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
           for (int g = 0; g < 4; ++g)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) wgmma_reg_fence(fa[mb][g][e]);
-      }
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 1] = clock64();
-      // small variables out of the bulk-copied image, before barrier #1 lets warp 0 overwrite it with the next pull
-      const float bias = unit_ok ? raw_b[et] : 0.f;
-      float wl[kFsMaxC];
+            for (int e = 0; e < 4; ++e) fa[mb][g][e] = 0.f;
+        if (nkc > 0) {
+          wgmma_fence();
+          for (int i = 0; i < nkc; ++i) {
+            const uint32_t a_addr = sbase + kOffW + i * kFsWChunk;
+            const uint32_t b_addr = sbase + kOffXk + i * kFsXChunk;
 #pragma unroll
-      for (int c = 0; c < kFsMaxC; ++c) wl[c] = (unit_ok && c < C) ? raw_wl[c * H + et] : 0.f;
-      const float blast = hc_ok ? raw_bl[hc] : 0.f;
-      {
-        // reduce-scatter: batch columns 4d..4d+3 go to CTA d; element pair (e, e + 1) of n8 group g is columns
-        // 8 g + 2 fc, +1 of row fr + 8 (e >> 1): CTA 2 g + (fc >> 1), at column offset 2 (fc & 1) of its float4
+            for (int j = 0; j < 4; ++j)   // K-major: advance 32 B inside the 128 B swizzle atom; SBO = 8 rows x 128 B
 #pragma unroll
-        for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-#pragma unroll
-            for (int e = 0; e < 4; e += 2) {
-              const uint32_t row = static_cast<uint32_t>(mb * 64 + fr + 8 * (e >> 1));
-              const uint32_t d = static_cast<uint32_t>(2 * g + (fc >> 1));
-              const uint32_t off = kOffRed + ((rank * 128u + row) << 4) + static_cast<uint32_t>(fc & 1) * 8u;
-              st_shared_cluster_v2f32(mapa_shared_cluster(sbase + off, d), fa[mb][g][e], fa[mb][g][e + 1]);
-            }
-      }
-      cluster_sync_all();                                   // #1
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 2] = clock64();
-      float hv[kFsRows];
-      {
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int s = 0; s < kFusedCluster; ++s) {
-          const float4 t = *reinterpret_cast<const float4*>(red + (s * 128 + et) * 4);
-          acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
-        }
-        hv[0] = unit_ok ? fmaxf(acc.x + bias, 0.f) : 0.f;
-        hv[1] = unit_ok ? fmaxf(acc.y + bias, 0.f) : 0.f;
-        hv[2] = unit_ok ? fmaxf(acc.z + bias, 0.f) : 0.f;
-        hv[3] = unit_ok ? fmaxf(acc.w + bias, 0.f) : 0.f;
-      }
-      // ---- head on my 4 batch rows ----
-#pragma unroll
-      for (int i = 0; i < kFsRows; ++i) val[i * 128 + et] = hv[i];
-#pragma unroll
-      for (int c = 0; c < kFsMaxC; ++c) wls[c * kFsWlStride + et] = wl[c];
-      named_bar_sync(1, 128);
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 3] = clock64();
-      {
-        // logits: warp q = row q of this CTA, lane = (class, half of the hidden units)
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-        const float* hrow = val + q * 128 + kh * 64;
-        const float* wrow = wls + hc * kFsWlStride + kh * 64;
-#pragma unroll
-        for (int k = 0; k < 64; k += 4) {   // units >= H are zero in both operands
-          const float4 hvv = *reinterpret_cast<const float4*>(hrow + k);
-          const float4 wv = *reinterpret_cast<const float4*>(wrow + k);
-          a0 = fmaf(hvv.x, wv.x, a0); a1 = fmaf(hvv.y, wv.y, a1);
-          a2 = fmaf(hvv.z, wv.z, a2); a3 = fmaf(hvv.w, wv.w, a3);
-        }
-        float dot = (a0 + a1) + (a2 + a3);
-        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-        const float y = ylab;
-        const float z = hc_ok ? dot + blast : -INFINITY;
-        float zmax = z, ybest = hc_ok ? y : -INFINITY, ysum = y;
-#pragma unroll
-        for (int o = 16; o > 1; o >>= 1) {   // over the 16 classes (lane bit 0 is the k-half: both halves hold the same)
-          zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
-          ybest = fmaxf(ybest, __shfl_xor_sync(0xffffffffu, ybest, o));
-          ysum += __shfl_xor_sync(0xffffffffu, ysum, o);
-        }
-        int zarg = (hc_ok && z == zmax) ? hc : kFsMaxC, yarg = (hc_ok && y == ybest) ? hc : kFsMaxC;  // first maximum wins
-        const float e = hc_ok ? __expf(z - zmax) : 0.f;
-        float esum = e;
-#pragma unroll
-        for (int o = 16; o > 1; o >>= 1) {
-          zarg = min(zarg, __shfl_xor_sync(0xffffffffu, zarg, o));
-          yarg = min(yarg, __shfl_xor_sync(0xffffffffu, yarg, o));
-          esum += __shfl_xor_sync(0xffffffffu, esum, o);
-        }
-        const float pc = __fdividef(e, esum);
-        float dl = 0.f, lc = 0.f;
-        if (p.loss_kind == LOSS_BOOK) {
-          // L = -(1/(B*C)) sum y*log(clip(p,1e-10,1));  dL/dp = -y/(B*C*p) where the clip passes gradient (DS:52-53)
-          const float k = 1.f / (static_cast<float>(B) * static_cast<float>(C));
-          const bool pass = hc_ok && (pc >= 1e-10f) && (pc <= 1.0f);
-          const float g = pass ? (-k * y / pc) : 0.f;
-          float gp = g * pc;
-#pragma unroll
-          for (int o = 16; o > 1; o >>= 1) gp += __shfl_xor_sync(0xffffffffu, gp, o);
-          dl = pc * (g - gp);
-          lc = hc_ok ? -k * y * __logf(fminf(fmaxf(pc, 1e-10f), 1.0f)) : 0.f;
-        } else {
-          // L = (1/B) sum_b -sum_c y*log_softmax(z);  dz = (p*sum(y) - y)/B   (DS:35)
-          const float k = 1.f / static_cast<float>(B);
-          dl = k * (pc * ysum - y);
-          lc = hc_ok ? -k * y * (z - (zmax + __logf(esum))) : 0.f;
-        }
-        if (kh == 0) dls[q * kFsMaxC + hc] = (hrow_ok && hc_ok) ? dl : 0.f;
-        float loss_part = (hrow_ok && kh == 0) ? lc : 0.f;
-        float corr_part = (hrow_ok && lane == 0 && zarg == yarg) ? 1.f : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) loss_part += __shfl_xor_sync(0xffffffffu, loss_part, o);
-        corr_part = __shfl_sync(0xffffffffu, corr_part, 0);
-        if (lane == 0) { redw[q] = loss_part; redw[4 + q] = corr_part; }
-      }
-      named_bar_sync(1, 128);
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 4] = clock64();
-      // ---- gradients of my rows; thread -> hidden unit et ----
-      float dw[kFsPart];
-#pragma unroll
-      for (int c = 0; c < kFsPart; ++c) dw[c] = 0.f;
-      float dp[kFsRows];
-      float dbh = 0.f;
-#pragma unroll
-      for (int i = 0; i < kFsRows; ++i) {
-        float dh = 0.f;
-#pragma unroll
-        for (int c4 = 0; c4 < kFsMaxC / 4; ++c4) {
-          const float4 d = *reinterpret_cast<const float4*>(dls + i * kFsMaxC + 4 * c4);   // broadcast reads
-          dh = fmaf(d.x, wl[4 * c4 + 0], dh); dh = fmaf(d.y, wl[4 * c4 + 1], dh);
-          dh = fmaf(d.z, wl[4 * c4 + 2], dh); dh = fmaf(d.w, wl[4 * c4 + 3], dh);
-          if (4 * c4 + 0 < kFsPart - 1) dw[4 * c4 + 0] = fmaf(d.x, hv[i], dw[4 * c4 + 0]);
-          if (4 * c4 + 1 < kFsPart - 1) dw[4 * c4 + 1] = fmaf(d.y, hv[i], dw[4 * c4 + 1]);
-          if (4 * c4 + 2 < kFsPart - 1) dw[4 * c4 + 2] = fmaf(d.z, hv[i], dw[4 * c4 + 2]);
-          if (4 * c4 + 3 < kFsPart - 1) dw[4 * c4 + 3] = fmaf(d.w, hv[i], dw[4 * c4 + 3]);
-        }
-        dp[i] = hv[i] > 0.f ? dh : 0.f;       // rows >= B carry dlogits == 0 -> dp == 0
-        dbh += dp[i];
-      }
-      dw[kFsPart - 1] = dbh;
-      {
-        // all-gather of dpre^T: row et (128 B = 32 batch values), my 16-byte chunk is number `rank`; K-major
-        // SWIZZLE_128B: chunk j of row r sits at r * 128 + ((j ^ (r & 7)) << 4)
-        const uint32_t a_off = kOffA + static_cast<uint32_t>(et) * 128u + ((rank ^ (static_cast<uint32_t>(et) & 7u)) << 4);
-#pragma unroll
-        for (uint32_t d = 0; d < kFusedCluster; ++d)
-          st_shared_cluster_v4f32(mapa_shared_cluster(sbase + a_off, d), dp[0], dp[1], dp[2], dp[3]);
-        // reduce-scatter of the small-gradient partials: hidden units [16 d, 16 d + 16) are summed by CTA d
-        const uint32_t sg_off = kOffSg + ((rank * 16u + (static_cast<uint32_t>(et) & 15u)) * kFsPart) * 4u;
-        const uint32_t sg_dst = mapa_shared_cluster(sbase + sg_off, static_cast<uint32_t>(et) >> 4);
-        st_shared_cluster_v4f32(sg_dst, dw[0], dw[1], dw[2], dw[3]);
-        st_shared_cluster_v4f32(sg_dst + 16u, dw[4], dw[5], dw[6], dw[7]);
-        st_shared_cluster_v4f32(sg_dst + 32u, dw[8], dw[9], dw[10], dw[11]);
-        if (et < kFsMaxC) {
-          float sdl = 0.f;
-#pragma unroll
-          for (int i = 0; i < kFsRows; ++i) sdl += dls[i * kFsMaxC + et];
-          st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffDbl + (rank * kFsMaxC + et) * 4u, 0), sdl);
-        }
-        if (et == 0) {
-          st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffScal + (rank * 2u) * 4u, 0),
-                                (redw[0] + redw[1]) + (redw[2] + redw[3]));
-          st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffScal + (rank * 2u + 1u) * 4u, 0),
-                                (redw[4] + redw[5]) + (redw[6] + redw[7]));
-        }
-      }
-      fence_proxy_async_smem_cluster();
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 5] = clock64();
-      cluster_sync_all();                                   // #2
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 6] = clock64();
-
-      // ---- small gradients: sum the 8 sources for my 16 hidden units and push them ----
-      {
-        const FsPush pw_l = fs_resolve(p.shard[p.shard_wl].push, seq);
-        const FsPush pb_h = fs_resolve(p.shard[p.shard_bh].push, seq);
-        const int u = et & 15, vg = et >> 4;   // values vg (0..7) and vg + 8 (8..11) of unit u
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int s = 0; s < kFusedCluster; ++s) {
-          s0 += sg[(s * 16 + u) * kFsPart + vg];
-          if (vg < 4) s1 += sg[(s * 16 + u) * kFsPart + vg + 8];
-        }
-        const int unit = static_cast<int>(rank) * 16 + u;
-        if (unit < H) {
-          if (vg < C) fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg) * H + unit, s0);
-          if (vg < 3 && vg + 8 < C)
-            fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg + 8) * H + unit, s1);
-          if (vg == 3) fs_push_value(p.shard[p.shard_bh].push, pb_h.base + p.off_bh + unit, s1);
-        }
-        if (rank == 0 && et < C) {
-          const FsPush pb_l = fs_resolve(p.shard[p.shard_bl].push, seq);
-          float s = 0.f;
-#pragma unroll
-          for (int src = 0; src < kFusedCluster; ++src) s += dbl[src * kFsMaxC + et];
-          fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, s);
-        }
-      }
-
-      // ---- dW^T tile of my K-slice: wgmma -> registers -> swizzled staging tile; warp 4 TMA-stores it (the push) ----
-      fence_proxy_async_smem_cta();   // generic-proxy (DSMEM) writes of dpre^T -> tensor-core reads
-      mbar_wait(bar_xmn, jl & 1);
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 7] = clock64();
-      if (nkc > 0) {
-        // D[feature f][hidden h] = sum_b x[b][f] dpre^T[h][b]: M = my features (m64 blocks), N = 128 hidden units,
-        // K = 32 batch rows. A = x^T from registers, read out of the K-major x tile ([b][f], 128-byte swizzled);
-        // B = dpre^T, K-major in shared memory. Rows of a block beyond my slice compute garbage and are not stored.
-        const int nmb = (nkc * 32 + 63) >> 6;
-        const uint8_t* xs = smem + kOffXmn;
-        float da[2][16][4];
-#pragma unroll
-        for (int mb = 0; mb < 2; ++mb) {
-          if (mb < nmb) {
-            uint32_t a[4][4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int f0 = mb * 64 + fr, b0 = 8 * j + fc;
-              auto xat = [&](int f, int b) -> uint32_t {   // x[b][f]: chunk f / 32 of the x tile
-                const uint32_t o = static_cast<uint32_t>(f >> 5) * kFsXChunk + sw128_offset(b, f & 31, 4);
-                return (f >> 5) < nkc ? *reinterpret_cast<const uint32_t*>(xs + o) : 0u;
-              };
-              a[j][0] = xat(f0, b0);
-              a[j][1] = xat(f0 + 8, b0);
-              a[j][2] = xat(f0, b0 + 4);
-              a[j][3] = xat(f0 + 8, b0 + 4);
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              fs_mma_m64n128(da[mb], a[j], make_wgmma_desc_sw128(sbase + kOffA + j * 32), j > 0 ? 1u : 0u);
-            wgmma_commit();
-            wgmma_wait0();
-#pragma unroll
-            for (int g = 0; g < 16; ++g)
-#pragma unroll
-              for (int e = 0; e < 4; ++e) wgmma_reg_fence(da[mb][g][e]);
+              for (int mb = 0; mb < 2; ++mb)
+                fs_mma_m64n32(fa[mb], make_wgmma_desc_sw128(a_addr + mb * 64 * 128 + j * 32),
+                              make_wgmma_desc_sw128(b_addr + j * 32), (i > 0 || j > 0) ? 1u : 0u);
           }
+          wgmma_commit();
+          wgmma_wait0();
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) wgmma_reg_fence(fa[mb][g][e]);
         }
-        const PushTarget& tw = p.shard[sl.shard].push;
-        const float sc = tw.mode == PUSH_ATOMIC ? tw.scale : 1.f;
-        // staging tile of chunk i: [128 hidden rows][32 features] fp32, SWIZZLE_128B (the TMA store's box)
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 1] = clock64();
+        // small variables out of the bulk-copied image, before barrier #1 lets warp 0 overwrite it with the next pull
+        const float bias = unit_ok ? raw_b[et] : 0.f;
+        float wl[kFsMaxC];
 #pragma unroll
-        for (int mb = 0; mb < 2; ++mb) {
-          if (mb < nmb) {
+        for (int c = 0; c < kFsMaxC; ++c) wl[c] = (unit_ok && c < C) ? raw_wl[c * H + et] : 0.f;
+        const float blast = hc_ok ? raw_bl[hc] : 0.f;
+        {
+          // reduce-scatter: batch columns 4d..4d+3 go to CTA d; element pair (e, e + 1) of n8 group g is columns
+          // 8 g + 2 fc, +1 of row fr + 8 (e >> 1): CTA 2 g + (fc >> 1), at column offset 2 (fc & 1) of its float4
 #pragma unroll
-            for (int g = 0; g < 16; ++g)
+          for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int f = mb * 64 + fr + 8 * (e >> 1);
-                const int h = 8 * g + 2 * fc + (e & 1);
-                if ((f >> 5) < nkc)
-                  *reinterpret_cast<float*>(smem + kOffStage + (f >> 5) * kFsWChunk + sw128_offset(h, f & 31, 4)) =
-                      sc * da[mb][g][e];
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int e = 0; e < 4; e += 2) {
+                const uint32_t row = static_cast<uint32_t>(mb * 64 + fr + 8 * (e >> 1));
+                const uint32_t d = static_cast<uint32_t>(2 * g + (fc >> 1));
+                const uint32_t off = kOffRed + ((rank * 128u + row) << 4) + static_cast<uint32_t>(fc & 1) * 8u;
+                st_shared_cluster_v2f32(mapa_shared_cluster(sbase + off, d), fa[mb][g][e], fa[mb][g][e + 1]);
               }
+        }
+        cluster_sync_all();                                   // #1
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 2] = clock64();
+        float hv[kFsRows];
+        {
+          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int s = 0; s < kFusedCluster; ++s) {
+            const float4 t = *reinterpret_cast<const float4*>(red + (s * 128 + et) * 4);
+            acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
+          }
+          hv[0] = unit_ok ? fmaxf(acc.x + bias, 0.f) : 0.f;
+          hv[1] = unit_ok ? fmaxf(acc.y + bias, 0.f) : 0.f;
+          hv[2] = unit_ok ? fmaxf(acc.z + bias, 0.f) : 0.f;
+          hv[3] = unit_ok ? fmaxf(acc.w + bias, 0.f) : 0.f;
+        }
+        // ---- head on my 4 batch rows ----
+#pragma unroll
+        for (int i = 0; i < kFsRows; ++i) val[i * 128 + et] = hv[i];
+#pragma unroll
+        for (int c = 0; c < kFsMaxC; ++c) wls[c * kFsWlStride + et] = wl[c];
+        named_bar_sync(1, 128);
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 3] = clock64();
+        {
+          // logits: warp q = row q of this CTA, lane = (class, half of the hidden units)
+          float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+          const float* hrow = val + q * 128 + kh * 64;
+          const float* wrow = wls + hc * kFsWlStride + kh * 64;
+#pragma unroll
+          for (int k = 0; k < 64; k += 4) {   // units >= H are zero in both operands
+            const float4 hvv = *reinterpret_cast<const float4*>(hrow + k);
+            const float4 wv = *reinterpret_cast<const float4*>(wrow + k);
+            a0 = fmaf(hvv.x, wv.x, a0); a1 = fmaf(hvv.y, wv.y, a1);
+            a2 = fmaf(hvv.z, wv.z, a2); a3 = fmaf(hvv.w, wv.w, a3);
+          }
+          float dot = (a0 + a1) + (a2 + a3);
+          dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+          const float y = ylab;
+          const float z = hc_ok ? dot + blast : -INFINITY;
+          float zmax = z, ybest = hc_ok ? y : -INFINITY, ysum = y;
+#pragma unroll
+          for (int o = 16; o > 1; o >>= 1) {   // over the 16 classes (lane bit 0 is the k-half: both halves hold the same)
+            zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
+            ybest = fmaxf(ybest, __shfl_xor_sync(0xffffffffu, ybest, o));
+            ysum += __shfl_xor_sync(0xffffffffu, ysum, o);
+          }
+          int zarg = (hc_ok && z == zmax) ? hc : kFsMaxC, yarg = (hc_ok && y == ybest) ? hc : kFsMaxC;  // first maximum wins
+          const float e = hc_ok ? __expf(z - zmax) : 0.f;
+          float esum = e;
+#pragma unroll
+          for (int o = 16; o > 1; o >>= 1) {
+            zarg = min(zarg, __shfl_xor_sync(0xffffffffu, zarg, o));
+            yarg = min(yarg, __shfl_xor_sync(0xffffffffu, yarg, o));
+            esum += __shfl_xor_sync(0xffffffffu, esum, o);
+          }
+          const float pc = __fdividef(e, esum);
+          float dl = 0.f, lc = 0.f;
+          if (p.loss_kind == LOSS_BOOK) {
+            // L = -(1/(B*C)) sum y*log(clip(p,1e-10,1));  dL/dp = -y/(B*C*p) where the clip passes gradient (DS:52-53)
+            const float k = 1.f / (static_cast<float>(B) * static_cast<float>(C));
+            const bool pass = hc_ok && (pc >= 1e-10f) && (pc <= 1.0f);
+            const float g = pass ? (-k * y / pc) : 0.f;
+            float gp = g * pc;
+#pragma unroll
+            for (int o = 16; o > 1; o >>= 1) gp += __shfl_xor_sync(0xffffffffu, gp, o);
+            dl = pc * (g - gp);
+            lc = hc_ok ? -k * y * __logf(fminf(fmaxf(pc, 1e-10f), 1.0f)) : 0.f;
+          } else {
+            // L = (1/B) sum_b -sum_c y*log_softmax(z);  dz = (p*sum(y) - y)/B   (DS:35)
+            const float k = 1.f / static_cast<float>(B);
+            dl = k * (pc * ysum - y);
+            lc = hc_ok ? -k * y * (z - (zmax + __logf(esum))) : 0.f;
+          }
+          if (kh == 0) dls[q * kFsMaxC + hc] = (hrow_ok && hc_ok) ? dl : 0.f;
+          float loss_part = (hrow_ok && kh == 0) ? lc : 0.f;
+          float corr_part = (hrow_ok && lane == 0 && zarg == yarg) ? 1.f : 0.f;
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) loss_part += __shfl_xor_sync(0xffffffffu, loss_part, o);
+          corr_part = __shfl_sync(0xffffffffu, corr_part, 0);
+          if (lane == 0) { redw[q] = loss_part; redw[4 + q] = corr_part; }
+        }
+        named_bar_sync(1, 128);
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 4] = clock64();
+        // ---- gradients of my rows; thread -> hidden unit et ----
+        float dw[kFsPart];
+#pragma unroll
+        for (int c = 0; c < kFsPart; ++c) dw[c] = 0.f;
+        float dp[kFsRows];
+        float dbh = 0.f;
+#pragma unroll
+        for (int i = 0; i < kFsRows; ++i) {
+          float dh = 0.f;
+#pragma unroll
+          for (int c4 = 0; c4 < kFsMaxC / 4; ++c4) {
+            const float4 d = *reinterpret_cast<const float4*>(dls + i * kFsMaxC + 4 * c4);   // broadcast reads
+            dh = fmaf(d.x, wl[4 * c4 + 0], dh); dh = fmaf(d.y, wl[4 * c4 + 1], dh);
+            dh = fmaf(d.z, wl[4 * c4 + 2], dh); dh = fmaf(d.w, wl[4 * c4 + 3], dh);
+            if (4 * c4 + 0 < kFsPart - 1) dw[4 * c4 + 0] = fmaf(d.x, hv[i], dw[4 * c4 + 0]);
+            if (4 * c4 + 1 < kFsPart - 1) dw[4 * c4 + 1] = fmaf(d.y, hv[i], dw[4 * c4 + 1]);
+            if (4 * c4 + 2 < kFsPart - 1) dw[4 * c4 + 2] = fmaf(d.z, hv[i], dw[4 * c4 + 2]);
+            if (4 * c4 + 3 < kFsPart - 1) dw[4 * c4 + 3] = fmaf(d.w, hv[i], dw[4 * c4 + 3]);
+          }
+          dp[i] = hv[i] > 0.f ? dh : 0.f;       // rows >= B carry dlogits == 0 -> dp == 0
+          dbh += dp[i];
+        }
+        dw[kFsPart - 1] = dbh;
+        // Multi-tile: the small gradients, loss and correct count add up over the row tiles in shared memory (the
+        // same thread owns the same words in every tile) and are reduce-scattered once, in the last tile.
+        auto carry = [&](float v, float* run) -> float {
+          if (t > 0) v += *run;
+          if (!last) *run = v;
+          return v;
+        };
+        if constexpr (kMulti) {
+#pragma unroll
+          for (int c = 0; c < kFsPart; ++c) dw[c] = carry(dw[c], acc + c * 128 + et);
+        }
+        {
+          // all-gather of dpre^T: row et (128 B = 32 batch values), my 16-byte chunk is number `rank`; K-major
+          // SWIZZLE_128B: chunk j of row r sits at r * 128 + ((j ^ (r & 7)) << 4)
+          const uint32_t a_off = kOffA + static_cast<uint32_t>(et) * 128u + ((rank ^ (static_cast<uint32_t>(et) & 7u)) << 4);
+#pragma unroll
+          for (uint32_t d = 0; d < kFusedCluster; ++d)
+            st_shared_cluster_v4f32(mapa_shared_cluster(sbase + a_off, d), dp[0], dp[1], dp[2], dp[3]);
+          if (last) {
+            // reduce-scatter of the small-gradient partials: hidden units [16 d, 16 d + 16) are summed by CTA d
+            const uint32_t sg_off = kOffSg + ((rank * 16u + (static_cast<uint32_t>(et) & 15u)) * kFsPart) * 4u;
+            const uint32_t sg_dst = mapa_shared_cluster(sbase + sg_off, static_cast<uint32_t>(et) >> 4);
+            st_shared_cluster_v4f32(sg_dst, dw[0], dw[1], dw[2], dw[3]);
+            st_shared_cluster_v4f32(sg_dst + 16u, dw[4], dw[5], dw[6], dw[7]);
+            st_shared_cluster_v4f32(sg_dst + 32u, dw[8], dw[9], dw[10], dw[11]);
+          }
+          if (et < kFsMaxC) {
+            float sdl = 0.f;
+#pragma unroll
+            for (int i = 0; i < kFsRows; ++i) sdl += dls[i * kFsMaxC + et];
+            if constexpr (kMulti) sdl = carry(sdl, acc_dbl + et);
+            if (last) st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffDbl + (rank * kFsMaxC + et) * 4u, 0), sdl);
+          }
+          if (et == 0) {
+            float ls = (redw[0] + redw[1]) + (redw[2] + redw[3]);
+            if constexpr (kMulti) ls = carry(ls, acc_scal);
+            if (last) st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffScal + (rank * 2u) * 4u, 0), ls);
+            float cs = (redw[4] + redw[5]) + (redw[6] + redw[7]);
+            if constexpr (kMulti) cs = carry(cs, acc_scal + 1);
+            if (last) st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffScal + (rank * 2u + 1u) * 4u, 0), cs);
           }
         }
+        fence_proxy_async_smem_cluster();
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 5] = clock64();
+        cluster_sync_all();                                   // #2
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 6] = clock64();
+
+        // ---- small gradients: sum the 8 sources for my 16 hidden units and push them ----
+        if (last) {
+          const FsPush pw_l = fs_resolve(p.shard[p.shard_wl].push, push_seq);
+          const FsPush pb_h = fs_resolve(p.shard[p.shard_bh].push, push_seq);
+          const int u = et & 15, vg = et >> 4;   // values vg (0..7) and vg + 8 (8..11) of unit u
+          float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+          for (int s = 0; s < kFusedCluster; ++s) {
+            s0 += sg[(s * 16 + u) * kFsPart + vg];
+            if (vg < 4) s1 += sg[(s * 16 + u) * kFsPart + vg + 8];
+          }
+          const int unit = static_cast<int>(rank) * 16 + u;
+          if (unit < H) {
+            if (vg < C) fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg) * H + unit, s0);
+            if (vg < 3 && vg + 8 < C)
+              fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg + 8) * H + unit, s1);
+            if (vg == 3) fs_push_value(p.shard[p.shard_bh].push, pb_h.base + p.off_bh + unit, s1);
+          }
+          if (rank == 0 && et < C) {
+            const FsPush pb_l = fs_resolve(p.shard[p.shard_bl].push, push_seq);
+            float s = 0.f;
+#pragma unroll
+            for (int src = 0; src < kFusedCluster; ++src) s += dbl[src * kFsMaxC + et];
+            fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, s);
+          }
+        }
+
+        // ---- dW^T tile of my K-slice: wgmma -> registers -> swizzled staging tile; warp 4 TMA-stores it (the push) ----
+        fence_proxy_async_smem_cta();   // generic-proxy (DSMEM) writes of dpre^T -> tensor-core reads
+        mbar_wait(bar_xmn, (jl * static_cast<uint32_t>(T) + static_cast<uint32_t>(t)) & 1u);
+        if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 7] = clock64();
+        if (nkc > 0) {
+          // D[feature f][hidden h] = sum_b x[b][f] dpre^T[h][b]: M = my features (m64 blocks), N = 128 hidden units,
+          // K = 32 batch rows. A = x^T from registers, read out of the K-major x tile ([b][f], 128-byte swizzled);
+          // B = dpre^T, K-major in shared memory. Rows of a block beyond my slice compute garbage and are not stored.
+          const int nmb = (nkc * 32 + 63) >> 6;
+          const uint8_t* xs = smem + kOffXmn;
+          float da[2][16][4];
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb) {
+            if (mb < nmb) {
+              uint32_t a[4][4];
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int f0 = mb * 64 + fr, b0 = 8 * j + fc;
+                auto xat = [&](int f, int b) -> uint32_t {   // x[b][f]: chunk f / 32 of the x tile
+                  const uint32_t o = static_cast<uint32_t>(f >> 5) * kFsXChunk + sw128_offset(b, f & 31, 4);
+                  return (f >> 5) < nkc ? *reinterpret_cast<const uint32_t*>(xs + o) : 0u;
+                };
+                a[j][0] = xat(f0, b0);
+                a[j][1] = xat(f0 + 8, b0);
+                a[j][2] = xat(f0, b0 + 4);
+                a[j][3] = xat(f0 + 8, b0 + 4);
+              }
+              wgmma_fence();
+#pragma unroll
+              for (int j = 0; j < 4; ++j)
+                fs_mma_m64n128(da[mb], a[j], make_wgmma_desc_sw128(sbase + kOffA + j * 32), j > 0 ? 1u : 0u);
+              wgmma_commit();
+              wgmma_wait0();
+#pragma unroll
+              for (int g = 0; g < 16; ++g)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) wgmma_reg_fence(da[mb][g][e]);
+            }
+          }
+          if constexpr (kMulti) {
+            if (!last) mbar_arrive(bar_xmn_empty);   // Xmn is read: warp 4 may load the next tile's x into it
+          }
+          const PushTarget& tw = p.shard[sl.shard].push;
+          const float sc = tw.mode == PUSH_ATOMIC ? tw.scale : 1.f;
+          // staging tile of chunk i: [128 hidden rows][32 features] fp32, SWIZZLE_128B (the TMA store's box); row
+          // tiles after the first add into it (every thread owns the same elements in every tile)
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb) {
+            if (mb < nmb) {
+#pragma unroll
+              for (int g = 0; g < 16; ++g)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const int f = mb * 64 + fr + 8 * (e >> 1);
+                  const int h = 8 * g + 2 * fc + (e & 1);
+                  if ((f >> 5) < nkc) {
+                    float* st = reinterpret_cast<float*>(smem + kOffStage + (f >> 5) * kFsWChunk + sw128_offset(h, f & 31, 4));
+                    if (kMulti && t > 0) *st += sc * da[mb][g][e];
+                    else *st = sc * da[mb][g][e];
+                  }
+                }
+            }
+          }
+        }
+        if (last) {
+          fence_proxy_async_smem_cta();  // staging writes -> visible to the TMA engine (shared memory only: does not
+                                         // wait for the small-gradient peer stores issued above)
+          named_bar_arrive(2, 160);      // hand the tile to warp 4 (non-blocking) ...
+          if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 8] = clock64();
+          cluster_sync_all();            // #3 ... and go on to the next step
+          if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 9] = clock64();
+        }
       }
-      fence_proxy_async_smem_cta();    // staging writes -> visible to the TMA engine (shared memory only: does not
-                                       // wait for the small-gradient peer stores issued above)
-      named_bar_arrive(2, 160);        // hand the tile to warp 4 (non-blocking) ...
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 8] = clock64();
-      cluster_sync_all();              // #3 ... and go on to the next step
-      if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 9] = clock64();
       cur = ctl_next[(jl + 1) & 1];
     }
   }
@@ -691,51 +779,58 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-cudaError_t prepare_fused_kernel() {
-  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(kFsSmemBytes));
+template <int kMaxTiles>
+static cudaError_t prepare_fused_instance() {
+  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(fs_smem_bytes<kMaxTiles>()));
   if (e != cudaSuccess) return e;
   cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, fused_step_kernel);   // force-load (see preload_ps_kernels)
+  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles>);   // force-load (see preload_ps_kernels)
 }
 
-size_t fused_smem_bytes() { return kFsSmemBytes; }
+cudaError_t prepare_fused_kernel() {
+  const cudaError_t e = prepare_fused_instance<1>();
+  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles>();
+}
 
-cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
-  if (lanes < 1 || p.B < 1 || p.B > 32 || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 || (p.I & 3) ||
-      p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1)
-    return cudaErrorInvalidValue;
-  for (int r = 0; r < kFusedCluster; ++r)
-    if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
+static bool fused_multi_tile(int B) { return B > 32; }
+
+size_t fused_smem_bytes(int B) { return fused_multi_tile(B) ? fs_smem_bytes<kFsMaxTiles>() : fs_smem_bytes<1>(); }
+
+// One launch config for both instantiations: `lanes` clusters of 8 CTAs.
+static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t stream, cudaLaunchAttribute* attr) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(kFusedCluster, lanes, 1);
   cfg.blockDim = dim3(kFsThreads);
-  cfg.dynamicSmemBytes = kFsSmemBytes;
+  cfg.dynamicSmemBytes = fused_smem_bytes(B);
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = kFusedCluster;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, fused_step_kernel, maps, p);
+  return cfg;
 }
 
-// How many clusters of the fused kernel can be co-resident on the device (upper bound for `lanes`).
-cudaError_t fused_max_lanes(int* out) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(kFusedCluster, 1, 1);
-  cfg.blockDim = dim3(kFsThreads);
-  cfg.dynamicSmemBytes = kFsSmemBytes;
+cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
+  if (lanes < 1 || p.B < 1 || p.B > 32 * kFsMaxTiles || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 ||
+      (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1)
+    return cudaErrorInvalidValue;
+  for (int r = 0; r < kFusedCluster; ++r)
+    if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kFusedCluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel, &cfg);
+  const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
+  if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles>, maps, p);
+  return cudaLaunchKernelEx(&cfg, fused_step_kernel<1>, maps, p);
+}
+
+// How many clusters of the fused kernel that runs batch B can be co-resident on the device (upper bound for `lanes`).
+cudaError_t fused_max_lanes(int B, int* out) {
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
+  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles>, &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1>, &cfg);
 }
 
 }  // namespace dm

@@ -191,7 +191,7 @@ struct PsServeParams {
 
 // ------------------------------------------------------------------------------------------------
 // Fused worker step (fused_step_sm90.cu): one 8-CTA thread-block cluster runs whole training steps of the
-// 784-H-10 MLP (H <= 128, batch <= 32) back to back inside one launch: TMA pull of its K-slice of W from the ps
+// 784-H-10 MLP (H <= 128, batch <= 256) back to back inside one launch: TMA pull of its K-slice of W from the ps
 // shard, wgmma forward (split-K over the cluster, DSMEM reduce-scatter), classifier head, DSMEM all-gather of
 // the pre-activation gradient, wgmma dW of its own column slice, gradient push + flag. `lanes` clusters of one
 // launch work on different steps concurrently.
@@ -227,7 +227,8 @@ struct FusedParams {
   int shard_bh, shard_wl, shard_bl;          // FusedParams::shard index owning hid_b / sm_w / sm_b
   int flag_bh, flag_wl, flag_bl;             // their flag indices on those shards
   uint64_t off_bh, off_wl, off_bl;           // element offsets inside those shards' arenas
-  // inputs: batch of step s = rows [(row_start + s * row_stride) % row_wrap, +32) of the x / y matrices
+  // inputs: batch of step s = rows [(row_start + s * row_stride) % row_wrap, +B) of the x / y matrices (x is read in
+  // whole 32-row tiles: the x map must cover round_up(B, 32) rows from there)
   const float* y_base;
   uint64_t row_start, row_stride, row_wrap;
   // bookkeeping

@@ -51,8 +51,9 @@ class EngineConfig:
     sharding: str = "round_robin"    # "round_robin" (reference parity) | "byte_balanced" | "row_split" (the hidden
                                      # weight is split along its input features over every ps task; fused engine)
     engine: str = "auto"             # "fused": one persistent kernel runs whole steps (784-H-10 models, H <= 128,
-                                     # batch <= 32, fp32) | "graph": per-layer kernels chained in a CUDA graph (any
-                                     # model / dtype) | "auto": fused when the model is eligible
+                                     # batch <= 256, fp32) | "graph": per-layer kernels chained in a CUDA graph (any
+                                     # model / dtype) | "auto": fused when the model is eligible and the batch is
+                                     # <= 32 rows (any eligible batch with sharding "row_split")
     strict_steps: bool = False       # fused engine and cpu backend: a lane pulls the weights of its next step only
                                      # after the ps has acknowledged its previous push (the reference's read-your-writes
                                      # order inside one worker); default: the pull overlaps the previous step's backward
@@ -132,14 +133,16 @@ class EngineConfig:
     def resolve_engine(self, spec, batch_size: int) -> str:
         """Which step engine (and therefore which shard tiling) ps and worker tasks use. Both sides evaluate the
         same rule from the same flags; the rendezvous descriptor check catches a mismatch."""
-        from .sharding import fused_eligible
+        from .sharding import FUSED_AUTO_MAX_BATCH, FUSED_MAX_BATCH, fused_eligible
 
         ok = fused_eligible(spec, batch_size, self.dtype)
         if self.engine == "fused" and not ok:
-            raise ValueError("engine 'fused' needs one hidden layer of <= 128 units, <= 11 classes, batch <= 32, fp32 "
-                             "and 8 <= ceil(in_features / 32) <= 32")
+            raise ValueError(f"engine 'fused' needs one hidden layer of <= 128 units, <= 11 classes, "
+                             f"batch <= {FUSED_MAX_BATCH}, fp32 and 8 <= ceil(in_features / 32) <= 32")
         if self.engine == "graph" or not ok:
             if self.sharding == "row_split":
                 raise ValueError("sharding 'row_split' needs the fused engine")
             return "graph"
+        if self.engine == "auto" and batch_size > FUSED_AUTO_MAX_BATCH and self.sharding != "row_split":
+            return "graph"   # host-fed training is not faster on the fused engine there (sharding.FUSED_AUTO_MAX_BATCH)
         return "fused"

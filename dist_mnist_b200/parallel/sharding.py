@@ -33,7 +33,12 @@ from ..models.mlp import MLPSpec, VarSpec
 FUSED_CLUSTER = 8     # CTAs per cluster of the fused step kernel == column slices of the hidden weight
 FUSED_MAX_CHUNKS = 4  # 32-feature k-chunks per CTA
 FUSED_MAX_HIDDEN = 128
-FUSED_MAX_BATCH = 32
+FUSED_MAX_BATCH = 256   # ceil(B / 32) row tiles of 32 rows per step (`engine="fused"`)
+# `engine="auto"` picks the fused engine only up to one row tile (or when `row_split` needs it). Above 32 rows the fused
+# kernel is 2.1-3.2x the graph engine's device-timed steps/s, but host-fed training through `Worker.run_steps` is not
+# faster: at a batch that is not a multiple of 32 the fused executor row-gathers every batch (batch 100 on an H100
+# 80GB HBM3 at 400 W: 5-8 k steps/s fused, 47-70 k graph), and at 256 it is 16-18 k against 21-29 k.
+FUSED_AUTO_MAX_BATCH = 32
 FUSED_MAX_CLASSES = 11
 PS_ROW_BLOCKS = 4     # fused tiling: ps items (CTAs) per pushed column slice
 TILE_M = 128          # rows of a dW tile / width of a bias or head slice
@@ -186,7 +191,7 @@ def _items_for(role: str, offset: int, rows: int, cols: int, ld: int, dw_tile_n:
 
 def fused_eligible(spec: MLPSpec, batch_size: int, dtype: str = "fp32") -> bool:
     """Can the fused step kernel (csrc/fused_step_sm90.cu) run this model? One hidden layer of <= 128 units, <= 11
-    classes, batch <= 32, fp32 storage (tf32 MMA), 8 <= ceil(in / 32) <= 32 and in % 4 == 0."""
+    classes, batch <= FUSED_MAX_BATCH, fp32 storage (tf32 MMA), 8 <= ceil(in / 32) <= 32 and in % 4 == 0."""
     sizes = spec.layer_sizes
     if len(sizes) != 2 or dtype != "fp32":
         return False
@@ -214,7 +219,7 @@ def build_layout(spec: MLPSpec, num_ps: int, strategy: str = "round_robin", dw_t
         raise ValueError(f"unknown engine {engine!r}")
     if strategy == "row_split" and engine != "fused":
         raise ValueError("sharding 'row_split' splits the hidden weight along the K-slices of the fused step kernel; "
-                         "it needs the fused engine (one hidden layer <= 128 units, batch <= 32, fp32)")
+                         f"it needs the fused engine (one hidden layer <= 128 units, batch <= {FUSED_MAX_BATCH}, fp32)")
     placement = place_variables(spec, num_ps, strategy)
     shards = [ShardLayout(ps=k) for k in range(num_ps)]
     shards[placement[GLOBAL_STEP]].owns_global_step = True

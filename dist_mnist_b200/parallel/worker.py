@@ -8,8 +8,9 @@ Reference parity (`/root/reference/distributed_server-basic.py`):
                 bumps `global_step`; the worker gets `loss` and `global_step` back. No locks, no barriers.
 
 GPU backend, two step engines (`EngineConfig.engine`, resolved by `EngineConfig.resolve_engine`):
-  * "fused" (784-H-10 models, H <= 128, batch <= 32, fp32 — the reference's live configuration): whole steps run
-    inside one persistent kernel (csrc/fused_step_sm90.cu): an 8-CTA cluster pulls its K-slices of W from the ps
+  * "fused" (784-H-10 models, H <= 128, batch <= 256, fp32 — the reference's live configuration): whole steps run
+    inside one persistent kernel (csrc/fused_step_sm90.cu), a batch as ceil(B / 32) row tiles of 32 rows that share
+    one pull of W: an 8-CTA cluster pulls its K-slices of W from the ps
     shard(s) with TMA over NVLink, wgmma forward with a DSMEM reduce-scatter, head, DSMEM all-gather, wgmma dW
     whose epilogue pushes into the ps mailbox; `cfg.lanes` clusters work on different steps concurrently. The
     native executor (csrc/fused_exec.cu) feeds it chunk by chunk: gather pool -> pinned staging -> H2D -> one launch.
@@ -125,7 +126,7 @@ class Worker:
         self.layout = layout or build_layout(spec, cluster.num_ps, cfg.sharding, dw_tile_n_for(cfg.dtype),
                                              engine=self.engine, ps_row_blocks=cfg.ps_row_blocks)
         if self.engine == "fused":
-            self.B_pad = N.FUSED_ROWS_PER_SLOT   # the fused kernel always works on 32-row tiles (rows >= batch masked)
+            self.B_pad = _round_up(batch_size, N.FUSED_ROW_TILE)   # whole 32-row tiles (rows >= batch masked)
         self.rdv = rdv or Rendezvous(cluster, "worker", task_index)
         self.lib = N.lib()
         self.is_chief = task_index == 0  # DS:108
@@ -625,7 +626,7 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
-        N.check(self.lib.dm_fused_max_lanes(self.device, C.byref(max_lanes)), "fused occupancy")
+        N.check(self.lib.dm_fused_max_lanes(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
         lanes = max(1, min(cfg.lanes, max_lanes.value if max_lanes.value > 0 else cfg.lanes))
         self.fused_lanes = lanes
         if "DM_GATHER_THREADS" not in os.environ:
@@ -646,8 +647,8 @@ class Worker:
         N.check(self.lib.dm_fexec_buffers(self._fexec, C.byref(xd), C.byref(yd), C.byref(xs), C.byref(ys),
                                           C.byref(ctl), C.byref(slots)))
         self._fx_x_dev, self._fx_y_dev, self._fx_ctl, self._fx_slots = xd.value, yd.value, ctl.value, slots.value
-        self.x_bytes = N.FUSED_ROWS_PER_SLOT * I * 4
-        self.y_bytes = N.FUSED_ROWS_PER_SLOT * Cn * 4
+        self.x_bytes = self.B_pad * I * 4
+        self.y_bytes = self.B_pad * Cn * 4
         names = spec.variable_names()
         hb, wl, bl = lay.by_name[names[0][1]], lay.by_name[names[1][0]], lay.by_name[names[1][1]]
         hw = lay.by_name[names[0][0]]
@@ -680,7 +681,7 @@ class Worker:
         p.flag_bh, p.flag_wl, p.flag_bl = hb.flag_base, wl.flag_base, bl.flag_base
         p.off_bh, p.off_wl, p.off_bl = hb.offset, wl.offset, bl.offset
         p.y_base = self._fx_y_dev
-        p.row_start, p.row_stride, p.row_wrap = 0, N.FUSED_ROWS_PER_SLOT, self._fx_slots * N.FUSED_ROWS_PER_SLOT
+        p.row_start, p.row_stride, p.row_wrap = 0, self.B_pad, self._fx_slots * self.B_pad
         p.nslots = cfg.nslots
         p.ps_global_step = (self.ps_segs[self.gs_owner].addr("ctrl", 4 * CTRL_GLOBAL_STEP)
                             if cfg.push_mode == "atomic" else None)
@@ -688,11 +689,11 @@ class Worker:
             self._fx_dbg = torch.zeros(64, dtype=torch.int64, device=f"cuda:{self.device}")
             p.debug_ts = self._fx_dbg.data_ptr()
         self._fx_params = p
-        self._fx_maps = self._fused_maps(self._fx_x_dev, self._fx_slots * N.FUSED_ROWS_PER_SLOT)
+        self._fx_maps = self._fused_maps(self._fx_x_dev, self._fx_slots * self.B_pad)
         N.check(self.lib.dm_fexec_set_params(self._fexec, C.addressof(self._fx_maps), C.addressof(p)), "set params")
         self._fx_ds_maps: Dict[Tuple[int, int], N.FusedMaps] = {}
-        self._fx_stage_x = torch.zeros(1, N.FUSED_ROWS_PER_SLOT, I, dtype=torch.float32)
-        self._fx_stage_y = torch.zeros(1, N.FUSED_ROWS_PER_SLOT, Cn, dtype=torch.float32)
+        self._fx_stage_x = torch.zeros(1, self.B_pad, I, dtype=torch.float32)
+        self._fx_stage_y = torch.zeros(1, self.B_pad, Cn, dtype=torch.float32)
         self._fx_tickets: Dict[int, StepOutput] = {}
         self._fx_ticket = 0
         # evaluation buffers (allocated now: nothing is allocated once a persistent ps kernel may be resident)
@@ -779,7 +780,8 @@ class Worker:
                 raise ValueError("fused run_resident: dataset rows must be dense fp32 [in] / [classes]")
             key = (x_base_ptr, n_rows)
             if key not in self._fx_ds_maps:
-                self._fx_ds_maps[key] = self._fused_maps(x_base_ptr, n_rows + N.FUSED_ROWS_PER_SLOT)
+                # the last batch may start at row n_rows - 1 and the kernel reads whole 32-row tiles from there
+                self._fx_ds_maps[key] = self._fused_maps(x_base_ptr, n_rows + self.B_pad)
             # wait_applied: the launch itself ends with the wait for the ps acknowledgement of its last push (no extra
             # kernel); only meaningful when a persistent ps kernel is serving
             wa = int(wait_applied and not self._ps_local)
@@ -1086,8 +1088,9 @@ class NativeLoader:
     Fused engine on cuda: the loader keeps an *epoch feed* — like TF's DataSet it holds the rows of an epoch physically
     in shuffled order (two pinned buffers: current and next epoch), so a batch is a contiguous slice of pinned memory
     that the executor DMAs to the GPU without touching it; the next epoch's buffer is filled by the executor's helper
-    threads while the current one is consumed (csrc/fused_exec.cu). ``epoch_feed=False`` (or ``DM_EPOCH_FEED=0``)
-    keeps the row-gather path for every batch."""
+    threads while the current one is consumed (csrc/fused_exec.cu). That needs a batch of whole 32-row tiles (32, 64,
+    ..., 256: a ring slot is then exactly one dense batch); other batch sizes, ``epoch_feed=False`` and
+    ``DM_EPOCH_FEED=0`` keep the row-gather path for every batch."""
 
     def __init__(self, worker: Worker, images: torch.Tensor, labels: torch.Tensor, seed: int = 0, shuffle: bool = True,
                  epoch_feed: Optional[bool] = None):
@@ -1100,7 +1103,7 @@ class NativeLoader:
         if epoch_feed is None:
             epoch_feed = os.environ.get("DM_EPOCH_FEED", "1") != "0"
         want_feed = (epoch_feed and worker.cfg.backend == "cuda" and worker.engine == "fused"
-                     and worker.batch == N.FUSED_ROWS_PER_SLOT and worker.ld_in == pix and n >= 1024)
+                     and worker.batch % N.FUSED_ROW_TILE == 0 and worker.ld_in == pix and n >= 1024)
         if worker.cfg.backend == "cuda" and not want_feed:
             self.images = self.images.pin_memory()
             self.labels = self.labels.pin_memory()
