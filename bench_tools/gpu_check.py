@@ -324,7 +324,7 @@ def check_ps_serve(ieee: bool = False) -> bool:
         P.inbox_table = table.data_ptr()
         P.exit_counter = exitc.data_ptr()
         torch.cuda.synchronize()
-        N.check(N.lib().dm_launch_ps_serve(C.addressof(P), 8, N.current_stream_ptr()), "ps_serve")
+        N.check(N.lib().dm_launch_ps_serve(C.addressof(P), 8, 1, N.current_stream_ptr()), "ps_serve")
         torch.cuda.synchronize()
         # reference: with everything pre-staged, the kernel sees (w0,w1,w2) ready for seq1, then for seq2
         mask_items = torch.zeros(arena, dtype=torch.bool, device=dev)

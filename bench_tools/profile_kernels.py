@@ -267,7 +267,7 @@ def main() -> int:
             p.launch(stream)
             if evs:
                 evs[it][j + 1].record()
-        N.check(N.lib().dm_launch_ps_serve(C.addressof(P), min(32, n_items), stream), "ps_serve")
+        N.check(N.lib().dm_launch_ps_serve(C.addressof(P), min(32, n_items), 1, stream), "ps_serve")
         if evs:
             evs[it][len(plans) + 1].record()
     torch.cuda.synchronize()

@@ -116,6 +116,7 @@ class PsServeParams(C.Structure):
 FUSED_CLUSTER = 8
 FUSED_MAX_CHUNKS = 4
 FUSED_MAX_SHARDS = 8
+LANE_REC_WORDS = 16   # protocol.h kLaneRecWords
 FUSED_ROW_TILE = 32   # rows of one row tile of the fused kernel; a batch occupies round_up(batch, 32) rows
 
 
@@ -145,6 +146,7 @@ class FusedParams(C.Structure):
         ("ps_global_step", C.c_void_p),
         ("results", C.c_void_p),
         ("debug_ts", C.c_void_p),
+        ("lane_rec", C.c_void_p),
         ("exit_counter", C.c_void_p),
         ("clear_stop", C.c_uint32), ("wait_acks", C.c_uint32),
     ]
@@ -209,7 +211,7 @@ def _declare(l: C.CDLL) -> None:
         "dm_launch_gemm": (i, [vp, vp, vp, i, i, i, i, vp]),
         "dm_launch_head": (i, [vp, vp]),
         "dm_launch_accuracy": (i, [vp, vp, i, i, vp, vp]),
-        "dm_launch_ps_serve": (i, [vp, i, vp]),
+        "dm_launch_ps_serve": (i, [vp, i, i, vp]),
         "dm_launch_dense_apply": (i, [vp, vp, vp, vp, vp, sz, i, f, f, f, f, u32, vp]),
         "dm_launch_shadow_refresh": (i, [vp, vp, sz, vp]),
         "dm_launch_worker_done": (i, [vp, vp, vp]),

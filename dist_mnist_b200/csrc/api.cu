@@ -28,7 +28,7 @@ cudaError_t preload_p2p_kernels();
 cudaError_t launch_head(const HeadParams& p, cudaStream_t stream);
 cudaError_t launch_accuracy(const float* logits, const float* labels, int B, int C, uint32_t* correct,
                             cudaStream_t stream);
-cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, cudaStream_t stream);
+cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cudaStream_t stream);
 cudaError_t launch_dense_apply(float* params, float* m, float* v, const float* grad, uint16_t* shadow, size_t n,
                                int opt, float lr, float beta1, float beta2, float eps, uint32_t t,
                                cudaStream_t stream);
@@ -301,10 +301,10 @@ int dm_launch_accuracy(const void* logits, const void* labels, int B, int C, voi
                               static_cast<uint32_t*>(correct), static_cast<cudaStream_t>(stream)));
   return 0;
 }
-int dm_launch_ps_serve(const void* params, int n_ctas, void* stream) {
+int dm_launch_ps_serve(const void* params, int n_ctas, int cluster, void* stream) {
   dm::PsServeParams p;
   memcpy(&p, params, sizeof(p));
-  DM_CUDA(dm::launch_ps_serve(p, n_ctas, static_cast<cudaStream_t>(stream)));
+  DM_CUDA(dm::launch_ps_serve(p, n_ctas, cluster, static_cast<cudaStream_t>(stream)));
   return 0;
 }
 int dm_launch_dense_apply(void* params, void* m, void* v, const void* grad, void* shadow, size_t n, int opt, float lr,

@@ -26,6 +26,12 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 
+__device__ __forceinline__ uint32_t sm_id() {
+  uint32_t s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+
 // Spin-wait guard: a kernel that waits longer than this traps instead of hanging the GPU
 // (a trap is a failed call the host can report; a hang is not).
 #ifndef DM_SPIN_TIMEOUT_NS

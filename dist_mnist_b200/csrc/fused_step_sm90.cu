@@ -192,6 +192,11 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 
   if (p.debug_ts != nullptr && blockIdx.y == 0 && rank == 0 && threadIdx.x == 0)
     p.debug_ts[60] = static_cast<long long>(globaltimer_ns());                                 // kernel entry
+  if (p.lane_rec != nullptr && threadIdx.x == 0) {
+    unsigned long long* rec = p.lane_rec + blockIdx.y * kLaneRecWords;
+    rec[rank] = sm_id();
+    if (rank == 0) rec[11] = globaltimer_ns();
+  }
   if (warp == kFsProducerWarp && lane == 0) {
     prefetch_tensormap(&maps.w[rank]);
     prefetch_tensormap(&maps.xk);
@@ -211,7 +216,12 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
   auto claim = [&]() -> uint32_t {
     if (*reinterpret_cast<volatile uint32_t*>(p.stop_word) != 0u) return kFusedNoStep;
     const uint32_t g = atomicAdd(p.step_counter, 1u);
-    return g < p.n_steps ? g : kFusedNoStep;
+    if (g >= p.n_steps) return kFusedNoStep;
+    if (p.lane_rec != nullptr) {
+      unsigned long long* rec = p.lane_rec + blockIdx.y * kLaneRecWords;
+      if (rec[8]++ == 0) rec[9] = globaltimer_ns();
+    }
+    return g;
   };
   auto broadcast_next = [&](uint32_t which, uint32_t g) {
 #pragma unroll
@@ -760,6 +770,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
   __syncthreads();
   cluster_sync_all();   // nobody leaves while a peer might still address its shared memory
   if (rank == 0 && threadIdx.x == 0) {
+    if (p.lane_rec != nullptr) p.lane_rec[blockIdx.y * kLaneRecWords + 10] = globaltimer_ns();
     // The last cluster to finish re-arms the launch state (no host-side memset / copy between launches) and, when asked
     // to, waits for the ps acknowledgement of every push made so far — every other cluster has published its steps
     // before it got here, so *seq_word is final.

@@ -183,11 +183,13 @@ struct PsServeParams {
   uint32_t oneshot;            // 1: apply whatever is pending and exit after the first full sweep that finds nothing
   uint32_t ieee_math;          //    (stream-ordered after the workers' kernels: profiler / sanitizer safe)
                                // ieee_math 1: Adam with correctly rounded sqrt / divide (`--adam_math ieee`)
-  // Optional per-CTA serve statistics [gridDim.x][8] (accumulated over launches, written when a CTA exits):
+  // Optional per-CTA serve statistics [kPsStatsCtas][8] (accumulated over launches, written when a CTA exits):
   // passes with work, pushes applied, cycles in apply, cycles in bookkeeping, idle poll rounds, cycles idle,
-  // largest number of pushes taken in one pass, poll cycles of working passes. Null = off.
+  // largest number of pushes taken in one pass, poll cycles of working passes; then [kPsStatsCtas] the SM each CTA
+  // of the last launch ran on. Null = off.
   unsigned long long* stats;
 };
+constexpr int kPsStatsCtas = 160;
 
 // ------------------------------------------------------------------------------------------------
 // Fused worker step (fused_step_sm90.cu): one 8-CTA thread-block cluster runs whole training steps of the
@@ -200,6 +202,7 @@ constexpr int kFusedCluster = 8;
 constexpr int kFusedMaxChunks = 4;   // 32-feature k-chunks per CTA  (in_features <= 8 * 4 * 32)
 constexpr int kFusedMaxShards = 8;
 constexpr uint32_t kFusedNoStep = 0xFFFFFFFFu;
+constexpr int kLaneRecWords = 16;   // FusedParams::lane_rec: [0, 8) SM ids, 8 steps, 9 first claim, 10 end, 11 entry
 
 struct FusedSlice {        // what CTA `rank` of every cluster owns
   int kc_begin;            // first k-chunk (x 32 input features)
@@ -242,6 +245,9 @@ struct FusedParams {
   uint32_t* ps_global_step;  // atomic mode: peer pointer to the shared step counter
   StepResult* results;     // [n_steps] pinned host memory, written by the kernel
   long long* debug_ts;     // optional phase stamps of cluster 0 / CTA 0
+  // optional lane residency record, [lanes][kLaneRecWords] (null in production): the SM of each CTA of the cluster,
+  // then steps the cluster claimed, globaltimer at its first claim, after its last step, and at kernel entry
+  unsigned long long* lane_rec;
   uint32_t* exit_counter;  // device word: clusters that have finished (self-resetting)
   uint32_t clear_stop;     // 1: the last cluster to exit zeroes *stop_word (last launch of a run)
   uint32_t wait_acks;      // 1: the last cluster to exit returns only after every shard has acknowledged every push made

@@ -374,20 +374,36 @@ __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_co
       unsigned long long* o = P.stats + static_cast<size_t>(blockIdx.x) * 8;
       o[0] += st_pass; o[1] += st_push; o[2] += st_apply; o[3] += st_book; o[4] += st_idle_n; o[5] += st_idle;
       o[6] = max(o[6], st_max); o[7] += st_poll;
+      P.stats[kPsStatsCtas * 8 + blockIdx.x] = sm_id();
     }
     atomicAdd(P.exit_counter, 1u);
   }
 }
 
-cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, cudaStream_t stream) {
-  if (p.n_workers > kMaxWorkers || p.n_workers < 1) return cudaErrorInvalidValue;
-  if (n_ctas > p.n_items) n_ctas = p.n_items;
+// `cluster` > 1: the grid is launched as clusters of that many CTAs. The kernel has no cluster-scope code; the
+// clusters only make the hardware place the CTAs GPC by GPC (a cluster lives inside one GPC), so that they leave
+// whole GPCs' worth of SMs to the 8-CTA clusters of a fused worker step kernel on the same GPU.
+cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cudaStream_t stream) {
+  if (p.n_workers > kMaxWorkers || p.n_workers < 1 || cluster < 1 || cluster > 8) return cudaErrorInvalidValue;
+  const int max_ctas = (p.n_items + cluster - 1) / cluster * cluster;   // whole clusters: a CTA may own no item
+  if (n_ctas > max_ctas) n_ctas = max_ctas;
   const int min_ctas = (p.n_items + kMaxOwn - 1) / kMaxOwn;  // a CTA caches at most kMaxOwn items
   if (n_ctas < min_ctas) n_ctas = min_ctas;
   if (n_ctas < 1) n_ctas = 1;
-  if (p.ieee_math) ps_serve_kernel<true><<<n_ctas, kPsThreads, 0, stream>>>(p);
-  else ps_serve_kernel<false><<<n_ctas, kPsThreads, 0, stream>>>(p);
-  return cudaGetLastError();
+  if (n_ctas % cluster != 0) return cudaErrorInvalidValue;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(n_ctas);
+  cfg.blockDim = dim3(kPsThreads);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = cluster > 1 ? 1 : 0;
+  if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<true>, p);
+  return cudaLaunchKernelEx(&cfg, ps_serve_kernel<false>, p);
 }
 
 // ------------------------------------------------------------------------------------------

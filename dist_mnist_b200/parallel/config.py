@@ -62,8 +62,9 @@ class EngineConfig:
     ps_mode: str = "persistent"      # "persistent": resident serve kernel | "oneshot": the serve kernel is launched
                                      # after the workers' kernels, applies what is pending and exits (in-process
                                      # clusters under profilers / sanitizers; `smoke()`)
-    ps_ctas: int = 0                 # CTAs of the persistent PS kernel (0 = auto: 120 on a dedicated ps GPU,
-                                     # 32 when a worker shares the GPU)
+    ps_ctas: int = 0                 # CTAs of the persistent PS kernel (0 = auto, ps.serve_geometry: 128 on a
+                                     # dedicated ps GPU, 40 beside a worker, in clusters of <= 8 beside a
+                                     # fused-engine worker; one item per CTA where possible)
     pipeline_slots: int = 0          # graph engine: worker executor ring depth (0 = auto: max(4, 2 x lanes))
     lanes: int = 1                   # steps of one worker in flight on the GPU at once. 1 = each step starts after
                                      # the previous one's kernels (reference-like); n = step i+1's pull/forward

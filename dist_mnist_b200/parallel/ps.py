@@ -17,7 +17,7 @@ import os
 import ctypes as C
 import threading
 import time
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 
 from .. import _native as N
@@ -33,6 +33,30 @@ CTRL_HOST_STOP = 1
 CTRL_EXIT_COUNTER = 2
 CTRL_WORKER_DONE = 16
 CTRL_WORDS = 64
+PS_STATS_CTAS = 160   # protocol.h kPsStatsCtas
+PS_MAX_CLUSTER = 8    # CTAs per cluster of a serve kernel packed beside a fused worker, at most
+PS_CTAS_SHARED = 40   # serve CTAs on a GPU shared with a worker, at most
+
+
+def serve_geometry(n_items: int, ps_ctas: int, shares_gpu: bool, engine: str) -> Tuple[int, int]:
+    """(CTAs, cluster size) of the persistent serve kernel of a shard with `n_items` items.
+
+    One item per CTA where possible: a dedicated ps GPU gives the serve kernel (almost) every SM, a GPU shared with a
+    worker keeps most SMs for the worker's step kernels. Every serve CTA fills an SM (512 threads x 128 registers), and
+    the fused step kernel runs as 8-CTA clusters, one CTA per SM, each cluster inside one GPC. Serve CTAs spread over
+    every GPC would leave each GPC room for fewer whole clusters; so beside a fused worker the serve kernel runs as the
+    fewest clusters of at most PS_MAX_CLUSTER CTAs that still give every item its own CTA (35 items: 5 clusters of 7).
+    The hardware places each cluster inside one GPC, where it takes exactly one of the device's cluster slots; the
+    worker caps its lanes accordingly. Rounding up to whole clusters may leave a CTA without an item. An explicit
+    `ps_ctas` is taken as it is, unclustered."""
+    if ps_ctas > 0:
+        return max(1, min(ps_ctas, n_items)), 1
+    n = max(1, min(PS_CTAS_SHARED if shares_gpu else 128, n_items))
+    if shares_gpu and engine == "fused":
+        clusters = -(-n // PS_MAX_CLUSTER)
+        size = -(-n // clusters)
+        return clusters * size, size
+    return n, 1
 
 
 def shard_carver(shard: ShardLayout, n_workers: int, nslots: int) -> Carver:
@@ -53,7 +77,7 @@ def shard_carver(shard: ShardLayout, n_workers: int, nslots: int) -> Carver:
     c.add("item_state", ni * C.sizeof(N.PsItemState))
     c.add("ctrl", CTRL_WORDS * 4)
     c.add("inbox_table", N.MAX_WORKERS * 8)
-    c.add("stats", 160 * 8 * 8)      # per-CTA serve statistics (DM_PS_STATS=1)
+    c.add("stats", PS_STATS_CTAS * 9 * 8)   # per-CTA serve statistics and SM ids (DM_PS_STATS=1)
     return c
 
 
@@ -194,8 +218,8 @@ class ParameterServer:
             if self.oneshot:
                 P.oneshot = 1   # nothing resident: `serve_once()` runs the kernel after the workers' kernels
             else:
-                n_ctas = self._serve_ctas()
-                N.check(self.lib.dm_launch_ps_serve(C.addressof(P), n_ctas, self._stream), "launch ps_serve")
+                n_ctas, cluster = self._serve_ctas()
+                N.check(self.lib.dm_launch_ps_serve(C.addressof(P), n_ctas, cluster, self._stream), "launch ps_serve")
         else:
             self._cpu_handle = self.lib.dm_cpu_ps_start(C.addressof(P))
         self._serving = True
@@ -212,7 +236,8 @@ class ParameterServer:
             return
         if after_stream is not None:
             N.check(self.lib.dm_stream_wait_stream(self._stream, after_stream), "order serve after worker")
-        N.check(self.lib.dm_launch_ps_serve(C.addressof(self._P), self._serve_ctas(), self._stream), "launch ps_serve")
+        n_ctas, cluster = self._serve_ctas()
+        N.check(self.lib.dm_launch_ps_serve(C.addressof(self._P), n_ctas, cluster, self._stream), "launch ps_serve")
         if wait:
             N.check(self.lib.dm_stream_sync(self._stream), "one-shot ps serve kernel")
 
@@ -339,7 +364,7 @@ class ParameterServer:
         `reset`: zero the counters afterwards (per-region statistics)."""
         if self.cfg.backend != "cuda" or os.environ.get("DM_PS_STATS") != "1":
             return None
-        n = 160 * 8
+        n = PS_STATS_CTAS * 9
         host = (C.c_uint64 * n)()
         N.check(self.lib.dm_memcpy_async(C.addressof(host), self.seg.addr("stats"), 8 * n, None))
         N.check(self.lib.dm_stream_sync(None))
@@ -347,7 +372,8 @@ class ParameterServer:
             zeros = (C.c_uint64 * n)()
             N.check(self.lib.dm_memcpy_async(self.seg.addr("stats"), C.addressof(zeros), 8 * n, None))
             N.check(self.lib.dm_stream_sync(None))
-        rows = [list(host[i * 8:(i + 1) * 8]) for i in range(160) if host[i * 8] or host[i * 8 + 4]]
+        live = [i for i in range(PS_STATS_CTAS) if host[i * 8] or host[i * 8 + 4]]
+        rows = [list(host[i * 8:(i + 1) * 8]) for i in live]
         if not rows:
             return None
         tot = [sum(r[j] for r in rows) for j in range(8)]
@@ -362,16 +388,13 @@ class ParameterServer:
             "poll_us_per_working_pass": round(tot[7] / max(tot[0], 1) / mhz, 2),
             "idle_polls": tot[4], "idle_poll_us": round(tot[5] / max(tot[4], 1) / mhz, 2),
             "busy_fraction": round((tot[2] + tot[3] + tot[7]) / max(tot[2] + tot[3] + tot[7] + tot[5], 1), 3),
+            "smids": [int(host[PS_STATS_CTAS * 8 + i]) for i in live],   # SM of each CTA in its last launch
         }
 
-    def _serve_ctas(self) -> int:
-        """One item per CTA where possible: a dedicated ps GPU gives the serve kernel (almost) every SM, a GPU
-        shared with a worker keeps most SMs for the worker's step kernels."""
-        want = self.cfg.ps_ctas
-        if want <= 0:
-            shared = any(d == self.device for d in self._attached_device.values())
-            want = 40 if shared else 128
-        return max(1, min(want, self.shard.n_items))
+    def _serve_ctas(self) -> Tuple[int, int]:
+        """(CTAs, cluster size) of this shard's serve kernel, from the workers attached now (see serve_geometry)."""
+        shared = any(d == self.device for d in self._attached_device.values())
+        return serve_geometry(self.shard.n_items, self.cfg.ps_ctas, shared, self.engine)
 
     def restart(self) -> None:
         """Relaunch the serve kernel / loop after `stop()` (all shard state lives in the segment, so serving
@@ -389,8 +412,8 @@ class ParameterServer:
             N.check(self.lib.dm_set_device(self.device), "set device")
             N.check(self.lib.dm_memset_async(self.seg.addr("ctrl", 4 * CTRL_HOST_STOP), 0, 4, self._ctl_stream))
             N.check(self.lib.dm_stream_sync(self._ctl_stream))
-            n_ctas = self._serve_ctas()
-            N.check(self.lib.dm_launch_ps_serve(C.addressof(self._P), n_ctas, self._stream), "launch ps_serve")
+            n_ctas, cluster = self._serve_ctas()
+            N.check(self.lib.dm_launch_ps_serve(C.addressof(self._P), n_ctas, cluster, self._stream), "launch ps_serve")
         else:
             self.lib.dm_store_release_u32(self.seg.addr("ctrl", 4 * CTRL_HOST_STOP), 0)
             self._cpu_handle = self.lib.dm_cpu_ps_start(C.addressof(self._P))

@@ -40,7 +40,7 @@ from ..ops import gemm as gemm_ops
 from ..ops import head as head_ops
 from .config import MAX_SLOTS, EngineConfig, OptimizerConfig
 from .peer_mem import Carver, Segment
-from .ps import CTRL_GLOBAL_STEP, CTRL_WORKER_DONE
+from .ps import CTRL_GLOBAL_STEP, CTRL_WORKER_DONE, serve_geometry
 from .sharding import FUSED_CLUSTER, ModelLayout, VarLayout, build_layout, dw_tile_n_for
 from ..utils.metrics import nvtx_annotate
 
@@ -627,7 +627,15 @@ class Worker:
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
         N.check(self.lib.dm_fused_max_lanes(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
-        lanes = max(1, min(cfg.lanes, max_lanes.value if max_lanes.value > 0 else cfg.lanes))
+        free = max_lanes.value
+        if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
+            # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots
+            for desc in self.ps_desc:
+                if desc.get("device") == self.device:
+                    n_ctas, cluster = serve_geometry(desc["n_items"], cfg.ps_ctas, True, self.engine)
+                    if cluster > 1:
+                        free -= n_ctas // cluster
+        lanes = max(1, min(cfg.lanes, free if max_lanes.value > 0 else cfg.lanes))
         self.fused_lanes = lanes
         if "DM_GATHER_THREADS" not in os.environ:
             # the gather pool spins while a run is active: share the host's cores between the worker processes of
