@@ -356,6 +356,101 @@ def check_ps_serve(ieee: bool = False) -> bool:
     return ok
 
 
+def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
+    """The serve kernel's Momentum / Adagrad / RMSProp instantiations (`opt`: an OptimizerConfig; `opt.math` picks the
+    fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
+    against the TF1 formulas in fp64 (parameters and both slot buffers within 1e-5 relative error; the bf16 shadow,
+    global_step and the acks exact). `resident`: one pushed push per worker and pass (lookahead 1) and one vectorisable
+    item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass."""
+    from bench_tools.gpu_e2e import tf1_apply
+    from dist_mnist_b200 import _native as N
+    dev = "cuda"
+    torch.manual_seed(6)
+    n_workers, nslots, n_push = 3, 3, 3
+    if resident:
+        rows, cols, blk = 100, 256, 16
+        items = [(r0 * cols, min(blk, rows - r0), cols, cols) for r0 in range(0, rows, blk)]   # 16 x 256 = 4096
+        arena = rows * cols
+    else:
+        rows, cols, ld, bn = 100, 784, 784, 64
+        items = [(c0, rows, min(bn, cols - c0), ld) for c0 in range(0, cols, bn)]
+        small_off = rows * ld
+        items.append((small_off, 1, 1110, 1110))           # not vectorisable: the scalar path
+        arena = (small_off + 1110 + 2 + 3) // 4 * 4
+    n_items = len(items)
+    m0, v0 = opt.slot_init()
+    params = torch.randn(arena, device=dev)
+    p0 = params.clone()
+    m = torch.full((arena,), m0, device=dev)
+    v = torch.full((arena,), v0, device=dev)
+    shadow = torch.zeros(arena, dtype=torch.bfloat16, device=dev)
+    mailbox = torch.zeros(n_workers, nslots, arena, device=dev)
+    flags = torch.zeros(n_workers, nslots, n_items, dtype=torch.int32, device=dev)
+    next_seq = torch.ones(n_workers, n_items, dtype=torch.int32, device=dev)
+    consumed = torch.zeros(n_workers, nslots, dtype=torch.int32, device=dev)
+    gstep = torch.zeros(1, dtype=torch.int32, device=dev)
+    done = torch.zeros(n_workers, dtype=torch.int32, device=dev)
+    stop = torch.zeros(1, dtype=torch.int32, device=dev)
+    exitc = torch.zeros(1, dtype=torch.int32, device=dev)
+    inbox = torch.zeros(n_workers, 2, dtype=torch.int32, device=dev)
+    host_items = (N.PsItem * n_items)()
+    for i, (off, r, c, l) in enumerate(items):
+        host_items[i].offset, host_items[i].rows, host_items[i].cols, host_items[i].ld = off, r, c, l
+        host_items[i].flags, host_items[i].flag_index = 1, i
+    items_t = torch.frombuffer(bytearray(bytes(host_items)), dtype=torch.uint8).to(dev)
+    st_host = (N.PsItemState * n_items)()
+    for i in range(n_items):
+        st_host[i].t, st_host[i].beta1_pow, st_host[i].beta2_pow = 0, 1.0, 1.0
+    state = torch.frombuffer(bytearray(bytes(st_host)), dtype=torch.uint8).to(dev)
+    grads = torch.randn(n_workers, n_push, arena, device=dev) * 0.1
+    for w in range(n_workers):
+        for s in range(1, n_push + 1):
+            mailbox[w, s % nslots] = grads[w, s - 1]
+            flags[w, s % nslots, :] = s
+        done[w] = n_push + 1
+    P = N.PsServeParams()
+    P.params, P.adam_m, P.adam_v, P.shadow_bf16 = params.data_ptr(), m.data_ptr(), v.data_ptr(), shadow.data_ptr()
+    P.items, P.item_state = items_t.data_ptr(), state.data_ptr()
+    P.n_items, P.n_workers, P.nslots, P.opt, P.apply_mode = n_items, n_workers, nslots, opt.native_kind, apply_mode
+    P.n_flags = n_items
+    P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
+    P.momentum, P.decay, P.nesterov = opt.momentum or 0.0, opt.decay or 0.0, int(opt.use_nesterov)
+    P.ieee_math = 1 if opt.math == "ieee" else 0
+    P.lookahead = 1 if resident else 0
+    P.mailbox, P.arena_elems = mailbox.data_ptr(), arena
+    P.flags, P.next_seq, P.consumed = flags.data_ptr(), next_seq.data_ptr(), consumed.data_ptr()
+    P.global_step, P.worker_done, P.host_stop = gstep.data_ptr(), done.data_ptr(), stop.data_ptr()
+    table = torch.tensor([inbox[w].data_ptr() for w in range(n_workers)], dtype=torch.int64, device=dev)
+    P.inbox_table = table.data_ptr()
+    P.exit_counter = exitc.data_ptr()
+    torch.cuda.synchronize()
+    n_ctas = n_items if resident else 8
+    N.check(N.lib().dm_launch_ps_serve(C.addressof(P), n_ctas, 1, N.current_stream_ptr()), "ps_serve")
+    torch.cuda.synchronize()
+    # reference (fp64): the kernel applies round k (the k-th push of every worker, workers in order) before round k + 1
+    mask = torch.zeros(arena, dtype=torch.bool, device=dev)
+    for (off, r, c, l) in items:
+        for rr in range(r):
+            mask[off + rr * l: off + rr * l + c] = True
+    pr, mr, vr = p0.double(), torch.full((arena,), m0, dtype=torch.float64, device=dev), \
+        torch.full((arena,), v0, dtype=torch.float64, device=dev)
+    for s in range(n_push):
+        group = [grads[w, s].double() for w in range(n_workers)]
+        for gg in ([sum(group)] if apply_mode == N.APPLY_MERGED else group):
+            pr, mr, vr = tf1_apply(opt, pr, mr, vr, gg)
+    pr, mr, vr = torch.where(mask, pr, p0.double()), torch.where(mask, mr, m0), torch.where(mask, vr, v0)
+    e_p, e_m, e_v = rel_err(params, pr), rel_err(m, mr), rel_err(v, vr)
+    shadow_exact = bool(torch.equal(shadow[mask], params[mask].to(torch.bfloat16)))
+    gs = int(gstep.item())
+    acks = inbox[:, 0].tolist()
+    good = (max(e_p, e_m, e_v) < 1e-5 and shadow_exact and gs == n_workers * n_push and acks == [n_push] * n_workers
+            and int(exitc.item()) == n_ctas)
+    name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''} momentum={opt.momentum} math={opt.math} "
+            f"mode={apply_mode} resident={resident}")
+    return report(name, good, f"err p={e_p:.1e} m={e_m:.1e} v={e_v:.1e} shadow_exact={shadow_exact} global_step={gs} "
+                              f"acks={acks} exit={int(exitc.item())}")
+
+
 def check_dense_apply() -> bool:
     from dist_mnist_b200 import _native as N
     ok = True

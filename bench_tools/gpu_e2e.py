@@ -20,6 +20,31 @@ from dist_mnist_b200.session import InProcessCluster
 from dist_mnist_b200.utils import data
 
 
+def tf1_apply(opt, p, m, v, g):
+    """One TF1 `training_ops` step of Momentum / Adagrad / RMSProp (not centered) on tensors, in their own dtype:
+    `m` is the slot kept in adam_m (momentum accumulator, RMSProp mom), `v` the one in adam_v (Adagrad accumulator,
+    RMSProp ms). Returns the new (p, m, v)."""
+    if opt.kind == "momentum":
+        m = opt.momentum * m + g
+        p = p - (g * opt.lr + m * opt.momentum * opt.lr) if opt.use_nesterov else p - opt.lr * m
+    elif opt.kind == "adagrad":
+        v = v + g * g
+        p = p - opt.lr * g / v.sqrt()
+    elif opt.kind == "rmsprop":
+        v = v + (g * g - v) * (1 - opt.decay)
+        m = opt.momentum * m + opt.lr * g / (v + opt.eps).sqrt()
+        p = p - m
+    else:
+        raise ValueError(opt.kind)
+    return p, m, v
+
+
+def ref_slots(opt, params):
+    """Initial (m, v) slot dicts of `opt` for `params` (Worker.initialize_variables writes the same values)."""
+    m0, v0 = opt.slot_init()
+    return ({k: torch.full_like(t, m0) for k, t in params.items()}, {k: torch.full_like(t, v0) for k, t in params.items()})
+
+
 def ref_step(spec, params, m, v, t, x, y, opt):
     loss, grads, _ = mlp.manual_loss_and_grads(spec, params, x, y)
     t += 1
@@ -27,6 +52,8 @@ def ref_step(spec, params, m, v, t, x, y, opt):
         g = grads[k]
         if opt.kind == "sgd":
             params[k] = params[k] - opt.lr * g
+        elif opt.kind != "adam":
+            params[k], m[k], v[k] = tf1_apply(opt, params[k], m[k], v[k], g)
         else:
             m[k] = opt.beta1 * m[k] + (1 - opt.beta1) * g
             v[k] = opt.beta2 * v[k] + (1 - opt.beta2) * g * g

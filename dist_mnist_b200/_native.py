@@ -23,7 +23,7 @@ MAX_WORKERS = 32
 PUSH_LOCAL, PUSH_MAILBOX, PUSH_ATOMIC = 0, 1, 2
 EPI_TRANSPOSED, EPI_ROWMAJOR_PUSH = 0, 1
 LOSS_BOOK, LOSS_XENT = 0, 1
-OPT_SGD, OPT_ADAM = 0, 1
+OPT_SGD, OPT_ADAM, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3, 4
 APPLY_PER_PUSH, APPLY_MERGED = 0, 1
 DT_F32, DT_BF16 = 0, 1
 
@@ -110,6 +110,7 @@ class PsServeParams(C.Structure):
         ("gpu_scope", C.c_uint32), ("lookahead", C.c_uint32),
         ("oneshot", C.c_uint32), ("ieee_math", C.c_uint32),
         ("stats", C.c_void_p),
+        ("momentum", C.c_float), ("decay", C.c_float), ("nesterov", C.c_uint32), ("pad_", C.c_uint32),
     ]
 
 

@@ -49,6 +49,22 @@ def engine_config_from_args(args, backend: str) -> EngineConfig:
                         strict_steps=args.strict_steps, ps_row_blocks=args.ps_row_blocks)
 
 
+# optimizer flag -> the optimizers that use it
+_OPT_FLAGS = {"momentum": ("momentum", "rmsprop"), "use_nesterov": ("momentum",), "rmsprop_decay": ("rmsprop",),
+              "initial_accumulator_value": ("adagrad",), "epsilon": ("adam", "rmsprop")}
+
+
+def optimizer_config_from_args(args) -> OptimizerConfig:
+    """The optimizer every task derives from the command line; a hyper-parameter flag the chosen optimizer does not
+    use is an error."""
+    for flag, kinds in _OPT_FLAGS.items():
+        if getattr(args, flag) not in (None, False) and args.optimizer not in kinds:
+            raise ValueError(f"--{flag} does not apply to --optimizer {args.optimizer} (only {', '.join(kinds)})")
+    return OptimizerConfig(args.optimizer, args.learning_rate, eps=args.epsilon, math=args.adam_math,
+                           momentum=args.momentum, use_nesterov=args.use_nesterov, decay=args.rmsprop_decay,
+                           initial_accumulator_value=args.initial_accumulator_value)
+
+
 def build_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(prog="distributed_server-basic", description=__doc__,
                                 formatter_class=argparse.RawDescriptionHelpFormatter)
@@ -65,9 +81,19 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--job_name", type=str, default=None, help="worker or ps")
     p.add_argument("--task_index", type=int, default=None)
     # ---- new-engine flags ----
-    p.add_argument("--optimizer", choices=["adam", "sgd"], default="adam", help="reference uses Adam (DS:102)")
+    p.add_argument("--optimizer", choices=["adam", "sgd", "momentum", "adagrad", "rmsprop"], default="adam",
+                   help="reference uses Adam (DS:102); momentum / adagrad / rmsprop are TF1's MomentumOptimizer, "
+                        "AdagradOptimizer and (non-centered) RMSPropOptimizer, applied on the ps")
     p.add_argument("--adam_math", choices=["fast", "ieee"], default="fast",
-                   help="ps-side Adam arithmetic (cuda): MUFU sqrt/reciprocal (default) or correctly rounded like TF's ApplyAdam")
+                   help="ps-side arithmetic of Adam, Adagrad and RMSProp (cuda): MUFU sqrt/reciprocal (default) or "
+                        "correctly rounded like TF's Apply* kernels")
+    # optimizer hyper-parameters: unset = the chosen optimizer's TF1 default; one it does not use is an error
+    p.add_argument("--momentum", type=float, default=None, help="momentum (0.9) and rmsprop (0.0)")
+    p.add_argument("--use_nesterov", action="store_true", help="momentum: Nesterov momentum")
+    p.add_argument("--rmsprop_decay", type=float, default=None, help="rmsprop: decay of the mean square (0.9)")
+    p.add_argument("--initial_accumulator_value", type=float, default=None,
+                   help="adagrad: starting value of the accumulator (0.1)")
+    p.add_argument("--epsilon", type=float, default=None, help="adam (1e-8) and rmsprop (1e-10)")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")
@@ -143,7 +169,7 @@ def run(args: argparse.Namespace) -> int:
     cluster.task_endpoint(args.job_name, args.task_index)
     backend = resolve_backend(args.backend)
     spec = mlp.get_model(args.model, args.hidden_units)
-    opt = OptimizerConfig(args.optimizer, args.learning_rate, math=args.adam_math)
+    opt = optimizer_config_from_args(args)
     cfg = engine_config_from_args(args, backend)
     cfg.validate(opt)
     device = -1

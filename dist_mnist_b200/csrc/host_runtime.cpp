@@ -47,15 +47,35 @@ struct CpuPs {
   std::atomic<uint64_t> applied{0};
 };
 
+// TF1 Apply{Momentum,Adagrad,RMSProp} with IEEE arithmetic (ps_apply_sm90.cu tf1_step)
+void tf1_step_cpu(const dm::PsServeParams& P, float& p, float& m, float& v, float g) {
+  if (P.opt == dm::OPT_MOMENTUM) {
+    m = P.momentum * m + g;
+    if (P.nesterov) p -= g * P.lr + m * P.momentum * P.lr;
+    else p -= P.lr * m;
+  } else if (P.opt == dm::OPT_ADAGRAD) {
+    v += g * g;
+    p -= P.lr * g / std::sqrt(v);
+  } else {   // OPT_RMSPROP
+    v += (g * g - v) * (1.f - P.decay);
+    m = P.momentum * m + P.lr * g / std::sqrt(v + P.eps);
+    p -= m;
+  }
+}
+
 void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItemState st, uint32_t mask,
                     const uint32_t* seqs) {
   const uint64_t wstride = static_cast<uint64_t>(P.nslots) * P.arena_elems;
+  const bool tf1 = P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
+  const bool use_m = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_RMSPROP;
+  const bool use_v = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
   for (int r = 0; r < it.rows; ++r) {
     for (int c = 0; c < it.cols; ++c) {
       const uint64_t a = it.offset + static_cast<uint64_t>(r) * it.ld + c;
       float p = P.params[a];
       float m = 0.f, v = 0.f;
-      if (P.opt == dm::OPT_ADAM) { m = P.adam_m[a]; v = P.adam_v[a]; }
+      if (use_m) m = P.adam_m[a];
+      if (use_v) v = P.adam_v[a];
       float b1p = st.beta1_pow, b2p = st.beta2_pow;
       float gsum = 0.f;
       uint32_t mm = mask;
@@ -65,7 +85,9 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         const uint32_t slot = seqs[w] % P.nslots;
         const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
         if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
-        if (P.opt == dm::OPT_ADAM) {
+        if (tf1) {
+          tf1_step_cpu(P, p, m, v, g);
+        } else if (P.opt == dm::OPT_ADAM) {
           b1p *= P.beta1; b2p *= P.beta2;
           const float lr_t = P.lr * std::sqrt(1.f - b2p) / (1.f - b1p);
           m = P.beta1 * m + (1.f - P.beta1) * g;
@@ -76,7 +98,9 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         }
       }
       if (P.apply_mode == dm::APPLY_MERGED) {
-        if (P.opt == dm::OPT_ADAM) {
+        if (tf1) {
+          tf1_step_cpu(P, p, m, v, gsum);
+        } else if (P.opt == dm::OPT_ADAM) {
           b1p *= P.beta1; b2p *= P.beta2;
           const float lr_t = P.lr * std::sqrt(1.f - b2p) / (1.f - b1p);
           m = P.beta1 * m + (1.f - P.beta1) * gsum;
@@ -87,7 +111,8 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         }
       }
       P.params[a] = p;
-      if (P.opt == dm::OPT_ADAM) { P.adam_m[a] = m; P.adam_v[a] = v; }
+      if (use_m) P.adam_m[a] = m;
+      if (use_v) P.adam_v[a] = v;
       if (P.shadow_bf16 != nullptr && (it.flags & 1)) P.shadow_bf16[a] = f32_to_bf16(p);
     }
   }

@@ -146,7 +146,9 @@ struct PsItemState {  // persisted across serve-kernel launches and checkpointed
   uint32_t pad_;
 };
 
-enum OptimizerKind : int { OPT_SGD = 0, OPT_ADAM = 1 };
+// TF1 `training_ops` rules applied per push (or per round, APPLY_MERGED). Slot buffers: adam_m = Adam m / momentum
+// accumulator / RMSProp mom; adam_v = Adam v / Adagrad accumulator / RMSProp ms.
+enum OptimizerKind : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_MOMENTUM = 2, OPT_ADAGRAD = 3, OPT_RMSPROP = 4 };
 enum ApplyMode : int {
   APPLY_PER_PUSH = 0,  // reference semantics: every worker push is its own optimizer step
   APPLY_MERGED = 1,    // pushes that are ready at the same poll are summed and applied as one step
@@ -182,12 +184,19 @@ struct PsServeParams {
   uint32_t lookahead;          // max pushes of one worker consumed per item pass (0 = auto: up to nslots)
   uint32_t oneshot;            // 1: apply whatever is pending and exit after the first full sweep that finds nothing
   uint32_t ieee_math;          //    (stream-ordered after the workers' kernels: profiler / sanitizer safe)
-                               // ieee_math 1: Adam with correctly rounded sqrt / divide (`--adam_math ieee`)
+                               // ieee_math 1: correctly rounded sqrt / divide in Adam, Adagrad and RMSProp
+                               //   (`--adam_math ieee`)
   // Optional per-CTA serve statistics [kPsStatsCtas][8] (accumulated over launches, written when a CTA exits):
   // passes with work, pushes applied, cycles in apply, cycles in bookkeeping, idle poll rounds, cycles idle,
   // largest number of pushes taken in one pass, poll cycles of working passes; then [kPsStatsCtas] the SM each CTA
   // of the last launch ran on. Null = off.
   unsigned long long* stats;
+  // hyper-parameters of the rules after Adam / SGD (appended, so that no earlier field moves); `eps` above is also
+  // RMSProp's epsilon
+  float momentum;              // OPT_MOMENTUM, OPT_RMSPROP
+  float decay;                 // OPT_RMSPROP (TF1 `decay`, rho)
+  uint32_t nesterov;           // OPT_MOMENTUM: 1 = use_nesterov
+  uint32_t pad_;
 };
 constexpr int kPsStatsCtas = 160;
 

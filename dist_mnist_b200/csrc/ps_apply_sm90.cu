@@ -4,7 +4,8 @@
 // /root/reference/distributed_server-basic.py:80-83) turned into a persistent GPU kernel: it owns the
 // shard (params + Adam slots + global_step, DS:88-91,102-103), polls the per-item flags that workers
 // publish with st.release.sys after their in-kernel P2P gradient stores, reduces whatever is ready
-// (many-to-one) and applies the optimizer in the same pass (ApplyAdam / SGD, SURVEY K7), bumps
+// (many-to-one) and applies the optimizer in the same pass (ApplyAdam / SGD, SURVEY K7; or TF1's
+// ApplyMomentum / ApplyAdagrad / ApplyRMSProp in their own instantiations), bumps
 // global_step (K8) and acknowledges into the worker's inbox over NVLink. No host, NCCL or gRPC in the loop.
 //
 // Work decomposition: items (2-D blocks of the arena) are dealt round-robin to CTAs; a CTA never shares
@@ -51,6 +52,42 @@ __device__ __forceinline__ float adam_lr_t(float lr, float b1p, float b2p) {
   else return lr * sqrt_approx(1.f - b2p) * rcp_approx(1.f - b1p);   // lr * sqrt(1 - b2^t) / (1 - b1^t)
 }
 
+// The other TF1 `training_ops` rules (Apply{Momentum,Adagrad,RMSProp}). Slots: adam_m holds the momentum accumulator /
+// RMSProp's mom, adam_v holds Adagrad's accumulator / RMSProp's ms (m and v below).
+__device__ __forceinline__ float rsqrt_approx(float x) {
+  float y;
+  asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+template <bool kIeee>
+__device__ __forceinline__ float div_sqrt(float a, float x) {   // a / sqrt(x)
+  if constexpr (kIeee) return __fdiv_rn(a, __fsqrt_rn(x));
+  else return a * rsqrt_approx(x);
+}
+template <int kOpt, bool kIeee>
+__device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, const PsServeParams& P) {
+  if constexpr (kOpt == OPT_MOMENTUM) {
+    // accum <- momentum accum + g ; p <- p - lr accum  (Nesterov: p <- p - lr g - lr momentum accum)
+    m = fmaf(P.momentum, m, g);
+    if (P.nesterov) p = p - fmaf(g, P.lr, m * P.momentum * P.lr);
+    else p = fmaf(-P.lr, m, p);
+  } else if constexpr (kOpt == OPT_ADAGRAD) {
+    // accum <- accum + g^2 ; p <- p - lr g / sqrt(accum)   (no epsilon)
+    v = fmaf(g, g, v);
+    p = p - div_sqrt<kIeee>(P.lr * g, v);
+  } else {
+    static_assert(kOpt == OPT_RMSPROP, "unknown optimizer family");
+    // ms <- ms + (g^2 - ms)(1 - decay) ; mom <- momentum mom + lr g / sqrt(ms + eps) ; p <- p - mom
+    v = fmaf(fmaf(g, g, -v), 1.f - P.decay, v);
+    m = fmaf(P.momentum, m, div_sqrt<kIeee>(P.lr * g, v + P.eps));
+    p = p - m;
+  }
+}
+
+// Optimizer family of a serve-kernel instantiation. Adam and SGD share the two instantiations that were measured (P.opt
+// picks the rule at run time; their SASS is unchanged by the other families); every other kind gets its own.
+constexpr int kFamAdamSgd = -1;
+
 // Apply every pending push to one item. s_pend[0..n_pend) lists the mailbox slots (element offset of the slot
 // inside P.mailbox) in application order — round k = the k-th pending push of every worker, oldest round first —
 // and s_round[i] is the round of entry i. One optimizer step per push, or per round in APPLY_MERGED mode
@@ -65,14 +102,17 @@ struct ResidentState {
   bool loaded;
 };
 
-template <bool kIeee>
+template <bool kIeee, int kFam>
 __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItemState st, const uint64_t* s_pend,
                            const uint32_t* s_round, const int n_pend, ResidentState* res = nullptr) {
   const int tid = threadIdx.x;
   const int total = it.rows * it.cols;
   const bool vec = ((it.cols & 3) == 0) && ((it.ld & 3) == 0) && ((it.offset & 3) == 0);
   const int step = vec ? 4 : 1;
-  const bool adam = P.opt == OPT_ADAM;
+  const bool adam = kFam == kFamAdamSgd && P.opt == OPT_ADAM;
+  // the slot buffers this rule reads and writes
+  const bool use_m = kFam == kFamAdamSgd ? adam : (kFam == OPT_MOMENTUM || kFam == OPT_RMSPROP);
+  const bool use_v = kFam == kFamAdamSgd ? adam : (kFam == OPT_ADAGRAD || kFam == OPT_RMSPROP);
   const bool merged = P.apply_mode == APPLY_MERGED;
   for (int e0 = tid * step; e0 < total; e0 += kPsThreads * step * kQuads) {
     uint64_t a[kQuads];
@@ -101,15 +141,18 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         if (vec) {
           const float4 t = __ldcg(reinterpret_cast<const float4*>(P.params + a[q]));
           pv[q][0] = t.x; pv[q][1] = t.y; pv[q][2] = t.z; pv[q][3] = t.w;
-          if (adam) {
+          if (use_m) {
             const float4 tm = __ldcg(reinterpret_cast<const float4*>(P.adam_m + a[q]));
-            const float4 tv = __ldcg(reinterpret_cast<const float4*>(P.adam_v + a[q]));
             mv[q][0] = tm.x; mv[q][1] = tm.y; mv[q][2] = tm.z; mv[q][3] = tm.w;
+          }
+          if (use_v) {
+            const float4 tv = __ldcg(reinterpret_cast<const float4*>(P.adam_v + a[q]));
             vv[q][0] = tv.x; vv[q][1] = tv.y; vv[q][2] = tv.z; vv[q][3] = tv.w;
           }
         } else {
           pv[q][0] = __ldcg(P.params + a[q]);
-          if (adam) { mv[q][0] = __ldcg(P.adam_m + a[q]); vv[q][0] = __ldcg(P.adam_v + a[q]); }
+          if (use_m) mv[q][0] = __ldcg(P.adam_m + a[q]);
+          if (use_v) vv[q][0] = __ldcg(P.adam_v + a[q]);
         }
       }
     }
@@ -120,10 +163,12 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
       for (int j = 0; j < 4; ++j) gsum[q][j] = 0.f;
 
-    for (int i0 = 0; i0 < n_pend; i0 += kChunk) {
-      float g[kChunk][kQuads][4];
+    // the other families' straight-line update keeps more values live: a chunk of 8 spills there, 7 does not
+    constexpr int kCh = kFam == kFamAdamSgd ? kChunk : kChunk - 1;
+    for (int i0 = 0; i0 < n_pend; i0 += kCh) {
+      float g[kCh][kQuads][4];
 #pragma unroll
-      for (int ci = 0; ci < kChunk; ++ci) {
+      for (int ci = 0; ci < kCh; ++ci) {
         const bool live = i0 + ci < n_pend;
         const float* gbase = P.mailbox + s_pend[live ? i0 + ci : i0];
 #pragma unroll
@@ -139,7 +184,7 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         }
       }
 #pragma unroll
-      for (int ci = 0; ci < kChunk; ++ci) {
+      for (int ci = 0; ci < kCh; ++ci) {
         const int i = i0 + ci;
         if (i >= n_pend) break;
         bool do_step = true;
@@ -163,7 +208,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
           for (int j = 0; j < 4; ++j) {
             if (j >= step) continue;
             const float gv = merged ? gsum[q][j] : g[ci][q][j];
-            if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, lr_t, P.beta1, P.beta2, P.eps);
+            if constexpr (kFam != kFamAdamSgd) tf1_step<kFam, kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, P);
+            else if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, lr_t, P.beta1, P.beta2, P.eps);
             else pv[q][j] = fmaf(-P.lr, gv, pv[q][j]);
             if (merged) gsum[q][j] = 0.f;
           }
@@ -183,10 +229,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
       const bool shadow = P.shadow_bf16 != nullptr && (it.flags & 1);
       if (vec) {
         *reinterpret_cast<float4*>(P.params + a[q]) = make_float4(pv[q][0], pv[q][1], pv[q][2], pv[q][3]);
-        if (adam) {
-          *reinterpret_cast<float4*>(P.adam_m + a[q]) = make_float4(mv[q][0], mv[q][1], mv[q][2], mv[q][3]);
-          *reinterpret_cast<float4*>(P.adam_v + a[q]) = make_float4(vv[q][0], vv[q][1], vv[q][2], vv[q][3]);
-        }
+        if (use_m) *reinterpret_cast<float4*>(P.adam_m + a[q]) = make_float4(mv[q][0], mv[q][1], mv[q][2], mv[q][3]);
+        if (use_v) *reinterpret_cast<float4*>(P.adam_v + a[q]) = make_float4(vv[q][0], vv[q][1], vv[q][2], vv[q][3]);
         if (shadow) {
           __nv_bfloat162 lo = __floats2bfloat162_rn(pv[q][0], pv[q][1]);
           __nv_bfloat162 hi = __floats2bfloat162_rn(pv[q][2], pv[q][3]);
@@ -197,7 +241,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         }
       } else {
         P.params[a[q]] = pv[q][0];
-        if (adam) { P.adam_m[a[q]] = mv[q][0]; P.adam_v[a[q]] = vv[q][0]; }
+        if (use_m) P.adam_m[a[q]] = mv[q][0];
+        if (use_v) P.adam_v[a[q]] = vv[q][0];
         if (shadow) {
           __nv_bfloat16 b = __float2bfloat16(pv[q][0]);
           P.shadow_bf16[a[q]] = *reinterpret_cast<uint16_t*>(&b);
@@ -207,177 +252,17 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
   }
 }
 
+// Adam / SGD: ps_serve_kernel<kIeee>, the two instantiations that were measured.
 template <bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
-  // Everything the poll loop needs about this CTA's items lives in shared memory: the only global traffic of an
-  // idle poll is one acquire load of a flag word per (worker, look-ahead slot).
-  __shared__ PsItem s_item[kMaxOwn];
-  __shared__ PsItemState s_state[kMaxOwn];
-  __shared__ uint32_t s_next[kMaxOwn][kMaxWorkers];  // next expected push seq per (owned item, worker)
-  __shared__ uint64_t s_pend[kMaxPending];
-  __shared__ uint32_t s_round[kMaxPending];
-  __shared__ uint32_t s_npend;
-  __shared__ uint32_t s_any;
-  __shared__ uint32_t s_exit;
-  const int tid = threadIdx.x;
-  const int lane = tid & 31;
-  const int warp = tid >> 5;
-  uint32_t iter = 0;
-  int n_own = 0;
-  for (int item = blockIdx.x; item < P.n_items && n_own < kMaxOwn; item += gridDim.x) ++n_own;
-  for (int i = tid; i < n_own; i += kPsThreads) {
-    const int item = blockIdx.x + i * gridDim.x;
-    s_item[i] = P.items[item];
-    s_state[i] = P.item_state[item];
-  }
-  for (int i = tid; i < n_own * kMaxWorkers; i += kPsThreads) {
-    const int own = i / kMaxWorkers, w = i - own * kMaxWorkers;
-    s_next[own][w] = w < P.n_workers ? P.next_seq[static_cast<size_t>(w) * P.n_items + blockIdx.x + own * gridDim.x] : 0u;
-  }
-  __syncthreads();
-  // poll lanes, round-major: lane = k * n_workers + w checks push s_next[w] + k of worker w. Pushes of one worker
-  // are consumed in order, so only its contiguous ready prefix k = 0 .. cnt-1 is taken in a pass; lane order is
-  // then exactly the application order (round k = k-th pending push of every worker, oldest round first).
-  const int nw = P.n_workers;
-  int kdepth = max(1, min(min(P.nslots, 16), 32 / nw));
-  if (P.lookahead != 0u) kdepth = min(kdepth, static_cast<int>(P.lookahead));
-  const int pk = lane / nw, pw = lane - pk * nw;
-  const bool pvalid = pk < kdepth;
-  const uint64_t wstride = static_cast<uint64_t>(P.nslots) * P.arena_elems;
-
-  // Register-resident optimizer state: a CTA that owns exactly one vectorisable item of at most one sweep keeps the
-  // item's parameters and Adam slots in registers from pass to pass (it is the only writer while it runs; the host
-  // writes variables only while no serve kernel is resident). Results are still stored every pass — the workers pull
-  // the parameters, checkpoints read the slots — but the three load round trips (~1 us of a ~6.7 us pass) are gone.
-  ResidentState resident;
-  resident.loaded = false;
-  bool use_resident = false;
-  if (n_own == 1) {
-    const PsItem it0 = s_item[0];
-    use_resident = ((it0.cols & 3) == 0) && ((it0.ld & 3) == 0) && ((it0.offset & 3) == 0) &&
-                   (it0.rows * it0.cols <= kPsThreads * kQuads * 4);
-  }
-
-  // serve statistics (thread 0's view; the CTA barriers make it representative)
-  unsigned long long st_pass = 0, st_push = 0, st_apply = 0, st_book = 0, st_idle_n = 0, st_idle = 0, st_max = 0,
-                     st_poll = 0;
-  const bool stats_on = P.stats != nullptr;
-
-  for (;;) {
-    bool sweep_any = false;   // (uniform over the CTA: s_any is read after a barrier)
-    for (int own = 0; own < n_own; ++own) {
-      const int item = blockIdx.x + own * gridDim.x;
-      const long long c0 = stats_on ? clock64() : 0;
-      uint32_t p_seq = 0, p_cnt = 0, p_taken = 0;   // warp 0: this lane's push seq, its worker's prefix, all taken
-      bool p_take = false;
-      if (warp == 0) {
-        uint32_t ready = 0, slot = 0;
-        if (pvalid) {
-          p_seq = s_next[own][pw] + pk;
-          slot = p_seq % P.nslots;
-          const uint32_t f = ld_acquire_scoped_u32(
-              P.flags + (static_cast<size_t>(pw) * P.nslots + slot) * P.n_flags + s_item[own].flag_index, P.gpu_scope);
-          ready = (f == p_seq) ? 1u : 0u;
-        }
-        const uint32_t b = __ballot_sync(0xffffffffu, ready);
-        if (pvalid)
-          while (p_cnt < static_cast<uint32_t>(kdepth) && ((b >> (p_cnt * nw + pw)) & 1u)) ++p_cnt;
-        p_take = pvalid && static_cast<uint32_t>(pk) < p_cnt;
-        p_taken = __ballot_sync(0xffffffffu, p_take);
-        if (p_take) {
-          const int pos = __popc(p_taken & ((1u << lane) - 1u));
-          s_pend[pos] = static_cast<uint64_t>(pw) * wstride + static_cast<uint64_t>(slot) * P.arena_elems;
-          s_round[pos] = pk;
-        }
-        if (lane == 0) {
-          s_any = p_taken;
-          s_npend = __popc(p_taken);
-        }
-      }
-      __syncthreads();
-      const long long c1 = stats_on ? clock64() : 0;
-      if (!s_any && stats_on) { ++st_idle_n; st_idle += c1 - c0; }
-      if (s_any) {
-        sweep_any = true;
-        const PsItemState st = s_state[own];
-        apply_item<kIeee>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend), use_resident ? &resident : nullptr);
-        __syncthreads();   // every thread's parameter stores precede warp 0's release operations below
-        const long long c2 = stats_on ? clock64() : 0;
-        if (stats_on) {
-          ++st_pass; st_push += s_npend; st_apply += c2 - c1; st_poll += c1 - c0;
-          st_max = max(st_max, static_cast<unsigned long long>(s_npend));
-        }
-        if (warp == 0) {
-          if (lane == 0) {
-            const uint32_t npush = __popc(p_taken);
-            const uint32_t rounds = (31u - __clz(p_taken)) / nw + 1u;   // lanes are round-major
-            const uint32_t nsteps = (P.apply_mode == APPLY_MERGED) ? rounds : npush;
-            PsItemState ns = st;
-            ns.t += nsteps;
-            for (uint32_t k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
-            s_state[own] = ns;
-            P.item_state[item] = ns;   // persisted for checkpoints / a relaunch (never read back in this loop)
-          }
-          if (p_take) {
-            const uint32_t slot = p_seq % P.nslots;
-            const uint32_t done = atomicAdd(&P.consumed[pw * P.nslots + slot], 1u) + 1u;
-            if (done == static_cast<uint32_t>(P.n_items)) {
-              // this worker's push `p_seq` is fully applied: one global step (reference DS:91,103)
-              P.consumed[pw * P.nslots + slot] = 0;
-              const uint32_t gs = atomicAdd(P.global_step, 1u) + 1u;
-              uint32_t* ib = P.inbox_table[pw];
-              if (ib != nullptr) {
-                red_max_relaxed_scoped_u32(ib + 1, gs, P.gpu_scope);
-                red_max_release_scoped_u32(ib, p_seq, P.gpu_scope);  // ack: the mailbox slot may be reused
-              }
-            }
-          }
-          if (pvalid && pk == 0 && p_cnt > 0) {
-            const uint32_t nx = p_seq + p_cnt;
-            s_next[own][pw] = nx;
-            P.next_seq[static_cast<size_t>(pw) * P.n_items + item] = nx;
-          }
-        }
-        if (stats_on) { __syncwarp(); st_book += clock64() - c2; }
-      }
-      __syncthreads();
-    }
-    // ---- exit protocol: host stop request, or every worker has left and all their pushes are applied ----
-    // (checked every 32nd poll round only: the check itself costs several system-scope loads, and the poll
-    //  loop's period is the PS's reaction latency)
-    if (tid == 0) {
-      uint32_t ex = 0;
-      // one-shot mode: everything that will ever be pushed was pushed before this launch (stream order), so a
-      // full sweep without work means the shard is up to date
-      if (P.oneshot && !sweep_any) ex = 1;
-      const bool check = !P.oneshot && (iter & 31u) == 0u;
-      if (check && *P.host_stop != 0u) ex = 1;
-      if (check && !ex) {
-        bool all_done = true;
-        for (int w = 0; w < P.n_workers && all_done; ++w) {
-          const uint32_t d = ld_acquire_sys_u32(P.worker_done + w);  // = last push seq + 1, 0 while active
-          if (d == 0) { all_done = false; break; }
-          if (d == kWorkerDead) continue;   // presumed dead: whatever it left half-pushed is dropped
-          for (int own = 0; own < n_own; ++own)
-            if (s_next[own][w] != d) { all_done = false; break; }
-        }
-        if (all_done) ex = 1;
-      }
-      s_exit = ex;
-    }
-    __syncthreads();
-    if (s_exit) break;
-    ++iter;
-  }
-  if (tid == 0) {
-    if (stats_on) {
-      unsigned long long* o = P.stats + static_cast<size_t>(blockIdx.x) * 8;
-      o[0] += st_pass; o[1] += st_push; o[2] += st_apply; o[3] += st_book; o[4] += st_idle_n; o[5] += st_idle;
-      o[6] = max(o[6], st_max); o[7] += st_poll;
-      P.stats[kPsStatsCtas * 8 + blockIdx.x] = sm_id();
-    }
-    atomicAdd(P.exit_counter, 1u);
-  }
+  constexpr int kFam = kFamAdamSgd;
+#include "ps_serve_body.cuh"
+}
+// Momentum / Adagrad / RMSProp: ps_serve_kernel<kOpt, kIeee>.
+template <int kOpt, bool kIeee>
+__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
+  constexpr int kFam = kOpt;
+#include "ps_serve_body.cuh"
 }
 
 // `cluster` > 1: the grid is launched as clusters of that many CTAs. The kernel has no cluster-scope code; the
@@ -402,8 +287,22 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = cluster > 1 ? 1 : 0;
-  if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<true>, p);
-  return cudaLaunchKernelEx(&cfg, ps_serve_kernel<false>, p);
+  switch (p.opt) {
+    case OPT_SGD:
+    case OPT_ADAM:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<false>, p);
+    case OPT_MOMENTUM:   // no square root: one instantiation serves both math modes
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_MOMENTUM, false>, p);
+    case OPT_ADAGRAD:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADAGRAD, true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADAGRAD, false>, p);
+    case OPT_RMSPROP:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, false>, p);
+    default:
+      return cudaErrorInvalidValue;
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -504,6 +403,11 @@ cudaError_t preload_ps_kernels() {
   cudaError_t e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<false>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, dense_apply_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, shadow_refresh_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, wait_ack_kernel)) != cudaSuccess) return e;

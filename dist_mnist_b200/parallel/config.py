@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import os
 from dataclasses import dataclass, asdict
+from typing import Optional, Tuple
 
 from .. import _native as N
 
@@ -15,30 +16,72 @@ def _env_flag(name: str, default: bool) -> bool:
     return default if v is None else v not in ("0", "", "false", "False")
 
 
+_NATIVE_KINDS = {"adam": N.OPT_ADAM, "sgd": N.OPT_SGD, "momentum": N.OPT_MOMENTUM, "adagrad": N.OPT_ADAGRAD,
+                 "rmsprop": N.OPT_RMSPROP}
+# the kinds after Adam / SGD: their slot buffers hold other state, so ps, chief and checkpoints must agree on the kind
+TF1_SLOT_KINDS = ("momentum", "adagrad", "rmsprop")
+# hyper-parameters beyond lr / beta1 / beta2 / eps, the kinds that use each, and the TF1 default per kind
+# (TF1's MomentumOptimizer has no default momentum; 0.9 here)
+_EXTRA_DEFAULTS = {
+    "momentum": {"momentum": 0.9, "rmsprop": 0.0},
+    "decay": {"rmsprop": 0.9},
+    "initial_accumulator_value": {"adagrad": 0.1},
+}
+
+
 @dataclass(frozen=True)
 class OptimizerConfig:
     """Reference: `tf.train.AdamOptimizer(FLAGS.learning_rate)` with TF defaults (DS:102); SGD is the
-    north-star "async-SGD" variant."""
-    kind: str = "adam"          # "adam" | "sgd"
+    north-star "async-SGD" variant. "momentum", "adagrad" and "rmsprop" are TF1's `MomentumOptimizer`,
+    `AdagradOptimizer` and (non-centered) `RMSPropOptimizer`, applied on the ps with the `training_ops` formulas.
+
+    A hyper-parameter left at None takes the kind's TF1 default; giving one that the kind does not use is an error."""
+    kind: str = "adam"          # "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop"
     lr: float = 1e-4            # --learning_rate default (DS:15)
     beta1: float = 0.9
     beta2: float = 0.999
-    eps: float = 1e-8
-    math: str = "fast"          # ps-side Adam arithmetic on the cuda backend: "fast" (MUFU sqrt / reciprocal, <= 2 ulp,
-                                # the measured configuration) | "ieee" (correctly rounded sqrt and divide, like TF's
-                                # ApplyAdam; ~4x the per-push apply cost). The cpu backend is always IEEE.
+    eps: Optional[float] = None   # Adam 1e-8 (also kept for the kinds without an epsilon), RMSProp 1e-10
+    math: str = "fast"          # ps-side arithmetic of every rule with a square root (Adam, Adagrad, RMSProp) on the
+                                # cuda backend: "fast" (MUFU, <= 2 ulp, the measured configuration) | "ieee" (correctly
+                                # rounded sqrt and divide, like TF's Apply* kernels; ~4x the per-push apply cost for
+                                # Adam). The cpu backend is always IEEE.
+    momentum: Optional[float] = None    # "momentum" (0.9), "rmsprop" (0.0)
+    use_nesterov: bool = False          # "momentum"
+    decay: Optional[float] = None       # "rmsprop" (0.9)
+    initial_accumulator_value: Optional[float] = None   # "adagrad" (0.1): Adagrad's slot starts here, not at 0
 
     def __post_init__(self):
         if self.math not in ("fast", "ieee"):
             raise ValueError(f"unknown adam math {self.math!r} (fast | ieee)")
+        if self.eps is None:
+            object.__setattr__(self, "eps", 1e-10 if self.kind == "rmsprop" else 1e-8)
+        for name, defaults in _EXTRA_DEFAULTS.items():
+            if getattr(self, name) is None:
+                object.__setattr__(self, name, defaults.get(self.kind))
+            elif self.kind not in defaults:
+                raise ValueError(f"optimizer {self.kind!r} has no hyper-parameter {name!r}")
+        if self.use_nesterov and self.kind != "momentum":
+            raise ValueError(f"use_nesterov applies to the momentum optimizer, not {self.kind!r}")
+        if self.kind == "adagrad" and not self.initial_accumulator_value > 0:
+            raise ValueError("initial_accumulator_value must be positive (Adagrad divides by its square root)")
 
     @property
     def native_kind(self) -> int:
-        if self.kind == "adam":
-            return N.OPT_ADAM
-        if self.kind == "sgd":
-            return N.OPT_SGD
-        raise ValueError(f"unknown optimizer {self.kind!r} (adam | sgd)")
+        if self.kind in _NATIVE_KINDS:
+            return _NATIVE_KINDS[self.kind]
+        raise ValueError(f"unknown optimizer {self.kind!r} ({' | '.join(_NATIVE_KINDS)})")
+
+    def slot_init(self) -> Tuple[float, float]:
+        """Initial values of the two slot buffers (adam_m, adam_v): Adagrad's accumulator starts at
+        initial_accumulator_value and RMSProp's ms at 1 (TF1's `ones_initializer`); every other slot at 0."""
+        if self.kind == "adagrad":
+            return 0.0, float(self.initial_accumulator_value)
+        if self.kind == "rmsprop":
+            return 0.0, 1.0
+        return 0.0, 0.0
+
+    def as_dict(self) -> dict:
+        return asdict(self)
 
 
 @dataclass(frozen=True)

@@ -124,6 +124,7 @@ class ParameterServer:
             "arena_elems": self.shard.arena_elems, "n_items": self.shard.n_items, "n_flags": self.shard.n_flags,
             "nslots": cfg.nslots, "engine": self.engine,
             "n_workers": self.n_workers, "owns_global_step": self.shard.owns_global_step,
+            "optimizer": opt.as_dict(),   # the chief initialises the slots for this rule (Worker.connect checks it)
         })
         self.rdv.put(f"ps/{task_index}/segment", desc)
 
@@ -169,6 +170,9 @@ class ParameterServer:
         P.oneshot = 0
         P.opt, P.apply_mode = opt.native_kind, cfg.native_apply_mode
         P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
+        P.momentum = opt.momentum or 0.0
+        P.decay = opt.decay or 0.0
+        P.nesterov = int(opt.use_nesterov)
         P.ieee_math = 1 if opt.math == "ieee" else 0
         P.mailbox, P.arena_elems = s.addr("mailbox"), sh.arena_elems
         P.flags, P.next_seq, P.consumed = s.addr("flags"), s.addr("next_seq"), s.addr("consumed")
@@ -384,6 +388,7 @@ class ParameterServer:
             "ctas": len(rows), "passes": tot[0], "pushes": tot[1],
             "pushes_per_pass": round(tot[1] / max(tot[0], 1), 2), "max_pushes_in_pass": max(r[6] for r in rows),
             "apply_us_per_pass": round(tot[2] / max(tot[0], 1) / mhz, 2),
+            "apply_cycles_per_push": round(tot[2] / max(tot[1], 1)),
             "bookkeeping_us_per_pass": round(tot[3] / max(tot[0], 1) / mhz, 2),
             "poll_us_per_working_pass": round(tot[7] / max(tot[0], 1) / mhz, 2),
             "idle_polls": tot[4], "idle_poll_us": round(tot[5] / max(tot[4], 1) / mhz, 2),

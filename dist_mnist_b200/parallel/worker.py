@@ -38,7 +38,7 @@ from ..models import mlp
 from ..models.mlp import MLPSpec
 from ..ops import gemm as gemm_ops
 from ..ops import head as head_ops
-from .config import MAX_SLOTS, EngineConfig, OptimizerConfig
+from .config import MAX_SLOTS, TF1_SLOT_KINDS, EngineConfig, OptimizerConfig
 from .peer_mem import Carver, Segment
 from .ps import CTRL_GLOBAL_STEP, CTRL_WORKER_DONE, serve_geometry
 from .sharding import FUSED_CLUSTER, ModelLayout, VarLayout, build_layout, dw_tile_n_for
@@ -169,6 +169,13 @@ class Worker:
             desc = self.rdv.get(f"ps/{k}/segment", timeout_s)
             if desc["nslots"] != cfg.nslots or desc["n_workers"] != self.cluster.num_workers:
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: {desc}")
+            # the ps applies the rule, the chief initialises its slots: with Momentum / Adagrad / RMSProp on either
+            # side both must run the same optimizer (an Adam / SGD pairing is not checked, as before)
+            ps_opt = desc.get("optimizer") or {}
+            if ((ps_opt.get("kind") in TF1_SLOT_KINDS or self.opt.kind in TF1_SLOT_KINDS)
+                    and ps_opt != self.opt.as_dict()):
+                raise RuntimeError(f"ps {k} was started with a different engine configuration: optimizer "
+                                   f"{ps_opt}, this worker has {self.opt.as_dict()}")
             sh = self.layout.shards[k]
             if (desc["arena_elems"] != sh.arena_elems or desc["n_items"] != sh.n_items
                     or desc.get("n_flags", sh.n_flags) != sh.n_flags or desc.get("engine", self.engine) != self.engine):
@@ -406,9 +413,9 @@ class Worker:
             raise RuntimeError("only the chief (worker 0) initialises variables")
         params = params if params is not None else mlp.init_params(self.spec, seed)
         self.write_variables(params)
-        zeros = {k: torch.zeros_like(v) for k, v in params.items()}
-        self.write_variables(zeros, "adam_m")
-        self.write_variables(zeros, "adam_v")
+        m0, v0 = self.opt.slot_init()   # Adagrad's accumulator and RMSProp's ms do not start at 0
+        self.write_variables({k: torch.full_like(v, m0) for k, v in params.items()}, "adam_m")
+        self.write_variables({k: torch.full_like(v, v0) for k, v in params.items()}, "adam_v")
         self.rdv.put("init/done", {"seed": seed, "by": self.task_index})
 
     def variables_are_live(self) -> bool:

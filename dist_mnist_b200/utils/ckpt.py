@@ -16,6 +16,8 @@ from typing import Optional
 
 import torch
 
+from ..parallel.config import TF1_SLOT_KINDS
+
 FORMAT_VERSION = 1
 
 
@@ -29,7 +31,9 @@ def save_checkpoint(worker, directory: str) -> str:
         "hidden": tuple(worker.spec.hidden),
         "global_step": gstep,
         "optimizer": {"kind": worker.opt.kind, "lr": worker.opt.lr, "beta1": worker.opt.beta1,
-                      "beta2": worker.opt.beta2, "eps": worker.opt.eps},
+                      "beta2": worker.opt.beta2, "eps": worker.opt.eps, "momentum": worker.opt.momentum,
+                      "use_nesterov": worker.opt.use_nesterov, "decay": worker.opt.decay,
+                      "initial_accumulator_value": worker.opt.initial_accumulator_value},
         "variables": worker.read_variables("params"),       # [out, in] layout, see models/mlp.py
         "adam_m": worker.read_variables("adam_m"),
         "adam_v": worker.read_variables("adam_v"),
@@ -75,6 +79,11 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
         raise RuntimeError(f"unsupported checkpoint format in {path}")
     if tuple(state["hidden"]) != tuple(worker.spec.hidden):
         raise RuntimeError(f"checkpoint {path} is for hidden={state['hidden']}, model has {worker.spec.hidden}")
+    # adam_m / adam_v hold a different optimizer's state under Momentum / Adagrad / RMSProp (TF fails on the missing
+    # slot variables in this case)
+    kind = state.get("optimizer", {}).get("kind")
+    if kind != worker.opt.kind and (kind in TF1_SLOT_KINDS or worker.opt.kind in TF1_SLOT_KINDS):
+        raise RuntimeError(f"checkpoint {path} holds {kind!r} optimizer slots, this run uses {worker.opt.kind!r}")
     worker.write_variables(state["variables"], "params")
     worker.write_variables(state["adam_m"], "adam_m")
     worker.write_variables(state["adam_v"], "adam_v")
