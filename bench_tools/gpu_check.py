@@ -9,6 +9,8 @@ mismatch so one GPU call yields the full picture:
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
+import struct
 import subprocess
 import sys
 import time
@@ -257,9 +259,10 @@ def check_accuracy() -> bool:
     return ok
 
 
-def check_ps_serve(ieee: bool = False) -> bool:
+def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0) -> bool:
     """Single-GPU test of the persistent PS kernel: mailboxes and inboxes are local buffers. `ieee`: the
-    `--adam_math ieee` instantiation (correctly rounded sqrt / divide)."""
+    `--adam_math ieee` instantiation (correctly rounded sqrt / divide). `schedule` (an LrSchedule): the scheduled
+    instantiations, every item starting at schedule step `sched_step`; the reference then runs in fp64."""
     from dist_mnist_b200 import _native as N
     ok = True
     dev = "cuda"
@@ -302,6 +305,7 @@ def check_ps_serve(ieee: bool = False) -> bool:
         st_host = (N.PsItemState * n_items)()
         for i in range(n_items):
             st_host[i].t, st_host[i].beta1_pow, st_host[i].beta2_pow = 0, 1.0, 1.0
+            st_host[i].sched_step = sched_step
         state.view(torch.uint8).view(-1).copy_(torch.frombuffer(bytearray(bytes(st_host)), dtype=torch.uint8).cuda())
         # gradients: worker w push s
         grads = torch.randn(n_workers, n_push, arena, device=dev) * 0.1
@@ -317,6 +321,8 @@ def check_ps_serve(ieee: bool = False) -> bool:
         P.n_flags = n_items
         P.lr, P.beta1, P.beta2, P.eps = 1e-2, 0.9, 0.999, 1e-8
         P.ieee_math = 1 if ieee else 0
+        if schedule is not None:
+            schedule.fill_native(P)
         P.mailbox, P.arena_elems = mailbox.data_ptr(), arena
         P.flags, P.next_seq, P.consumed = flags.data_ptr(), next_seq.data_ptr(), consumed.data_ptr()
         P.global_step, P.worker_done, P.host_stop = gstep.data_ptr(), done.data_ptr(), stop.data_ptr()
@@ -331,38 +337,63 @@ def check_ps_serve(ieee: bool = False) -> bool:
         for (off, r, c, l) in items:
             for rr in range(r):
                 mask_items[off + rr * l: off + rr * l + c] = True
-        pr, mr, vr = p0.clone(), torch.zeros_like(p0), torch.zeros_like(p0)
+        dt = torch.float32 if schedule is None else torch.float64
+        pr, mr, vr = p0.to(dt), torch.zeros_like(p0, dtype=dt), torch.zeros_like(p0, dtype=dt)
         t = 0
         for s in range(n_push):
-            group = [grads[w, s] for w in range(n_workers)]
-            steps = [sum(group)] if apply_mode == N.APPLY_MERGED else group
-            for gg in steps:
+            group = [grads[w, s].to(dt) for w in range(n_workers)]
+            # (gradient, position of its first push in the application order: round-major, workers in order)
+            steps = ([(sum(group), s * n_workers)] if apply_mode == N.APPLY_MERGED
+                     else [(g, s * n_workers + w) for w, g in enumerate(group)])
+            for gg, pos in steps:
                 t += 1
+                lr = P.lr if schedule is None else schedule.lr_at(sched_step + pos, P.lr)
                 if opt == N.OPT_SGD:
-                    pr = pr - P.lr * gg
+                    pr = pr - lr * gg
                 else:
                     mr = 0.9 * mr + 0.1 * gg
                     vr = 0.999 * vr + 0.001 * gg * gg
-                    lr_t = P.lr * (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
+                    lr_t = lr * (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
                     pr = pr - lr_t * mr / (vr.sqrt() + 1e-8)
-        pr = torch.where(mask_items, pr, p0)
+        pr = torch.where(mask_items, pr, p0.to(dt)).float()
         e = rel_err(params, pr)
         e_sh = rel_err(shadow.float()[mask_items], pr[mask_items].to(torch.bfloat16).float())
         gs = int(gstep.item())
         acks = inbox[:, 0].tolist()
         good = e < 1e-5 and gs == n_workers * n_push and acks == [n_push] * n_workers and e_sh < 1e-3
-        ok &= report(f"ps_serve opt={opt} mode={apply_mode} math={'ieee' if ieee else 'fast'}", good,
+        sched = ""
+        if schedule is not None:
+            steps_now = sorted({int(x) & 0xFFFFFFFF for x in state[:, 3].tolist()})
+            good &= steps_now == [(sched_step + n_workers * n_push) & 0xFFFFFFFF]
+            sched = f" schedule={schedule.kind} from={sched_step} sched_step={steps_now}"
+        ok &= report(f"ps_serve opt={opt} mode={apply_mode} math={'ieee' if ieee else 'fast'}{sched}", good,
                      f"param_err={e:.1e} shadow_err={e_sh:.1e} global_step={gs} acks={acks} exit={int(exitc.item())}")
     return ok
 
 
-def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
+def _ref_apply(opt, p, m, v, g, lr, t):
+    """One optimizer step of any kind at rate `lr` (Adam: its t-th step), on tensors in their own dtype."""
+    if opt.kind == "sgd":
+        return p - lr * g, m, v
+    if opt.kind == "adam":
+        # the kernel's fp32 hyper-parameters: 1 - fp32(0.999) is 1.3e-5 away from 0.001 (relative), more than the bound
+        b1, b2, eps = (struct.unpack("f", struct.pack("f", x))[0] for x in (opt.beta1, opt.beta2, opt.eps))
+        m = b1 * m + (1 - b1) * g
+        v = b2 * v + (1 - b2) * g * g
+        lr_t = lr * (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
+        return p - lr_t * m / (v.sqrt() + eps), m, v
+    from bench_tools.gpu_e2e import tf1_apply
+    return tf1_apply(dataclasses.replace(opt, lr=lr), p, m, v, g)
+
+
+def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step: int = 0) -> bool:
     """The serve kernel's Momentum / Adagrad / RMSProp instantiations (`opt`: an OptimizerConfig; `opt.math` picks the
     fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
     against the TF1 formulas in fp64 (parameters and both slot buffers within 1e-5 relative error; the bf16 shadow,
     global_step and the acks exact). `resident`: one pushed push per worker and pass (lookahead 1) and one vectorisable
-    item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass."""
-    from bench_tools.gpu_e2e import tf1_apply
+    item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass.
+    A non-constant `opt.schedule` runs the scheduled instantiation (Adam and SGD too), every item starting at schedule
+    step `sched_step`; the check then includes every item's final sched_step."""
     from dist_mnist_b200 import _native as N
     dev = "cuda"
     torch.manual_seed(6)
@@ -401,6 +432,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
     st_host = (N.PsItemState * n_items)()
     for i in range(n_items):
         st_host[i].t, st_host[i].beta1_pow, st_host[i].beta2_pow = 0, 1.0, 1.0
+        st_host[i].sched_step = sched_step
     state = torch.frombuffer(bytearray(bytes(st_host)), dtype=torch.uint8).to(dev)
     grads = torch.randn(n_workers, n_push, arena, device=dev) * 0.1
     for w in range(n_workers):
@@ -416,6 +448,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
     P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
     P.momentum, P.decay, P.nesterov = opt.momentum or 0.0, opt.decay or 0.0, int(opt.use_nesterov)
     P.ieee_math = 1 if opt.math == "ieee" else 0
+    opt.schedule.fill_native(P)
     P.lookahead = 1 if resident else 0
     P.mailbox, P.arena_elems = mailbox.data_ptr(), arena
     P.flags, P.next_seq, P.consumed = flags.data_ptr(), next_seq.data_ptr(), consumed.data_ptr()
@@ -434,10 +467,16 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
             mask[off + rr * l: off + rr * l + c] = True
     pr, mr, vr = p0.double(), torch.full((arena,), m0, dtype=torch.float64, device=dev), \
         torch.full((arena,), v0, dtype=torch.float64, device=dev)
+    # push w of round k sits at position k * n_workers + w of the application order and is applied at schedule step
+    # sched_step + that position; a merged round at the position of its first push
+    t = 0
     for s in range(n_push):
         group = [grads[w, s].double() for w in range(n_workers)]
-        for gg in ([sum(group)] if apply_mode == N.APPLY_MERGED else group):
-            pr, mr, vr = tf1_apply(opt, pr, mr, vr, gg)
+        steps = ([(sum(group), s * n_workers)] if apply_mode == N.APPLY_MERGED
+                 else [(g, s * n_workers + w) for w, g in enumerate(group)])
+        for gg, pos in steps:
+            t += 1
+            pr, mr, vr = _ref_apply(opt, pr, mr, vr, gg, opt.lr_at(sched_step + pos), t)
     pr, mr, vr = torch.where(mask, pr, p0.double()), torch.where(mask, mr, m0), torch.where(mask, vr, v0)
     e_p, e_m, e_v = rel_err(params, pr), rel_err(m, mr), rel_err(v, vr)
     shadow_exact = bool(torch.equal(shadow[mask], params[mask].to(torch.bfloat16)))
@@ -447,8 +486,14 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False) -> bool:
             and int(exitc.item()) == n_ctas)
     name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''} momentum={opt.momentum} math={opt.math} "
             f"mode={apply_mode} resident={resident}")
+    extra = ""
+    if not opt.schedule.constant:
+        steps_now = sorted({int(x) & 0xFFFFFFFF for x in state.view(torch.int32).view(n_items, 4)[:, 3].tolist()})
+        good &= steps_now == [(sched_step + n_workers * n_push) & 0xFFFFFFFF]
+        name += f" schedule={opt.schedule.kind} from={sched_step}"
+        extra = f" sched_step={steps_now}"
     return report(name, good, f"err p={e_p:.1e} m={e_m:.1e} v={e_v:.1e} shadow_exact={shadow_exact} global_step={gs} "
-                              f"acks={acks} exit={int(exitc.item())}")
+                              f"acks={acks} exit={int(exitc.item())}{extra}")
 
 
 def check_dense_apply() -> bool:

@@ -6,6 +6,7 @@
 """
 from __future__ import annotations
 
+import dataclasses
 import subprocess
 import sys
 import os
@@ -45,7 +46,10 @@ def ref_slots(opt, params):
     return ({k: torch.full_like(t, m0) for k, t in params.items()}, {k: torch.full_like(t, v0) for k, t in params.items()})
 
 
-def ref_step(spec, params, m, v, t, x, y, opt):
+def ref_step(spec, params, m, v, t, x, y, opt, lr=None):
+    """One reference training step in place; `lr`: this step's rate (a learning-rate schedule's), else opt.lr."""
+    if lr is not None:
+        opt = dataclasses.replace(opt, lr=lr)
     loss, grads, _ = mlp.manual_loss_and_grads(spec, params, x, y)
     t += 1
     for k in params:

@@ -7,7 +7,10 @@ counters off, as in bench.py), one with DM_PS_STATS=1 for the serve kernel's app
 (`ParameterServer.serve_stats()`). The card's name and power limit are read in the same call. One JSON line per
 optimizer, then a table.
 
-    python bench_tools/optimizer_apply.py [--steps 20000] [--warmup 50] [--only rmsprop,adam]
+`--lr_schedule KIND` measures every optimizer twice, under that learning-rate schedule (the scheduled serve kernels)
+and at a constant rate, alternated in the same call: the cost of the rate table the scheduled kernels build per pass.
+
+    python bench_tools/optimizer_apply.py [--steps 20000] [--warmup 50] [--only rmsprop,adam] [--lr_schedule KIND]
 """
 from __future__ import annotations
 
@@ -23,15 +26,28 @@ if ROOT not in sys.path:
 RULES = ["adam", "sgd", "momentum", "nesterov", "adagrad", "rmsprop"]
 
 
-def optimizer(rule: str, lr: float):
+def schedule(kind: str, lr: float):
+    """A schedule of `kind` that changes the rate many times within a measured run."""
+    from dist_mnist_b200.parallel.config import LrSchedule
+
+    if kind in ("exponential_decay", "inverse_time_decay", "natural_exp_decay"):
+        return LrSchedule(kind, decay_steps=1000, decay_rate=0.96)
+    if kind in ("polynomial_decay", "cosine_decay"):
+        return LrSchedule(kind, decay_steps=100000)
+    if kind == "piecewise_constant":
+        return LrSchedule(kind, boundaries=(5000, 10000), values=(lr, lr / 10, lr / 100))
+    return LrSchedule()
+
+
+def optimizer(rule: str, lr: float, sched: str = "constant"):
     from dist_mnist_b200.parallel.config import OptimizerConfig
 
     if rule == "nesterov":
-        return OptimizerConfig("momentum", lr, use_nesterov=True)
-    return OptimizerConfig(rule, lr)
+        return OptimizerConfig("momentum", lr, use_nesterov=True, schedule=schedule(sched, lr))
+    return OptimizerConfig(rule, lr, schedule=schedule(sched, lr))
 
 
-def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0) -> dict:
+def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0, sched: str = "constant") -> dict:
     """One cluster in the bench configuration: warm-up, then one timed run_resident region after a ps restart."""
     import torch
 
@@ -43,7 +59,7 @@ def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0) -> di
     args = bench.parse_args(["--gpus", "1"])
     spec = mlp.get_model(args.model, args.hidden_units)
     cfg = bench.engine_config(args)
-    opt = optimizer(rule, args.learning_rate)
+    opt = optimizer(rule, args.learning_rate, sched)
     torch.cuda.set_device(dev)
     ds = data_utils.synthetic_mnist(data_utils.TRAIN_SIZE, seed=0)
     dev_x = ds.images.to(torch.float32).to(f"cuda:{dev}").contiguous()
@@ -87,6 +103,8 @@ def main(argv=None) -> int:
     ap.add_argument("--steps", type=int, default=20000)
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--only", type=str, default="", help="comma-separated subset of " + ",".join(RULES))
+    ap.add_argument("--lr_schedule", type=str, default="constant",
+                    help="also run every optimizer under this learning-rate schedule, alternated with constant")
     a = ap.parse_args(argv)
     import torch
 
@@ -99,21 +117,29 @@ def main(argv=None) -> int:
     for r in rules:
         if r not in RULES:
             raise SystemExit(f"unknown rule {r!r} ({', '.join(RULES)})")
+    from dist_mnist_b200.parallel.config import LR_SCHEDULES
+    if a.lr_schedule not in LR_SCHEDULES:
+        raise SystemExit(f"unknown lr_schedule {a.lr_schedule!r} ({', '.join(LR_SCHEDULES)})")
+    scheds = [a.lr_schedule, "constant"] if a.lr_schedule != "constant" else ["constant"]
     card = card_info(0)
     rows = []
     for r in rules:
-        timed = run_one(r, a.steps, a.warmup, stats=False)
-        counted = run_one(r, a.steps, a.warmup, stats=True)
-        row = {"optimizer": r, **timed, "apply_cycles_per_push": counted.get("apply_cycles_per_push"),
-               "pushes_per_pass": counted.get("pushes_per_pass"), "ps_busy_fraction": counted.get("busy_fraction"),
-               "steps_per_s_with_counters": counted["steps_per_s"], "card": card}
-        rows.append(row)
-        print(json.dumps(row), flush=True)
-    print(f"card {card}; {a.steps} timed steps per optimizer")
-    print(f"{'optimizer':>10} {'steps/s':>9} {'apply cycles/push':>18} {'pushes/pass':>12} {'ps busy':>8}")
+        for sc in scheds:
+            timed = run_one(r, a.steps, a.warmup, stats=False, sched=sc)
+            counted = run_one(r, a.steps, a.warmup, stats=True, sched=sc)
+            row = {"optimizer": r, "lr_schedule": sc, **timed,
+                   "apply_cycles_per_push": counted.get("apply_cycles_per_push"),
+                   "pushes_per_pass": counted.get("pushes_per_pass"), "ps_busy_fraction": counted.get("busy_fraction"),
+                   "steps_per_s_with_counters": counted["steps_per_s"], "card": card}
+            rows.append(row)
+            print(json.dumps(row), flush=True)
+    print(f"card {card}; {a.steps} timed steps per optimizer and schedule")
+    print(f"{'optimizer':>10} {'lr_schedule':>18} {'steps/s':>9} {'apply cycles/push':>18} {'pushes/pass':>12} "
+          f"{'ps busy':>8}")
     for row in rows:
-        print(f"{row['optimizer']:>10} {row['steps_per_s']:>9} {str(row['apply_cycles_per_push']):>18} "
-              f"{str(row['pushes_per_pass']):>12} {str(row['ps_busy_fraction']):>8}")
+        print(f"{row['optimizer']:>10} {row['lr_schedule']:>18} {row['steps_per_s']:>9} "
+              f"{str(row['apply_cycles_per_push']):>18} {str(row['pushes_per_pass']):>12} "
+              f"{str(row['ps_busy_fraction']):>8}")
     return 0
 
 

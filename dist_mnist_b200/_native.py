@@ -26,6 +26,8 @@ LOSS_BOOK, LOSS_XENT = 0, 1
 OPT_SGD, OPT_ADAM, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3, 4
 APPLY_PER_PUSH, APPLY_MERGED = 0, 1
 DT_F32, DT_BF16 = 0, 1
+LR_CONSTANT, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_NATURAL_EXP, LR_POLYNOMIAL, LR_COSINE, LR_PIECEWISE = range(7)
+MAX_LR_BOUNDARIES = 8   # protocol.h kMaxLrBoundaries
 
 
 class PushTarget(C.Structure):
@@ -92,7 +94,7 @@ class PsItem(C.Structure):
 
 
 class PsItemState(C.Structure):
-    _fields_ = [("t", C.c_uint32), ("beta1_pow", C.c_float), ("beta2_pow", C.c_float), ("pad_", C.c_uint32)]
+    _fields_ = [("t", C.c_uint32), ("beta1_pow", C.c_float), ("beta2_pow", C.c_float), ("sched_step", C.c_uint32)]
 
 
 class PsServeParams(C.Structure):
@@ -111,6 +113,10 @@ class PsServeParams(C.Structure):
         ("oneshot", C.c_uint32), ("ieee_math", C.c_uint32),
         ("stats", C.c_void_p),
         ("momentum", C.c_float), ("decay", C.c_float), ("nesterov", C.c_uint32), ("pad_", C.c_uint32),
+        ("lr_schedule", C.c_int), ("decay_steps", C.c_uint32), ("decay_rate", C.c_float), ("end_lr", C.c_float),
+        ("power", C.c_float), ("alpha", C.c_float), ("staircase", C.c_uint32), ("cycle", C.c_uint32),
+        ("n_boundaries", C.c_int), ("boundaries", C.c_uint32 * MAX_LR_BOUNDARIES),
+        ("values", C.c_float * (MAX_LR_BOUNDARIES + 1)),
     ]
 
 

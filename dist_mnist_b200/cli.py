@@ -26,7 +26,7 @@ import torch
 
 from .cluster import ClusterSpec, Rendezvous, default_device_index
 from .models import mlp
-from .parallel.config import EngineConfig, OptimizerConfig
+from .parallel.config import LR_SCHEDULES, SCHEDULE_PARAMS, EngineConfig, LrSchedule, OptimizerConfig
 from .parallel.ps import ParameterServer
 from .parallel.worker import Worker
 from .session import train_loop
@@ -54,6 +54,44 @@ _OPT_FLAGS = {"momentum": ("momentum", "rmsprop"), "use_nesterov": ("momentum",)
               "initial_accumulator_value": ("adagrad",), "epsilon": ("adam", "rmsprop")}
 
 
+# learning-rate schedule flag -> LrSchedule parameter
+_SCHED_FLAGS = {"decay_steps": "decay_steps", "decay_rate": "decay_rate", "staircase": "staircase",
+                "end_learning_rate": "end_learning_rate", "power": "power", "cycle": "cycle", "alpha": "alpha",
+                "lr_boundaries": "boundaries", "lr_values": "values"}
+
+
+class _StoreLearningRate(argparse.Action):
+    """--learning_rate, remembering that it was given (piecewise_constant takes its rates from --lr_values)."""
+
+    def __call__(self, parser, namespace, values, option_string=None):
+        setattr(namespace, self.dest, values)
+        namespace.learning_rate_given = True
+
+
+def _int_list(text: str):
+    return tuple(int(x) for x in text.split(",") if x.strip())
+
+
+def _float_list(text: str):
+    return tuple(float(x) for x in text.split(",") if x.strip())
+
+
+def lr_schedule_from_args(args) -> LrSchedule:
+    """The learning-rate schedule of `--lr_schedule` and its parameters; a parameter flag the chosen schedule does not
+    use is an error, and so is --learning_rate with piecewise_constant."""
+    kind = args.lr_schedule
+    given = {flag: getattr(args, flag) for flag in _SCHED_FLAGS
+             if getattr(args, flag) is not None and getattr(args, flag) is not False}
+    for flag in given:
+        name = _SCHED_FLAGS[flag]
+        if kind not in SCHEDULE_PARAMS[name]:
+            raise ValueError(f"--{flag} does not apply to --lr_schedule {kind} "
+                             f"(only {', '.join(SCHEDULE_PARAMS[name])})")
+    if kind == "piecewise_constant" and getattr(args, "learning_rate_given", False):
+        raise ValueError("--lr_schedule piecewise_constant takes its rates from --lr_values, not --learning_rate")
+    return LrSchedule(kind, **{_SCHED_FLAGS[flag]: v for flag, v in given.items()})
+
+
 def optimizer_config_from_args(args) -> OptimizerConfig:
     """The optimizer every task derives from the command line; a hyper-parameter flag the chosen optimizer does not
     use is an error."""
@@ -62,7 +100,8 @@ def optimizer_config_from_args(args) -> OptimizerConfig:
             raise ValueError(f"--{flag} does not apply to --optimizer {args.optimizer} (only {', '.join(kinds)})")
     return OptimizerConfig(args.optimizer, args.learning_rate, eps=args.epsilon, math=args.adam_math,
                            momentum=args.momentum, use_nesterov=args.use_nesterov, decay=args.rmsprop_decay,
-                           initial_accumulator_value=args.initial_accumulator_value)
+                           initial_accumulator_value=args.initial_accumulator_value,
+                           schedule=lr_schedule_from_args(args))
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -75,7 +114,7 @@ def build_parser() -> argparse.ArgumentParser:
                    help="stop at this *global* step (reference: flag default 10000 is dead, hook hard-codes 4000)")
     p.add_argument("--batch_size", type=int, default=32,
                    help="per-worker batch (reference: flag default 100 is dead, next_batch(32) is hard-coded)")
-    p.add_argument("--learning_rate", type=float, default=0.0001)
+    p.add_argument("--learning_rate", type=float, default=0.0001, action=_StoreLearningRate)
     p.add_argument("--ps_hosts", type=str, default=None)
     p.add_argument("--worker_hosts", type=str, default=None)
     p.add_argument("--job_name", type=str, default=None, help="worker or ps")
@@ -94,6 +133,24 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--initial_accumulator_value", type=float, default=None,
                    help="adagrad: starting value of the accumulator (0.1)")
     p.add_argument("--epsilon", type=float, default=None, help="adam (1e-8) and rmsprop (1e-10)")
+    # learning-rate schedule over the global step (TF1's tf.train.*_decay / piecewise_constant), evaluated on the ps
+    # when a push is applied; a parameter flag the schedule does not use is an error
+    p.add_argument("--lr_schedule", choices=list(LR_SCHEDULES), default="constant",
+                   help="rate of a push at global step s, from lr0 = --learning_rate (constant: lr0)")
+    p.add_argument("--decay_steps", type=int, default=None,
+                   help="exponential / inverse_time / natural_exp / polynomial / cosine decay (required)")
+    p.add_argument("--decay_rate", type=float, default=None,
+                   help="exponential_decay / inverse_time_decay / natural_exp_decay (required)")
+    p.add_argument("--staircase", action="store_true",
+                   help="exponential / inverse_time / natural_exp decay: decay at whole multiples of decay_steps")
+    p.add_argument("--end_learning_rate", type=float, default=None, help="polynomial_decay (1e-4)")
+    p.add_argument("--power", type=float, default=None, help="polynomial_decay (1.0)")
+    p.add_argument("--cycle", action="store_true", help="polynomial_decay: restart past decay_steps")
+    p.add_argument("--alpha", type=float, default=None, help="cosine_decay: final rate as a fraction of lr0 (0.0)")
+    p.add_argument("--lr_boundaries", type=_int_list, default=None,
+                   help="piecewise_constant: 1..8 increasing global steps, e.g. 1000,2000")
+    p.add_argument("--lr_values", type=_float_list, default=None,
+                   help="piecewise_constant: one rate more than boundaries, e.g. 0.1,0.01,0.001")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")
@@ -217,7 +274,8 @@ def run(args: argparse.Namespace) -> int:
     metrics = None
     if args.metrics_file or args.log_steps_per_sec:
         metrics = TrainMetricsWriter(args.metrics_file, args.task_index, args.batch_size,
-                                     every_steps=max(1, args.log_every), echo=args.log_steps_per_sec)
+                                     every_steps=max(1, args.log_every), echo=args.log_steps_per_sec,
+                                     lr_at=None if opt.schedule.constant else opt.lr_at)
     try:
         res = train_loop(worker, dataset, train_steps=args.train_steps, log_every=args.log_every,
                          checkpoint_dir=args.checkpoint_dir, save_checkpoint_secs=args.save_checkpoint_secs,

@@ -23,6 +23,7 @@
 #include <string>
 #include <thread>
 
+#include "lr_schedule.h"
 #include "protocol.h"
 
 namespace {
@@ -48,17 +49,17 @@ struct CpuPs {
 };
 
 // TF1 Apply{Momentum,Adagrad,RMSProp} with IEEE arithmetic (ps_apply_sm90.cu tf1_step)
-void tf1_step_cpu(const dm::PsServeParams& P, float& p, float& m, float& v, float g) {
+void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, float& v, float g) {
   if (P.opt == dm::OPT_MOMENTUM) {
     m = P.momentum * m + g;
-    if (P.nesterov) p -= g * P.lr + m * P.momentum * P.lr;
-    else p -= P.lr * m;
+    if (P.nesterov) p -= g * lr + m * P.momentum * lr;
+    else p -= lr * m;
   } else if (P.opt == dm::OPT_ADAGRAD) {
     v += g * g;
-    p -= P.lr * g / std::sqrt(v);
+    p -= lr * g / std::sqrt(v);
   } else {   // OPT_RMSPROP
     v += (g * g - v) * (1.f - P.decay);
-    m = P.momentum * m + P.lr * g / std::sqrt(v + P.eps);
+    m = P.momentum * m + lr * g / std::sqrt(v + P.eps);
     p -= m;
   }
 }
@@ -69,6 +70,10 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
   const bool tf1 = P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
   const bool use_m = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_RMSPROP;
   const bool use_v = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
+  // rate of the k-th push of the pass (workers in order), lr(sched_step + k); a merged step uses lr(sched_step)
+  float lrs[dm::kMaxWorkers];
+  for (int k = 0; k < __builtin_popcount(mask); ++k)
+    lrs[k] = P.lr_schedule == dm::LR_CONSTANT ? P.lr : dm::scheduled_lr(P, st.sched_step + k);
   for (int r = 0; r < it.rows; ++r) {
     for (int c = 0; c < it.cols; ++c) {
       const uint64_t a = it.offset + static_cast<uint64_t>(r) * it.ld + c;
@@ -79,35 +84,38 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
       float b1p = st.beta1_pow, b2p = st.beta2_pow;
       float gsum = 0.f;
       uint32_t mm = mask;
+      int k = 0;
       while (mm) {
         const int w = __builtin_ffs(mm) - 1;
         mm &= mm - 1;
         const uint32_t slot = seqs[w] % P.nslots;
         const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
         if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
+        const float lr = lrs[k++];
         if (tf1) {
-          tf1_step_cpu(P, p, m, v, g);
+          tf1_step_cpu(P, lr, p, m, v, g);
         } else if (P.opt == dm::OPT_ADAM) {
           b1p *= P.beta1; b2p *= P.beta2;
-          const float lr_t = P.lr * std::sqrt(1.f - b2p) / (1.f - b1p);
+          const float lr_t = lr * std::sqrt(1.f - b2p) / (1.f - b1p);
           m = P.beta1 * m + (1.f - P.beta1) * g;
           v = P.beta2 * v + (1.f - P.beta2) * g * g;
           p -= lr_t * m / (std::sqrt(v) + P.eps);
         } else {
-          p -= P.lr * g;
+          p -= lr * g;
         }
       }
       if (P.apply_mode == dm::APPLY_MERGED) {
+        const float lr = lrs[0];
         if (tf1) {
-          tf1_step_cpu(P, p, m, v, gsum);
+          tf1_step_cpu(P, lr, p, m, v, gsum);
         } else if (P.opt == dm::OPT_ADAM) {
           b1p *= P.beta1; b2p *= P.beta2;
-          const float lr_t = P.lr * std::sqrt(1.f - b2p) / (1.f - b1p);
+          const float lr_t = lr * std::sqrt(1.f - b2p) / (1.f - b1p);
           m = P.beta1 * m + (1.f - P.beta1) * gsum;
           v = P.beta2 * v + (1.f - P.beta2) * gsum * gsum;
           p -= lr_t * m / (std::sqrt(v) + P.eps);
         } else {
-          p -= P.lr * gsum;
+          p -= lr * gsum;
         }
       }
       P.params[a] = p;
@@ -143,6 +151,7 @@ void serve_loop(CpuPs* ps) {
       dm::PsItemState ns = st;
       ns.t += nsteps;
       for (int k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
+      if (P.lr_schedule != dm::LR_CONSTANT) ns.sched_step += npush;   // one schedule step per push, both apply modes
       P.item_state[item] = ns;
       uint32_t mm = mask;
       while (mm) {

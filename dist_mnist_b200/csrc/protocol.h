@@ -143,7 +143,8 @@ struct PsItemState {  // persisted across serve-kernel launches and checkpointed
   uint32_t t;        // number of pushes applied to this item (Adam step count)
   float beta1_pow;
   float beta2_pow;
-  uint32_t pad_;
+  uint32_t sched_step;  // learning-rate schedule step: pushes applied to this item under a non-constant schedule
+                        // (set to the restored global_step by a checkpoint restore)
 };
 
 // TF1 `training_ops` rules applied per push (or per round, APPLY_MERGED). Slot buffers: adam_m = Adam m / momentum
@@ -153,6 +154,8 @@ enum ApplyMode : int {
   APPLY_PER_PUSH = 0,  // reference semantics: every worker push is its own optimizer step
   APPLY_MERGED = 1,    // pushes that are ready at the same poll are summed and applied as one step
 };
+
+constexpr int kMaxLrBoundaries = 8;   // PsServeParams::boundaries (piecewise_constant)
 
 struct PsServeParams {
   float* params;
@@ -197,6 +200,28 @@ struct PsServeParams {
   float decay;                 // OPT_RMSPROP (TF1 `decay`, rho)
   uint32_t nesterov;           // OPT_MOMENTUM: 1 = use_nesterov
   uint32_t pad_;
+  // learning-rate schedule (TF1 tf.train.*_decay / piecewise_constant; appended, so that no earlier field moves).
+  // The rate of a push is lr(s), s = the item's PsItemState::sched_step when the push is applied; `lr` above is lr0.
+  int lr_schedule;             // LrScheduleKind; LR_CONSTANT runs the unscheduled instantiations
+  uint32_t decay_steps;        // > 0 for every decay schedule
+  float decay_rate;            // exponential / inverse_time / natural_exp
+  float end_lr;                // polynomial: end_learning_rate
+  float power;                 // polynomial
+  float alpha;                 // cosine: floor of the rate as a fraction of lr0
+  uint32_t staircase;          // exponential / inverse_time / natural_exp: p = floor(s / decay_steps)
+  uint32_t cycle;              // polynomial
+  int n_boundaries;            // piecewise: 1 .. kMaxLrBoundaries
+  uint32_t boundaries[kMaxLrBoundaries];  // piecewise: strictly increasing steps
+  float values[kMaxLrBoundaries + 1];     // piecewise: n_boundaries + 1 rates
+};
+enum LrScheduleKind : int {
+  LR_CONSTANT = 0,
+  LR_EXPONENTIAL = 1,
+  LR_INVERSE_TIME = 2,
+  LR_NATURAL_EXP = 3,
+  LR_POLYNOMIAL = 4,
+  LR_COSINE = 5,
+  LR_PIECEWISE = 6,
 };
 constexpr int kPsStatsCtas = 160;
 

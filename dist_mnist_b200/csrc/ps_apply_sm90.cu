@@ -13,6 +13,7 @@
 // are consumed in order per item; different workers interleave arbitrarily (Hogwild, like the reference's
 // unlocked async apply).
 #include "common.cuh"
+#include "lr_schedule.h"
 #include "protocol.h"
 
 namespace dm {
@@ -64,22 +65,25 @@ __device__ __forceinline__ float div_sqrt(float a, float x) {   // a / sqrt(x)
   if constexpr (kIeee) return __fdiv_rn(a, __fsqrt_rn(x));
   else return a * rsqrt_approx(x);
 }
-template <int kOpt, bool kIeee>
-__device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, const PsServeParams& P) {
+// kSched: the step's rate is `lr_sched`; else P.lr (read from the parameter block as the measured instantiations do)
+template <int kOpt, bool kIeee, bool kSched>
+__device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, const PsServeParams& P,
+                                         const float& lr_sched) {
+  const float& lr = kSched ? lr_sched : P.lr;
   if constexpr (kOpt == OPT_MOMENTUM) {
     // accum <- momentum accum + g ; p <- p - lr accum  (Nesterov: p <- p - lr g - lr momentum accum)
     m = fmaf(P.momentum, m, g);
-    if (P.nesterov) p = p - fmaf(g, P.lr, m * P.momentum * P.lr);
-    else p = fmaf(-P.lr, m, p);
+    if (P.nesterov) p = p - fmaf(g, lr, m * P.momentum * lr);
+    else p = fmaf(-lr, m, p);
   } else if constexpr (kOpt == OPT_ADAGRAD) {
     // accum <- accum + g^2 ; p <- p - lr g / sqrt(accum)   (no epsilon)
     v = fmaf(g, g, v);
-    p = p - div_sqrt<kIeee>(P.lr * g, v);
+    p = p - div_sqrt<kIeee>(lr * g, v);
   } else {
     static_assert(kOpt == OPT_RMSPROP, "unknown optimizer family");
     // ms <- ms + (g^2 - ms)(1 - decay) ; mom <- momentum mom + lr g / sqrt(ms + eps) ; p <- p - mom
     v = fmaf(fmaf(g, g, -v), 1.f - P.decay, v);
-    m = fmaf(P.momentum, m, div_sqrt<kIeee>(P.lr * g, v + P.eps));
+    m = fmaf(P.momentum, m, div_sqrt<kIeee>(lr * g, v + P.eps));
     p = p - m;
   }
 }
@@ -102,9 +106,12 @@ struct ResidentState {
   bool loaded;
 };
 
-template <bool kIeee, int kFam>
+// kSched (the scheduled instantiations): the rate of the optimizer step whose pushes sit at positions i0..i1 of the
+// application order is s_lr[i0], the pass's rate table (lr(sched_step + i), built by the serve loop); else P.lr.
+template <bool kIeee, int kFam, bool kSched = false>
 __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItemState st, const uint64_t* s_pend,
-                           const uint32_t* s_round, const int n_pend, ResidentState* res = nullptr) {
+                           const uint32_t* s_round, const int n_pend, ResidentState* res = nullptr,
+                           const float* s_lr = nullptr) {
   const int tid = threadIdx.x;
   const int total = it.rows * it.cols;
   const bool vec = ((it.cols & 3) == 0) && ((it.ld & 3) == 0) && ((it.offset & 3) == 0);
@@ -163,8 +170,11 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
       for (int j = 0; j < 4; ++j) gsum[q][j] = 0.f;
 
-    // the other families' straight-line update keeps more values live: a chunk of 8 spills there, 7 does not
-    constexpr int kCh = kFam == kFamAdamSgd ? kChunk : kChunk - 1;
+    // the other families' straight-line update keeps more values live: a chunk of 8 spills there, 7 does not. The
+    // scheduled Adam / SGD instantiations (rate-table read, round start) spill at 8 too, and the IEEE one still at 7:
+    // 7 and 6 there; the scheduled Momentum / Adagrad / RMSProp ones do not spill at 7.
+    constexpr int kCh = kFam != kFamAdamSgd ? kChunk - 1 : !kSched ? kChunk : kIeee ? kChunk - 2 : kChunk - 1;
+    int r0 = 0;   // kSched, merged: position of the first push of the current round
     for (int i0 = 0; i0 < n_pend; i0 += kCh) {
       float g[kCh][kQuads][4];
 #pragma unroll
@@ -196,11 +206,16 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
           do_step = (i + 1 == n_pend) || (s_round[i + 1] != s_round[i]);   // last push of its round
         }
         if (!do_step) continue;
-        float lr_t = P.lr;
+        float lr = P.lr;
+        if constexpr (kSched) {
+          lr = s_lr[merged ? r0 : i];
+          r0 = i + 1;
+        }
+        float lr_t = lr;
         if (adam) {
           b1p *= P.beta1;
           b2p *= P.beta2;
-          lr_t = adam_lr_t<kIeee>(P.lr, b1p, b2p);
+          lr_t = adam_lr_t<kIeee>(lr, b1p, b2p);
         }
 #pragma unroll
         for (int q = 0; q < kQuads; ++q) {
@@ -208,9 +223,9 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
           for (int j = 0; j < 4; ++j) {
             if (j >= step) continue;
             const float gv = merged ? gsum[q][j] : g[ci][q][j];
-            if constexpr (kFam != kFamAdamSgd) tf1_step<kFam, kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, P);
+            if constexpr (kFam != kFamAdamSgd) tf1_step<kFam, kIeee, kSched>(pv[q][j], mv[q][j], vv[q][j], gv, P, lr);
             else if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, lr_t, P.beta1, P.beta2, P.eps);
-            else pv[q][j] = fmaf(-P.lr, gv, pv[q][j]);
+            else pv[q][j] = fmaf(-lr, gv, pv[q][j]);
             if (merged) gsum[q][j] = 0.f;
           }
         }
@@ -256,12 +271,22 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 template <bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kFamAdamSgd;
+  constexpr bool kSched = false;
 #include "ps_serve_body.cuh"
 }
 // Momentum / Adagrad / RMSProp: ps_serve_kernel<kOpt, kIeee>.
 template <int kOpt, bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kOpt;
+  constexpr bool kSched = false;
+#include "ps_serve_body.cuh"
+}
+// Any family under a non-constant learning-rate schedule (P.lr_schedule != LR_CONSTANT): ps_serve_sched_kernel<kFam,
+// kIeee>. Separate instantiations keep the seven above, and with them every constant-rate run, exactly as measured.
+template <int kFamT, bool kIeee>
+__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_sched_kernel(const __grid_constant__ PsServeParams P) {
+  constexpr int kFam = kFamT;
+  constexpr bool kSched = true;
 #include "ps_serve_body.cuh"
 }
 
@@ -287,6 +312,24 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = cluster > 1 ? 1 : 0;
+  if (p.lr_schedule != LR_CONSTANT) {
+    switch (p.opt) {
+      case OPT_SGD:
+      case OPT_ADAM:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<kFamAdamSgd, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<kFamAdamSgd, false>, p);
+      case OPT_MOMENTUM:
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_MOMENTUM, false>, p);
+      case OPT_ADAGRAD:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADAGRAD, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADAGRAD, false>, p);
+      case OPT_RMSPROP:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, false>, p);
+      default:
+        return cudaErrorInvalidValue;
+    }
+  }
   switch (p.opt) {
     case OPT_SGD:
     case OPT_ADAM:
@@ -408,6 +451,13 @@ cudaError_t preload_ps_kernels() {
   if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<kFamAdamSgd, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<kFamAdamSgd, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, dense_apply_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, shadow_refresh_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, wait_ack_kernel)) != cudaSuccess) return e;

@@ -1,7 +1,8 @@
 // Body of ps_serve_kernel, included once per kernel template (ps_apply_sm90.cu): it expects the kernel parameter
-// block `P` and the compile-time `kIeee` (correctly rounded sqrt / divide) and `kFam` (optimizer family) in scope.
-// A shared device function called by both kernels would give the Adam / SGD instantiations different SASS from
-// the one that was measured; included textually they compile exactly as before.
+// block `P` and the compile-time `kIeee` (correctly rounded sqrt / divide), `kFam` (optimizer family) and `kSched`
+// (non-constant learning-rate schedule) in scope. A shared device function called by both kernels would give the
+// Adam / SGD instantiations different SASS from the one that was measured; included textually they compile exactly
+// as before. Everything a schedule adds sits behind `if constexpr (kSched)`.
   // Everything the poll loop needs about this CTA's items lives in shared memory: the only global traffic of an
   // idle poll is one acquire load of a flag word per (worker, look-ahead slot).
   __shared__ PsItem s_item[kMaxOwn];
@@ -12,6 +13,7 @@
   __shared__ uint32_t s_npend;
   __shared__ uint32_t s_any;
   __shared__ uint32_t s_exit;
+  __shared__ float s_lr[kMaxPending];   // kSched: rate of the pass's i-th push, lr(sched_step + i)
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int warp = tid >> 5;
@@ -86,6 +88,11 @@
           s_any = p_taken;
           s_npend = __popc(p_taken);
         }
+        if constexpr (kSched) {
+          // the pass's rate table (one fp32 evaluation per lane): the i-th push of the application order is applied
+          // at schedule step sched_step + i; published to apply_item by the barrier below
+          if (lane < __popc(p_taken)) s_lr[lane] = scheduled_lr(P, s_state[own].sched_step + lane);
+        }
       }
       __syncthreads();
       const long long c1 = stats_on ? clock64() : 0;
@@ -93,8 +100,12 @@
       if (s_any) {
         sweep_any = true;
         const PsItemState st = s_state[own];
-        apply_item<kIeee, kFam>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
-                                use_resident ? &resident : nullptr);
+        if constexpr (kSched)
+          apply_item<kIeee, kFam, true>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
+                                        use_resident ? &resident : nullptr, s_lr);
+        else
+          apply_item<kIeee, kFam>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
+                                  use_resident ? &resident : nullptr);
         __syncthreads();   // every thread's parameter stores precede warp 0's release operations below
         const long long c2 = stats_on ? clock64() : 0;
         if (stats_on) {
@@ -109,6 +120,7 @@
             PsItemState ns = st;
             ns.t += nsteps;
             for (uint32_t k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
+            if constexpr (kSched) ns.sched_step += npush;   // one schedule step per push, in both apply modes
             s_state[own] = ns;
             P.item_state[item] = ns;   // persisted for checkpoints / a relaunch (never read back in this loop)
           }

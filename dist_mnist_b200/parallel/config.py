@@ -1,7 +1,9 @@
 """Engine configuration shared by ps and worker tasks."""
 from __future__ import annotations
 
+import math
 import os
+import struct
 from dataclasses import dataclass, asdict
 from typing import Optional, Tuple
 
@@ -29,6 +31,148 @@ _EXTRA_DEFAULTS = {
 }
 
 
+_NATIVE_SCHEDULES = {"constant": N.LR_CONSTANT, "exponential_decay": N.LR_EXPONENTIAL,
+                     "inverse_time_decay": N.LR_INVERSE_TIME, "natural_exp_decay": N.LR_NATURAL_EXP,
+                     "polynomial_decay": N.LR_POLYNOMIAL, "cosine_decay": N.LR_COSINE,
+                     "piecewise_constant": N.LR_PIECEWISE}
+LR_SCHEDULES = tuple(_NATIVE_SCHEDULES)
+_DECAY3 = ("exponential_decay", "inverse_time_decay", "natural_exp_decay")
+# schedule parameter -> the schedules that use it
+SCHEDULE_PARAMS = {
+    "decay_steps": _DECAY3 + ("polynomial_decay", "cosine_decay"),
+    "decay_rate": _DECAY3,
+    "staircase": _DECAY3,
+    "end_learning_rate": ("polynomial_decay",),
+    "power": ("polynomial_decay",),
+    "cycle": ("polynomial_decay",),
+    "alpha": ("cosine_decay",),
+    "boundaries": ("piecewise_constant",),
+    "values": ("piecewise_constant",),
+}
+_SCHEDULE_DEFAULTS = {"end_learning_rate": 1e-4, "power": 1.0, "alpha": 0.0}   # TF1's defaults
+
+
+@dataclass(frozen=True)
+class LrSchedule:
+    """TF1's `tf.train.*_decay(learning_rate, global_step, ...)` / `piecewise_constant(global_step, ...)` on the ps.
+
+    The rate of a push is `lr_at(s, lr0)` for the number `s` of pushes its item had already applied (the global step at
+    apply time; `lr0` is the optimizer's `lr`). A parameter left at None takes TF1's default; one that the kind does not
+    use is an error. The ps evaluates the rate in fp32; `lr_at` is the fp64 reference of that, rounded once to fp32."""
+    kind: str = "constant"
+    decay_steps: Optional[int] = None
+    decay_rate: Optional[float] = None
+    staircase: bool = False
+    end_learning_rate: Optional[float] = None
+    power: Optional[float] = None
+    cycle: bool = False
+    alpha: Optional[float] = None
+    boundaries: Optional[Tuple[int, ...]] = None
+    values: Optional[Tuple[float, ...]] = None
+
+    def __post_init__(self):
+        if self.kind not in _NATIVE_SCHEDULES:
+            raise ValueError(f"unknown lr_schedule {self.kind!r} ({' | '.join(LR_SCHEDULES)})")
+        for name, kinds in SCHEDULE_PARAMS.items():
+            v = getattr(self, name)
+            if v is not None and v is not False and self.kind not in kinds:
+                raise ValueError(f"lr_schedule {self.kind!r} has no parameter {name!r}")
+            if self.kind in kinds and getattr(self, name) is None and name in _SCHEDULE_DEFAULTS:
+                object.__setattr__(self, name, _SCHEDULE_DEFAULTS[name])
+        if self.boundaries is not None:
+            object.__setattr__(self, "boundaries", tuple(int(b) for b in self.boundaries))
+        if self.values is not None:
+            object.__setattr__(self, "values", tuple(float(v) for v in self.values))
+        k = self.kind
+        if k in SCHEDULE_PARAMS["decay_steps"]:
+            if self.decay_steps is None or int(self.decay_steps) != self.decay_steps or not 0 < self.decay_steps < 2 ** 32:
+                raise ValueError(f"lr_schedule {k!r} needs an integer decay_steps in [1, 2^32)")
+            object.__setattr__(self, "decay_steps", int(self.decay_steps))
+        if k in _DECAY3 and (self.decay_rate is None or not math.isfinite(self.decay_rate)):
+            raise ValueError(f"lr_schedule {k!r} needs a decay_rate")
+        if k == "polynomial_decay" and not (math.isfinite(self.end_learning_rate) and math.isfinite(self.power)):
+            raise ValueError("polynomial_decay needs a finite end_learning_rate and power")
+        if k == "cosine_decay" and not math.isfinite(self.alpha):
+            raise ValueError("cosine_decay needs a finite alpha")
+        if k == "piecewise_constant":
+            b, v = self.boundaries, self.values
+            if not b or len(b) > N.MAX_LR_BOUNDARIES:
+                raise ValueError(f"piecewise_constant needs 1..{N.MAX_LR_BOUNDARIES} boundaries")
+            if any(x < 0 or x >= 2 ** 32 for x in b) or any(b[i] >= b[i + 1] for i in range(len(b) - 1)):
+                raise ValueError("piecewise_constant boundaries must be strictly increasing steps in [0, 2^32)")
+            if v is None or len(v) != len(b) + 1:
+                raise ValueError("piecewise_constant needs len(boundaries) + 1 values")
+
+    @property
+    def native_kind(self) -> int:
+        return _NATIVE_SCHEDULES[self.kind]
+
+    @property
+    def constant(self) -> bool:
+        return self.kind == "constant"
+
+    def lr_at(self, step: int, lr0: float) -> float:
+        """The rate at step `step`: TF1's formula in fp64 (the step ratio is exact), rounded once to fp32."""
+        s, k = int(step), self.kind
+        if k == "piecewise_constant":
+            i = 0
+            while i < len(self.boundaries) and s > self.boundaries[i]:
+                i += 1
+            return _f32(self.values[i])
+        if k == "constant":
+            return _f32(lr0)
+        d = self.decay_steps
+        if k in _DECAY3:
+            p = float(s // d) if self.staircase else s / d
+            if k == "exponential_decay":
+                r = lr0 * self.decay_rate ** p
+            elif k == "inverse_time_decay":
+                r = lr0 / (1.0 + self.decay_rate * p)
+            else:
+                r = lr0 * math.exp(-self.decay_rate * p)
+        elif k == "polynomial_decay":
+            if self.cycle:
+                sp, dp = s, d * max(1, -(-s // d))
+            else:
+                sp, dp = min(s, d), d
+            r = (lr0 - self.end_learning_rate) * (1.0 - sp / dp) ** self.power + self.end_learning_rate
+        else:   # cosine_decay
+            f = min(s, d) / d
+            r = lr0 * ((1.0 - self.alpha) * 0.5 * (1.0 + math.cos(math.pi * f)) + self.alpha)
+        return _f32(r)
+
+    def fill_native(self, P) -> None:
+        """Write this schedule into a PsServeParams."""
+        P.lr_schedule = self.native_kind
+        P.decay_steps = int(self.decay_steps or 0)
+        P.decay_rate = self.decay_rate or 0.0
+        P.end_lr = self.end_learning_rate or 0.0
+        P.power = self.power or 0.0
+        P.alpha = self.alpha or 0.0
+        P.staircase, P.cycle = int(self.staircase), int(self.cycle)
+        b, v = self.boundaries or (), self.values or ()
+        P.n_boundaries = len(b)
+        for i, x in enumerate(b):
+            P.boundaries[i] = x
+        for i, x in enumerate(v):
+            P.values[i] = x
+
+    def as_dict(self) -> dict:
+        d = asdict(self)
+        for name in ("boundaries", "values"):   # JSON-shaped (rendezvous descriptors, checkpoints)
+            if d[name] is not None:
+                d[name] = list(d[name])
+        return d
+
+    @classmethod
+    def from_dict(cls, d: Optional[dict]) -> "LrSchedule":
+        return cls(**d) if d else cls()
+
+
+def _f32(x: float) -> float:
+    return struct.unpack("f", struct.pack("f", x))[0]
+
+
 @dataclass(frozen=True)
 class OptimizerConfig:
     """Reference: `tf.train.AdamOptimizer(FLAGS.learning_rate)` with TF defaults (DS:102); SGD is the
@@ -49,6 +193,7 @@ class OptimizerConfig:
     use_nesterov: bool = False          # "momentum"
     decay: Optional[float] = None       # "rmsprop" (0.9)
     initial_accumulator_value: Optional[float] = None   # "adagrad" (0.1): Adagrad's slot starts here, not at 0
+    schedule: LrSchedule = LrSchedule()   # learning-rate schedule over the global step (default: constant `lr`)
 
     def __post_init__(self):
         if self.math not in ("fast", "ieee"):
@@ -64,6 +209,12 @@ class OptimizerConfig:
             raise ValueError(f"use_nesterov applies to the momentum optimizer, not {self.kind!r}")
         if self.kind == "adagrad" and not self.initial_accumulator_value > 0:
             raise ValueError("initial_accumulator_value must be positive (Adagrad divides by its square root)")
+        if not isinstance(self.schedule, LrSchedule):
+            raise ValueError(f"schedule must be an LrSchedule, got {type(self.schedule).__name__}")
+
+    def lr_at(self, step: int) -> float:
+        """The learning rate of a push applied at global step `step` (LrSchedule.lr_at with lr0 = lr)."""
+        return self.schedule.lr_at(step, self.lr)
 
     @property
     def native_kind(self) -> int:
@@ -81,7 +232,9 @@ class OptimizerConfig:
         return 0.0, 0.0
 
     def as_dict(self) -> dict:
-        return asdict(self)
+        d = asdict(self)
+        d["schedule"] = self.schedule.as_dict()
+        return d
 
 
 @dataclass(frozen=True)
@@ -149,6 +302,9 @@ class EngineConfig:
         if self.push_mode == "atomic":
             if opt.kind != "sgd":
                 raise ValueError("push_mode='atomic' fuses the push with an SGD apply (red.add); use --optimizer sgd")
+            if not opt.schedule.constant:
+                raise ValueError("push_mode='atomic' folds a constant -lr into the worker's push; a learning-rate "
+                                 "schedule needs push_mode='mailbox'")
             if self.dtype != "fp32":
                 raise ValueError("push_mode='atomic' updates only the fp32 master copy; use dtype fp32")
             if self.backend != "cuda":

@@ -173,6 +173,7 @@ class ParameterServer:
         P.momentum = opt.momentum or 0.0
         P.decay = opt.decay or 0.0
         P.nesterov = int(opt.use_nesterov)
+        opt.schedule.fill_native(P)   # non-constant: the scheduled serve kernels / the cpu loop's rate table
         P.ieee_math = 1 if opt.math == "ieee" else 0
         P.mailbox, P.arena_elems = s.addr("mailbox"), sh.arena_elems
         P.flags, P.next_seq, P.consumed = s.addr("flags"), s.addr("next_seq"), s.addr("consumed")

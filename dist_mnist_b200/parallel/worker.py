@@ -38,7 +38,7 @@ from ..models import mlp
 from ..models.mlp import MLPSpec
 from ..ops import gemm as gemm_ops
 from ..ops import head as head_ops
-from .config import MAX_SLOTS, TF1_SLOT_KINDS, EngineConfig, OptimizerConfig
+from .config import MAX_SLOTS, TF1_SLOT_KINDS, EngineConfig, LrSchedule, OptimizerConfig
 from .peer_mem import Carver, Segment
 from .ps import CTRL_GLOBAL_STEP, CTRL_WORKER_DONE, serve_geometry
 from .sharding import FUSED_CLUSTER, ModelLayout, VarLayout, build_layout, dw_tile_n_for
@@ -176,6 +176,12 @@ class Worker:
                     and ps_opt != self.opt.as_dict()):
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: optimizer "
                                    f"{ps_opt}, this worker has {self.opt.as_dict()}")
+            # the ps evaluates the learning-rate schedule; a worker that reports lr_at(global_step) must agree on it
+            ps_sched = LrSchedule.from_dict(ps_opt.get("schedule"))
+            if ps_sched != self.opt.schedule or (not ps_sched.constant and ps_opt.get("lr") != self.opt.lr):
+                raise RuntimeError(f"ps {k} was started with a different engine configuration: learning-rate "
+                                   f"schedule {ps_sched} lr={ps_opt.get('lr')}, this worker has {self.opt.schedule} "
+                                   f"lr={self.opt.lr}")
             sh = self.layout.shards[k]
             if (desc["arena_elems"] != sh.arena_elems or desc["n_items"] != sh.n_items
                     or desc.get("n_flags", sh.n_flags) != sh.n_flags or desc.get("engine", self.engine) != self.engine):
@@ -405,6 +411,20 @@ class Worker:
 
     def write_item_state(self, k: int, state: torch.Tensor) -> None:
         self._copy_to_ps(k, "item_state", 0, state.to(torch.int32))
+
+    def read_sched_steps(self, k: int) -> List[int]:
+        """Every item's learning-rate schedule step (PsItemState::sched_step) on ps shard k."""
+        st = self.read_item_state(k).view(-1, 4)[: self.layout.shards[k].n_items, 3]
+        return [int(x) & 0xFFFFFFFF for x in st]
+
+    def set_sched_step(self, step: int) -> None:
+        """Chief-only, before the ps tasks serve: put every item of every shard at learning-rate schedule step `step`
+        (a checkpoint restore continues the schedule at the restored global_step). The other item state is kept."""
+        v = torch.tensor([int(step) & 0xFFFFFFFF], dtype=torch.int64).to(torch.int32)
+        for k in range(self.cluster.num_ps):
+            st = self.read_item_state(k).view(-1, 4).clone()
+            st[:, 3] = v
+            self.write_item_state(k, st.view(-1))
 
     @nvtx_annotate("dm.worker.initialize_variables")
     def initialize_variables(self, seed: int = 0, params: Optional[Dict[str, torch.Tensor]] = None) -> None:

@@ -33,7 +33,8 @@ def save_checkpoint(worker, directory: str) -> str:
         "optimizer": {"kind": worker.opt.kind, "lr": worker.opt.lr, "beta1": worker.opt.beta1,
                       "beta2": worker.opt.beta2, "eps": worker.opt.eps, "momentum": worker.opt.momentum,
                       "use_nesterov": worker.opt.use_nesterov, "decay": worker.opt.decay,
-                      "initial_accumulator_value": worker.opt.initial_accumulator_value},
+                      "initial_accumulator_value": worker.opt.initial_accumulator_value,
+                      "schedule": worker.opt.schedule.as_dict()},
         "variables": worker.read_variables("params"),       # [out, in] layout, see models/mlp.py
         "adam_m": worker.read_variables("adam_m"),
         "adam_v": worker.read_variables("adam_v"),
@@ -94,5 +95,8 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
             and state.get("dw_tile_n", 64) == worker.layout.dw_tile_n):
         for k, st in state["item_state"].items():
             worker.write_item_state(int(k), st)
+    # the learning-rate schedule continues at the restored global_step on every item, whether or not the item state
+    # was restored (TF1 evaluates it from global_step; like TF1 the schedule itself may change across a restore)
+    worker.set_sched_step(int(state["global_step"]))
     worker.write_global_step(int(state["global_step"]))
     return int(state["global_step"])

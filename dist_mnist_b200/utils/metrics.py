@@ -115,12 +115,15 @@ class TrainMetricsWriter:
     """The reference's implicit `StepCounterHook` / `SummarySaverHook` (MonitoredTrainingSession defaults, SURVEY
     §3.4): every `every_steps` local steps one JSON line {time, worker, local_steps, global_step, loss,
     batch_accuracy, steps_per_sec} is appended to `path` (accuracy comes for free: the head kernel counts the
-    correct predictions of every training batch), and optionally an INFO-style `global_step/sec` line is printed."""
+    correct predictions of every training batch), and optionally an INFO-style `global_step/sec` line is printed.
+    `lr_at` (a learning-rate schedule, global step -> rate) adds the rate at the line's global step as
+    `learning_rate`, like the learning-rate summary of a TF1 script."""
 
     def __init__(self, path: Optional[str], worker_index: int, batch_size: int, every_steps: int = 100,
-                 echo: bool = False, print_fn=print):
+                 echo: bool = False, print_fn=print, lr_at=None):
         self.path, self.worker, self.batch, self.every, self.echo, self.print_fn = (
             path, worker_index, batch_size, max(1, every_steps), echo, print_fn)
+        self.lr_at = lr_at
         self._fh = open(path, "a") if path else None
         self._t_last = time.time()
         self._steps = 0
@@ -151,6 +154,8 @@ class TrainMetricsWriter:
         }
         if self._gs_last is not None:
             rec["global_steps_per_sec"] = (int(global_step) - self._gs_last) / dt
+        if self.lr_at is not None:
+            rec["learning_rate"] = self.lr_at(int(global_step))
         if self._fh:
             self._fh.write(json.dumps(rec) + "\n")
             self._fh.flush()
