@@ -259,11 +259,14 @@ def check_accuracy() -> bool:
     return ok
 
 
-def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0) -> bool:
+def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0, moving_average_decay=None) -> bool:
     """Single-GPU test of the persistent PS kernel: mailboxes and inboxes are local buffers. `ieee`: the
     `--adam_math ieee` instantiation (correctly rounded sqrt / divide). `schedule` (an LrSchedule): the scheduled
-    instantiations, every item starting at schedule step `sched_step`; the reference then runs in fp64."""
+    instantiations, every item starting at schedule step `sched_step`; the reference then runs in fp64.
+    `moving_average_decay`: the averaging instantiations (num_updates on), shadows checked against fp64 as well."""
     from dist_mnist_b200 import _native as N
+    from dist_mnist_b200.parallel.config import OptimizerConfig
+    avg = OptimizerConfig("sgd", 1e-2, moving_average_decay=moving_average_decay) if moving_average_decay else None
     ok = True
     dev = "cuda"
     for opt, apply_mode in ((N.OPT_SGD, N.APPLY_PER_PUSH), (N.OPT_ADAM, N.APPLY_PER_PUSH), (N.OPT_ADAM, N.APPLY_MERGED),
@@ -323,6 +326,9 @@ def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0) -> bo
         P.ieee_math = 1 if ieee else 0
         if schedule is not None:
             schedule.fill_native(P)
+        ema = params.clone() if avg is not None else None
+        if ema is not None:
+            P.ema, P.ema_decay, P.ema_num_updates = ema.data_ptr(), avg.moving_average_decay, 1
         P.mailbox, P.arena_elems = mailbox.data_ptr(), arena
         P.flags, P.next_seq, P.consumed = flags.data_ptr(), next_seq.data_ptr(), consumed.data_ptr()
         P.global_step, P.worker_done, P.host_stop = gstep.data_ptr(), done.data_ptr(), stop.data_ptr()
@@ -337,8 +343,9 @@ def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0) -> bo
         for (off, r, c, l) in items:
             for rr in range(r):
                 mask_items[off + rr * l: off + rr * l + c] = True
-        dt = torch.float32 if schedule is None else torch.float64
+        dt = torch.float32 if schedule is None and avg is None else torch.float64
         pr, mr, vr = p0.to(dt), torch.zeros_like(p0, dtype=dt), torch.zeros_like(p0, dtype=dt)
+        er = p0.to(dt)
         t = 0
         for s in range(n_push):
             group = [grads[w, s].to(dt) for w in range(n_workers)]
@@ -355,17 +362,25 @@ def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0) -> bo
                     vr = 0.999 * vr + 0.001 * gg * gg
                     lr_t = lr * (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
                     pr = pr - lr_t * mr / (vr.sqrt() + 1e-8)
+                if avg is not None:   # the step ends at the round's last push (merged) or at its own
+                    last = s * n_workers + n_workers - 1 if apply_mode == N.APPLY_MERGED else pos
+                    er = er - (er - pr) * (1.0 - avg.ema_decay_at(sched_step + last + 1))
         pr = torch.where(mask_items, pr, p0.to(dt)).float()
         e = rel_err(params, pr)
+        if avg is not None:
+            e = max(e, rel_err(ema, torch.where(mask_items, er, p0.to(dt))))
         e_sh = rel_err(shadow.float()[mask_items], pr[mask_items].to(torch.bfloat16).float())
         gs = int(gstep.item())
         acks = inbox[:, 0].tolist()
         good = e < 1e-5 and gs == n_workers * n_push and acks == [n_push] * n_workers and e_sh < 1e-3
         sched = ""
-        if schedule is not None:
+        if schedule is not None or avg is not None:
             steps_now = sorted({int(x) & 0xFFFFFFFF for x in state[:, 3].tolist()})
             good &= steps_now == [(sched_step + n_workers * n_push) & 0xFFFFFFFF]
-            sched = f" schedule={schedule.kind} from={sched_step} sched_step={steps_now}"
+            kind = schedule.kind if schedule is not None else "constant"
+            sched = f" schedule={kind} from={sched_step} sched_step={steps_now}"
+        if avg is not None:
+            sched += f" ema={moving_average_decay} (param_err includes the shadows)"
         ok &= report(f"ps_serve opt={opt} mode={apply_mode} math={'ieee' if ieee else 'fast'}{sched}", good,
                      f"param_err={e:.1e} shadow_err={e_sh:.1e} global_step={gs} acks={acks} exit={int(exitc.item())}")
     return ok
@@ -393,7 +408,9 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     global_step and the acks exact). `resident`: one pushed push per worker and pass (lookahead 1) and one vectorisable
     item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass.
     A non-constant `opt.schedule` runs the scheduled instantiation (Adam and SGD too), every item starting at schedule
-    step `sched_step`; the check then includes every item's final sched_step."""
+    step `sched_step`; the check then includes every item's final sched_step. `opt.moving_average_decay` runs the
+    averaging instantiation (any rule, any schedule): the shadows start at the initial parameters and are checked
+    against fp64 within the same bound."""
     from dist_mnist_b200 import _native as N
     dev = "cuda"
     torch.manual_seed(6)
@@ -449,6 +466,9 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     P.momentum, P.decay, P.nesterov = opt.momentum or 0.0, opt.decay or 0.0, int(opt.use_nesterov)
     P.ieee_math = 1 if opt.math == "ieee" else 0
     opt.schedule.fill_native(P)
+    ema = params.clone() if opt.moving_averages else None
+    if ema is not None:
+        P.ema, P.ema_decay, P.ema_num_updates = ema.data_ptr(), opt.moving_average_decay, int(opt.moving_average_num_updates)
     P.lookahead = 1 if resident else 0
     P.mailbox, P.arena_elems = mailbox.data_ptr(), arena
     P.flags, P.next_seq, P.consumed = flags.data_ptr(), next_seq.data_ptr(), consumed.data_ptr()
@@ -469,6 +489,9 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
         torch.full((arena,), v0, dtype=torch.float64, device=dev)
     # push w of round k sits at position k * n_workers + w of the application order and is applied at schedule step
     # sched_step + that position; a merged round at the position of its first push
+    # moving averages: the step whose last push sits at position q moves the shadows by 1 - ema_decay_at(sched_step +
+    # q + 1) (fp32 decay as the kernel computes it, the update in fp64)
+    er = p0.double()
     t = 0
     for s in range(n_push):
         group = [grads[w, s].double() for w in range(n_workers)]
@@ -477,21 +500,28 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
         for gg, pos in steps:
             t += 1
             pr, mr, vr = _ref_apply(opt, pr, mr, vr, gg, opt.lr_at(sched_step + pos), t)
+            if ema is not None:
+                last = s * n_workers + n_workers - 1 if apply_mode == N.APPLY_MERGED else pos
+                er = er - (er - pr) * (1.0 - opt.ema_decay_at(sched_step + last + 1))
     pr, mr, vr = torch.where(mask, pr, p0.double()), torch.where(mask, mr, m0), torch.where(mask, vr, v0)
     e_p, e_m, e_v = rel_err(params, pr), rel_err(m, mr), rel_err(v, vr)
+    e_e = rel_err(ema, torch.where(mask, er, p0.double())) if ema is not None else 0.0
     shadow_exact = bool(torch.equal(shadow[mask], params[mask].to(torch.bfloat16)))
     gs = int(gstep.item())
     acks = inbox[:, 0].tolist()
-    good = (max(e_p, e_m, e_v) < 1e-5 and shadow_exact and gs == n_workers * n_push and acks == [n_push] * n_workers
-            and int(exitc.item()) == n_ctas)
+    good = (max(e_p, e_m, e_v, e_e) < 1e-5 and shadow_exact and gs == n_workers * n_push
+            and acks == [n_push] * n_workers and int(exitc.item()) == n_ctas)
     name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''} momentum={opt.momentum} math={opt.math} "
             f"mode={apply_mode} resident={resident}")
     extra = ""
-    if not opt.schedule.constant:
+    if not opt.schedule.constant or ema is not None:
         steps_now = sorted({int(x) & 0xFFFFFFFF for x in state.view(torch.int32).view(n_items, 4)[:, 3].tolist()})
         good &= steps_now == [(sched_step + n_workers * n_push) & 0xFFFFFFFF]
         name += f" schedule={opt.schedule.kind} from={sched_step}"
         extra = f" sched_step={steps_now}"
+    if ema is not None:
+        name += f" ema={opt.moving_average_decay} num_updates={opt.moving_average_num_updates}"
+        extra += f" err ema={e_e:.1e}"
     return report(name, good, f"err p={e_p:.1e} m={e_m:.1e} v={e_v:.1e} shadow_exact={shadow_exact} global_step={gs} "
                               f"acks={acks} exit={int(exitc.item())}{extra}")
 

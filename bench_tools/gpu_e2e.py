@@ -66,6 +66,14 @@ def ref_step(spec, params, m, v, t, x, y, opt, lr=None):
     return float(loss), t
 
 
+def ref_ema(opt, params, ema, n):
+    """TF1 `ExponentialMovingAverage.apply` in place, after the optimizer step that brought the global step to `n`:
+    shadow -= (shadow - p) * (1 - d) with d = opt.ema_decay_at(n), every op in fp32 as TF1's graph does it."""
+    omd = torch.tensor(1.0, dtype=torch.float32) - torch.tensor(opt.ema_decay_at(n), dtype=torch.float32)
+    for k in params:
+        ema[k] = ema[k] - (ema[k] - params[k]) * omd
+
+
 def wait_gstep(worker, target, timeout=10.0):
     t0 = time.time()
     while worker.read_global_step() < target:

@@ -9,8 +9,11 @@ optimizer, then a table.
 
 `--lr_schedule KIND` measures every optimizer twice, under that learning-rate schedule (the scheduled serve kernels)
 and at a constant rate, alternated in the same call: the cost of the rate table the scheduled kernels build per pass.
+`--moving_average_decay D` likewise measures every optimizer with moving averages of that decay (the averaging serve
+kernels) and without, alternated in the same call: the cost of the shadow load, update and store.
 
     python bench_tools/optimizer_apply.py [--steps 20000] [--warmup 50] [--only rmsprop,adam] [--lr_schedule KIND]
+                                          [--moving_average_decay D]
 """
 from __future__ import annotations
 
@@ -39,15 +42,17 @@ def schedule(kind: str, lr: float):
     return LrSchedule()
 
 
-def optimizer(rule: str, lr: float, sched: str = "constant"):
+def optimizer(rule: str, lr: float, sched: str = "constant", ema=None):
     from dist_mnist_b200.parallel.config import OptimizerConfig
 
     if rule == "nesterov":
-        return OptimizerConfig("momentum", lr, use_nesterov=True, schedule=schedule(sched, lr))
-    return OptimizerConfig(rule, lr, schedule=schedule(sched, lr))
+        return OptimizerConfig("momentum", lr, use_nesterov=True, schedule=schedule(sched, lr),
+                               moving_average_decay=ema)
+    return OptimizerConfig(rule, lr, schedule=schedule(sched, lr), moving_average_decay=ema)
 
 
-def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0, sched: str = "constant") -> dict:
+def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0, sched: str = "constant",
+            ema=None) -> dict:
     """One cluster in the bench configuration: warm-up, then one timed run_resident region after a ps restart."""
     import torch
 
@@ -59,7 +64,7 @@ def run_one(rule: str, steps: int, warmup: int, stats: bool, dev: int = 0, sched
     args = bench.parse_args(["--gpus", "1"])
     spec = mlp.get_model(args.model, args.hidden_units)
     cfg = bench.engine_config(args)
-    opt = optimizer(rule, args.learning_rate, sched)
+    opt = optimizer(rule, args.learning_rate, sched, ema)
     torch.cuda.set_device(dev)
     ds = data_utils.synthetic_mnist(data_utils.TRAIN_SIZE, seed=0)
     dev_x = ds.images.to(torch.float32).to(f"cuda:{dev}").contiguous()
@@ -105,6 +110,8 @@ def main(argv=None) -> int:
     ap.add_argument("--only", type=str, default="", help="comma-separated subset of " + ",".join(RULES))
     ap.add_argument("--lr_schedule", type=str, default="constant",
                     help="also run every optimizer under this learning-rate schedule, alternated with constant")
+    ap.add_argument("--moving_average_decay", type=float, default=None,
+                    help="also run every optimizer with moving averages of this decay, alternated with none")
     a = ap.parse_args(argv)
     import torch
 
@@ -121,23 +128,25 @@ def main(argv=None) -> int:
     if a.lr_schedule not in LR_SCHEDULES:
         raise SystemExit(f"unknown lr_schedule {a.lr_schedule!r} ({', '.join(LR_SCHEDULES)})")
     scheds = [a.lr_schedule, "constant"] if a.lr_schedule != "constant" else ["constant"]
+    emas = [a.moving_average_decay, None] if a.moving_average_decay is not None else [None]
     card = card_info(0)
     rows = []
     for r in rules:
-        for sc in scheds:
-            timed = run_one(r, a.steps, a.warmup, stats=False, sched=sc)
-            counted = run_one(r, a.steps, a.warmup, stats=True, sched=sc)
-            row = {"optimizer": r, "lr_schedule": sc, **timed,
+        for sc, ema in [(sc, e) for sc in scheds for e in emas]:
+            timed = run_one(r, a.steps, a.warmup, stats=False, sched=sc, ema=ema)
+            counted = run_one(r, a.steps, a.warmup, stats=True, sched=sc, ema=ema)
+            row = {"optimizer": r, "lr_schedule": sc, "moving_average_decay": ema, **timed,
                    "apply_cycles_per_push": counted.get("apply_cycles_per_push"),
                    "pushes_per_pass": counted.get("pushes_per_pass"), "ps_busy_fraction": counted.get("busy_fraction"),
                    "steps_per_s_with_counters": counted["steps_per_s"], "card": card}
             rows.append(row)
             print(json.dumps(row), flush=True)
-    print(f"card {card}; {a.steps} timed steps per optimizer and schedule")
-    print(f"{'optimizer':>10} {'lr_schedule':>18} {'steps/s':>9} {'apply cycles/push':>18} {'pushes/pass':>12} "
-          f"{'ps busy':>8}")
+    print(f"card {card}; {a.steps} timed steps per optimizer, schedule and averaging")
+    print(f"{'optimizer':>10} {'lr_schedule':>18} {'ema decay':>10} {'steps/s':>9} {'apply cycles/push':>18} "
+          f"{'pushes/pass':>12} {'ps busy':>8}")
     for row in rows:
-        print(f"{row['optimizer']:>10} {row['lr_schedule']:>18} {row['steps_per_s']:>9} "
+        print(f"{row['optimizer']:>10} {row['lr_schedule']:>18} {str(row['moving_average_decay']):>10} "
+              f"{row['steps_per_s']:>9} "
               f"{str(row['apply_cycles_per_push']):>18} {str(row['pushes_per_pass']):>12} "
               f"{str(row['ps_busy_fraction']):>8}")
     return 0

@@ -117,6 +117,7 @@ class PsServeParams(C.Structure):
         ("power", C.c_float), ("alpha", C.c_float), ("staircase", C.c_uint32), ("cycle", C.c_uint32),
         ("n_boundaries", C.c_int), ("boundaries", C.c_uint32 * MAX_LR_BOUNDARIES),
         ("values", C.c_float * (MAX_LR_BOUNDARIES + 1)),
+        ("ema", C.c_void_p), ("ema_decay", C.c_float), ("ema_num_updates", C.c_uint32),
     ]
 
 

@@ -98,10 +98,14 @@ def optimizer_config_from_args(args) -> OptimizerConfig:
     for flag, kinds in _OPT_FLAGS.items():
         if getattr(args, flag) not in (None, False) and args.optimizer not in kinds:
             raise ValueError(f"--{flag} does not apply to --optimizer {args.optimizer} (only {', '.join(kinds)})")
+    if args.moving_average_num_updates is not None and args.moving_average_decay is None:
+        raise ValueError("--moving_average_num_updates needs --moving_average_decay (moving averages are off)")
     return OptimizerConfig(args.optimizer, args.learning_rate, eps=args.epsilon, math=args.adam_math,
                            momentum=args.momentum, use_nesterov=args.use_nesterov, decay=args.rmsprop_decay,
                            initial_accumulator_value=args.initial_accumulator_value,
-                           schedule=lr_schedule_from_args(args))
+                           schedule=lr_schedule_from_args(args),
+                           moving_average_decay=args.moving_average_decay,
+                           moving_average_num_updates=args.moving_average_num_updates != "none")
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -151,6 +155,13 @@ def build_parser() -> argparse.ArgumentParser:
                    help="piecewise_constant: 1..8 increasing global steps, e.g. 1000,2000")
     p.add_argument("--lr_values", type=_float_list, default=None,
                    help="piecewise_constant: one rate more than boundaries, e.g. 0.1,0.01,0.001")
+    # TF1's ExponentialMovingAverage of every model variable, updated on the ps after each optimizer step and saved
+    # in checkpoints (utils/ckpt.load_variables(..., moving_averages=True) reads them back)
+    p.add_argument("--moving_average_decay", type=float, default=None,
+                   help="keep moving averages of the variables with this decay, in (0, 1), e.g. 0.9999 (unset: off)")
+    p.add_argument("--moving_average_num_updates", choices=["global_step", "none"], default=None,
+                   help="global_step (default): decay = min(D, (1 + step) / (10 + step)), TF1's num_updates=global_step;"
+                        " none: decay = D")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")

@@ -74,13 +74,20 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
   float lrs[dm::kMaxWorkers];
   for (int k = 0; k < __builtin_popcount(mask); ++k)
     lrs[k] = P.lr_schedule == dm::LR_CONSTANT ? P.lr : dm::scheduled_lr(P, st.sched_step + k);
+  // moving averages: 1 - d of the step that ends at the k-th push, d = ema_decay(sched_step + k + 1); a merged step
+  // ends at the last push of the pass
+  const bool ema = P.ema != nullptr;
+  const int npush = __builtin_popcount(mask);
+  float ema_omd[dm::kMaxWorkers];
+  for (int k = 0; ema && k < npush; ++k) ema_omd[k] = 1.f - dm::ema_decay(P, st.sched_step + k + 1);
   for (int r = 0; r < it.rows; ++r) {
     for (int c = 0; c < it.cols; ++c) {
       const uint64_t a = it.offset + static_cast<uint64_t>(r) * it.ld + c;
       float p = P.params[a];
-      float m = 0.f, v = 0.f;
+      float m = 0.f, v = 0.f, e = 0.f;
       if (use_m) m = P.adam_m[a];
       if (use_v) v = P.adam_v[a];
+      if (ema) e = P.ema[a];
       float b1p = st.beta1_pow, b2p = st.beta2_pow;
       float gsum = 0.f;
       uint32_t mm = mask;
@@ -91,6 +98,7 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         const uint32_t slot = seqs[w] % P.nslots;
         const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
         if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
+        const float omd = ema ? ema_omd[k] : 0.f;
         const float lr = lrs[k++];
         if (tf1) {
           tf1_step_cpu(P, lr, p, m, v, g);
@@ -103,6 +111,7 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         } else {
           p -= lr * g;
         }
+        if (ema) e -= (e - p) * omd;   // assign_moving_average
       }
       if (P.apply_mode == dm::APPLY_MERGED) {
         const float lr = lrs[0];
@@ -117,10 +126,12 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         } else {
           p -= lr * gsum;
         }
+        if (ema) e -= (e - p) * ema_omd[npush - 1];
       }
       P.params[a] = p;
       if (use_m) P.adam_m[a] = m;
       if (use_v) P.adam_v[a] = v;
+      if (ema) P.ema[a] = e;
       if (P.shadow_bf16 != nullptr && (it.flags & 1)) P.shadow_bf16[a] = f32_to_bf16(p);
     }
   }
@@ -151,7 +162,8 @@ void serve_loop(CpuPs* ps) {
       dm::PsItemState ns = st;
       ns.t += nsteps;
       for (int k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
-      if (P.lr_schedule != dm::LR_CONSTANT) ns.sched_step += npush;   // one schedule step per push, both apply modes
+      // one schedule step per push, both apply modes (also the moving averages' num_updates)
+      if (P.lr_schedule != dm::LR_CONSTANT || P.ema != nullptr) ns.sched_step += npush;
       P.item_state[item] = ns;
       uint32_t mm = mask;
       while (mm) {

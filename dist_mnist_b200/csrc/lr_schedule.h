@@ -1,6 +1,7 @@
 // Learning-rate schedules of the parameter server: TF1's tf.train.{exponential,inverse_time,natural_exp,polynomial,
-// cosine}_decay and piecewise_constant, evaluated at a step count `s` (PsItemState::sched_step). Shared by the
-// scheduled serve kernels (ps_apply_sm90.cu) and the cpu backend's serve loop (host_runtime.cpp).
+// cosine}_decay and piecewise_constant, evaluated at a step count `s` (PsItemState::sched_step), and the decay of
+// TF1's ExponentialMovingAverage. Shared by the scheduled and averaging serve kernels (ps_apply_sm90.cu) and the cpu
+// backend's serve loop (host_runtime.cpp).
 //
 // The rate is fp32 like TF1's float32 graph ops (powf / expf / cosf, IEEE division). The step becomes an exponent
 // through integer arithmetic, p = q + r / decay_steps with q = s / decay_steps, r = s % decay_steps (q alone with
@@ -58,6 +59,17 @@ DM_LR_HD float scheduled_lr(const PsServeParams& P, uint32_t s) {
     default:
       return lr0;
   }
+}
+
+// Decay of TF1's ExponentialMovingAverage for the optimizer step that brings an item to `n` applied pushes:
+// min(decay, (1 + n) / (10 + n)) from the float cast of n, in fp32 with IEEE division like TF1's graph. For
+// n >= (10 decay - 1) / (1 - decay) the min is `decay`; that bound lies below 2^24 for every decay <= 0.99999, so
+// the cast's rounding past 2^24 cannot change d there.
+DM_LR_HD float ema_decay(const PsServeParams& P, uint32_t n) {
+  if (!P.ema_num_updates) return P.ema_decay;
+  const float nf = static_cast<float>(n);
+  const float r = (1.f + nf) / (10.f + nf);
+  return P.ema_decay < r ? P.ema_decay : r;
 }
 
 }  // namespace dm

@@ -143,7 +143,8 @@ struct PsItemState {  // persisted across serve-kernel launches and checkpointed
   uint32_t t;        // number of pushes applied to this item (Adam step count)
   float beta1_pow;
   float beta2_pow;
-  uint32_t sched_step;  // learning-rate schedule step: pushes applied to this item under a non-constant schedule
+  uint32_t sched_step;  // pushes applied to this item under a non-constant learning-rate schedule or with moving
+                        // averages on: the schedule step, and TF1's num_updates of ExponentialMovingAverage
                         // (set to the restored global_step by a checkpoint restore)
 };
 
@@ -213,6 +214,13 @@ struct PsServeParams {
   int n_boundaries;            // piecewise: 1 .. kMaxLrBoundaries
   uint32_t boundaries[kMaxLrBoundaries];  // piecewise: strictly increasing steps
   float values[kMaxLrBoundaries + 1];     // piecewise: n_boundaries + 1 rates
+  // exponential moving averages of the parameters (TF1 tf.train.ExponentialMovingAverage.apply, zero_debias=False;
+  // appended, so that no earlier field moves). After every optimizer step of an element:
+  //   shadow -= (shadow - p) * (1 - d),  d = min(ema_decay, (1 + n) / (10 + n))  (d = ema_decay without num_updates)
+  // with n = the item's pushes applied, this step's included (PsItemState::sched_step after the step).
+  float* ema;                  // [arena] shadow variables of the fp32 parameters; null = off (unaveraged kernels)
+  float ema_decay;
+  uint32_t ema_num_updates;    // 1: d warms up with n (TF1 num_updates=global_step); 0: d = ema_decay
 };
 enum LrScheduleKind : int {
   LR_CONSTANT = 0,

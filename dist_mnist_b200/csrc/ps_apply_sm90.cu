@@ -105,13 +105,27 @@ struct ResidentState {
   float p[kQuads][4], m[kQuads][4], v[kQuads][4];
   bool loaded;
 };
+// The moving averages of that item (the averaging instantiations), valid whenever ResidentState::loaded is.
+struct ResidentEma {
+  float e[kQuads][4];
+};
+// Gradient loads in flight in the averaging instantiations (see kCh in apply_item).
+template <int kFam, bool kIeee>
+constexpr int kChEma() {
+  if constexpr (kFam == kFamAdamSgd) return kIeee ? kChunk - 3 : kChunk - 2;
+  else return (kFam == OPT_ADAGRAD || kIeee) ? kChunk - 2 : kChunk - 1;
+}
 
 // kSched (the scheduled instantiations): the rate of the optimizer step whose pushes sit at positions i0..i1 of the
 // application order is s_lr[i0], the pass's rate table (lr(sched_step + i), built by the serve loop); else P.lr.
-template <bool kIeee, int kFam, bool kSched = false>
+// kEma (the averaging instantiations, which are also kSched): the item's moving averages P.ema stay in registers for
+// the pass like the parameters, and after the optimizer step that ends at position i every element's shadow moves
+// toward the new parameter by 1 - s_ema[i], the pass's decay table (ema_decay(sched_step + i + 1)).
+template <bool kIeee, int kFam, bool kSched = false, bool kEma = false>
 __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItemState st, const uint64_t* s_pend,
                            const uint32_t* s_round, const int n_pend, ResidentState* res = nullptr,
-                           const float* s_lr = nullptr) {
+                           const float* s_lr = nullptr, const float* s_ema = nullptr,
+                           ResidentEma* res_ema = nullptr) {
   const int tid = threadIdx.x;
   const int total = it.rows * it.cols;
   const bool vec = ((it.cols & 3) == 0) && ((it.ld & 3) == 0) && ((it.offset & 3) == 0);
@@ -125,6 +139,7 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
     uint64_t a[kQuads];
     bool ok[kQuads];
     float pv[kQuads][4], mv[kQuads][4], vv[kQuads][4];
+    float ev[kQuads][4];   // kEma: the shadows
 #pragma unroll
     for (int q = 0; q < kQuads; ++q) {
       const int e = e0 + q * kPsThreads * step;
@@ -134,6 +149,10 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
       a[q] = it.offset + static_cast<uint64_t>(r) * it.ld + c;
 #pragma unroll
       for (int j = 0; j < 4; ++j) { pv[q][j] = 0.f; mv[q][j] = 0.f; vv[q][j] = 0.f; }
+      if constexpr (kEma) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) ev[q][j] = 0.f;
+      }
     }
     if (res != nullptr && res->loaded) {
       // the item's parameters and Adam slots never left this thread's registers: no load round trip in this pass
@@ -141,6 +160,12 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
       for (int q = 0; q < kQuads; ++q)
 #pragma unroll
         for (int j = 0; j < 4; ++j) { pv[q][j] = res->p[q][j]; mv[q][j] = res->m[q][j]; vv[q][j] = res->v[q][j]; }
+      if constexpr (kEma) {
+#pragma unroll
+        for (int q = 0; q < kQuads; ++q)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) ev[q][j] = res_ema->e[q][j];
+      }
     } else {
 #pragma unroll
       for (int q = 0; q < kQuads; ++q) {
@@ -156,10 +181,15 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
             const float4 tv = __ldcg(reinterpret_cast<const float4*>(P.adam_v + a[q]));
             vv[q][0] = tv.x; vv[q][1] = tv.y; vv[q][2] = tv.z; vv[q][3] = tv.w;
           }
+          if constexpr (kEma) {
+            const float4 te = __ldcg(reinterpret_cast<const float4*>(P.ema + a[q]));
+            ev[q][0] = te.x; ev[q][1] = te.y; ev[q][2] = te.z; ev[q][3] = te.w;
+          }
         } else {
           pv[q][0] = __ldcg(P.params + a[q]);
           if (use_m) mv[q][0] = __ldcg(P.adam_m + a[q]);
           if (use_v) vv[q][0] = __ldcg(P.adam_v + a[q]);
+          if constexpr (kEma) ev[q][0] = __ldcg(P.ema + a[q]);
         }
       }
     }
@@ -173,7 +203,11 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
     // the other families' straight-line update keeps more values live: a chunk of 8 spills there, 7 does not. The
     // scheduled Adam / SGD instantiations (rate-table read, round start) spill at 8 too, and the IEEE one still at 7:
     // 7 and 6 there; the scheduled Momentum / Adagrad / RMSProp ones do not spill at 7.
-    constexpr int kCh = kFam != kFamAdamSgd ? kChunk - 1 : !kSched ? kChunk : kIeee ? kChunk - 2 : kChunk - 1;
+    constexpr int kChNoEma = kFam != kFamAdamSgd ? kChunk - 1 : !kSched ? kChunk : kIeee ? kChunk - 2 : kChunk - 1;
+    // The averaging instantiations hold 8 shadows more per thread (kChEma): Momentum and fast RMSProp do not spill at
+    // 7; Adagrad (both), IEEE RMSProp and fast Adam / SGD spill at 7 and take 6; IEEE Adam / SGD spills at 6 and
+    // takes 5.
+    constexpr int kCh = kEma ? kChEma<kFam, kIeee>() : kChNoEma;
     int r0 = 0;   // kSched, merged: position of the first push of the current round
     for (int i0 = 0; i0 < n_pend; i0 += kCh) {
       float g[kCh][kQuads][4];
@@ -217,6 +251,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
           b2p *= P.beta2;
           lr_t = adam_lr_t<kIeee>(lr, b1p, b2p);
         }
+        float ema_omd = 0.f;   // kEma: 1 - d of this step, in fp32 like TF1's `1.0 - decay`
+        if constexpr (kEma) ema_omd = 1.f - s_ema[i];
 #pragma unroll
         for (int q = 0; q < kQuads; ++q) {
 #pragma unroll
@@ -226,6 +262,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
             if constexpr (kFam != kFamAdamSgd) tf1_step<kFam, kIeee, kSched>(pv[q][j], mv[q][j], vv[q][j], gv, P, lr);
             else if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, lr_t, P.beta1, P.beta2, P.eps);
             else pv[q][j] = fmaf(-lr, gv, pv[q][j]);
+            // assign_moving_average: shadow -= (shadow - p) * (1 - d), each op rounded as TF1's graph does
+            if constexpr (kEma) ev[q][j] = ev[q][j] - __fmul_rn(ev[q][j] - pv[q][j], ema_omd);
             if (merged) gsum[q][j] = 0.f;
           }
         }
@@ -236,6 +274,12 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
       for (int q = 0; q < kQuads; ++q)
 #pragma unroll
         for (int j = 0; j < 4; ++j) { res->p[q][j] = pv[q][j]; res->m[q][j] = mv[q][j]; res->v[q][j] = vv[q][j]; }
+      if constexpr (kEma) {
+#pragma unroll
+        for (int q = 0; q < kQuads; ++q)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) res_ema->e[q][j] = ev[q][j];
+      }
       res->loaded = true;
     }
 #pragma unroll
@@ -246,6 +290,7 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         *reinterpret_cast<float4*>(P.params + a[q]) = make_float4(pv[q][0], pv[q][1], pv[q][2], pv[q][3]);
         if (use_m) *reinterpret_cast<float4*>(P.adam_m + a[q]) = make_float4(mv[q][0], mv[q][1], mv[q][2], mv[q][3]);
         if (use_v) *reinterpret_cast<float4*>(P.adam_v + a[q]) = make_float4(vv[q][0], vv[q][1], vv[q][2], vv[q][3]);
+        if constexpr (kEma) *reinterpret_cast<float4*>(P.ema + a[q]) = make_float4(ev[q][0], ev[q][1], ev[q][2], ev[q][3]);
         if (shadow) {
           __nv_bfloat162 lo = __floats2bfloat162_rn(pv[q][0], pv[q][1]);
           __nv_bfloat162 hi = __floats2bfloat162_rn(pv[q][2], pv[q][3]);
@@ -258,6 +303,7 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         P.params[a[q]] = pv[q][0];
         if (use_m) P.adam_m[a[q]] = mv[q][0];
         if (use_v) P.adam_v[a[q]] = vv[q][0];
+        if constexpr (kEma) P.ema[a[q]] = ev[q][0];
         if (shadow) {
           __nv_bfloat16 b = __float2bfloat16(pv[q][0]);
           P.shadow_bf16[a[q]] = *reinterpret_cast<uint16_t*>(&b);
@@ -272,6 +318,7 @@ template <bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kFamAdamSgd;
   constexpr bool kSched = false;
+  constexpr bool kEma = false;
 #include "ps_serve_body.cuh"
 }
 // Momentum / Adagrad / RMSProp: ps_serve_kernel<kOpt, kIeee>.
@@ -279,6 +326,7 @@ template <int kOpt, bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kOpt;
   constexpr bool kSched = false;
+  constexpr bool kEma = false;
 #include "ps_serve_body.cuh"
 }
 // Any family under a non-constant learning-rate schedule (P.lr_schedule != LR_CONSTANT): ps_serve_sched_kernel<kFam,
@@ -287,6 +335,17 @@ template <int kFamT, bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_sched_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kFamT;
   constexpr bool kSched = true;
+  constexpr bool kEma = false;
+#include "ps_serve_body.cuh"
+}
+// Any family with moving averages of the parameters (P.ema != null), under any schedule: ps_serve_ema_kernel<kFam,
+// kIeee>. The rate table is compiled in as in the scheduled kernels (scheduled_lr is lr0 for LR_CONSTANT), so one
+// set serves a constant rate and every schedule; the fourteen above stay exactly as measured.
+template <int kFamT, bool kIeee>
+__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_ema_kernel(const __grid_constant__ PsServeParams P) {
+  constexpr int kFam = kFamT;
+  constexpr bool kSched = true;
+  constexpr bool kEma = true;
 #include "ps_serve_body.cuh"
 }
 
@@ -312,6 +371,24 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = cluster > 1 ? 1 : 0;
+  if (p.ema != nullptr) {
+    switch (p.opt) {
+      case OPT_SGD:
+      case OPT_ADAM:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<kFamAdamSgd, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<kFamAdamSgd, false>, p);
+      case OPT_MOMENTUM:
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_MOMENTUM, false>, p);
+      case OPT_ADAGRAD:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADAGRAD, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADAGRAD, false>, p);
+      case OPT_RMSPROP:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, false>, p);
+      default:
+        return cudaErrorInvalidValue;
+    }
+  }
   if (p.lr_schedule != LR_CONSTANT) {
     switch (p.opt) {
       case OPT_SGD:
@@ -458,6 +535,13 @@ cudaError_t preload_ps_kernels() {
   if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<kFamAdamSgd, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<kFamAdamSgd, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, dense_apply_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, shadow_refresh_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, wait_ack_kernel)) != cudaSuccess) return e;

@@ -1,8 +1,9 @@
 // Body of ps_serve_kernel, included once per kernel template (ps_apply_sm90.cu): it expects the kernel parameter
-// block `P` and the compile-time `kIeee` (correctly rounded sqrt / divide), `kFam` (optimizer family) and `kSched`
-// (non-constant learning-rate schedule) in scope. A shared device function called by both kernels would give the
-// Adam / SGD instantiations different SASS from the one that was measured; included textually they compile exactly
-// as before. Everything a schedule adds sits behind `if constexpr (kSched)`.
+// block `P` and the compile-time `kIeee` (correctly rounded sqrt / divide), `kFam` (optimizer family), `kSched`
+// (non-constant learning-rate schedule) and `kEma` (moving averages; implies kSched) in scope. A shared device
+// function called by both kernels would give the Adam / SGD instantiations different SASS from the one that was
+// measured; included textually they compile exactly as before. Everything a schedule adds sits behind
+// `if constexpr (kSched)`, everything averaging adds behind `if constexpr (kEma)`.
   // Everything the poll loop needs about this CTA's items lives in shared memory: the only global traffic of an
   // idle poll is one acquire load of a flag word per (worker, look-ahead slot).
   __shared__ PsItem s_item[kMaxOwn];
@@ -14,6 +15,7 @@
   __shared__ uint32_t s_any;
   __shared__ uint32_t s_exit;
   __shared__ float s_lr[kMaxPending];   // kSched: rate of the pass's i-th push, lr(sched_step + i)
+  __shared__ float s_ema[kMaxPending];  // kEma: decay of the step ending at the i-th push, ema_decay(sched_step + i + 1)
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int warp = tid >> 5;
@@ -46,6 +48,7 @@
   // the parameters, checkpoints read the slots — but the three load round trips (~1 us of a ~6.7 us pass) are gone.
   ResidentState resident;
   resident.loaded = false;
+  ResidentEma resident_ema;   // kEma: the shadows beside them
   bool use_resident = false;
   if (n_own == 1) {
     const PsItem it0 = s_item[0];
@@ -93,6 +96,11 @@
           // at schedule step sched_step + i; published to apply_item by the barrier below
           if (lane < __popc(p_taken)) s_lr[lane] = scheduled_lr(P, s_state[own].sched_step + lane);
         }
+        if constexpr (kEma) {
+          // the pass's decay table: the step that ends at the i-th push leaves the item at sched_step + i + 1
+          // applied pushes, TF1's num_updates = global_step after the apply_gradients op the average follows
+          if (lane < __popc(p_taken)) s_ema[lane] = ema_decay(P, s_state[own].sched_step + lane + 1);
+        }
       }
       __syncthreads();
       const long long c1 = stats_on ? clock64() : 0;
@@ -100,7 +108,11 @@
       if (s_any) {
         sweep_any = true;
         const PsItemState st = s_state[own];
-        if constexpr (kSched)
+        if constexpr (kEma)
+          apply_item<kIeee, kFam, true, true>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
+                                              use_resident ? &resident : nullptr, s_lr, s_ema,
+                                              use_resident ? &resident_ema : nullptr);
+        else if constexpr (kSched)
           apply_item<kIeee, kFam, true>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
                                         use_resident ? &resident : nullptr, s_lr);
         else
@@ -120,7 +132,8 @@
             PsItemState ns = st;
             ns.t += nsteps;
             for (uint32_t k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
-            if constexpr (kSched) ns.sched_step += npush;   // one schedule step per push, in both apply modes
+            // one schedule step per push, in both apply modes (also the num_updates of the averaging kernels)
+            if constexpr (kSched) ns.sched_step += npush;
             s_state[own] = ns;
             P.item_state[item] = ns;   // persisted for checkpoints / a relaunch (never read back in this loop)
           }

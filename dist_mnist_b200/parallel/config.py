@@ -194,6 +194,11 @@ class OptimizerConfig:
     decay: Optional[float] = None       # "rmsprop" (0.9)
     initial_accumulator_value: Optional[float] = None   # "adagrad" (0.1): Adagrad's slot starts here, not at 0
     schedule: LrSchedule = LrSchedule()   # learning-rate schedule over the global step (default: constant `lr`)
+    # TF1 `tf.train.ExponentialMovingAverage(decay, num_updates=global_step).apply(tf.trainable_variables())`, run on
+    # the ps after every optimizer step (zero_debias=False): every model variable gets a shadow that starts at the
+    # variable's initial value and moves by shadow -= (shadow - p) * (1 - d). None = off.
+    moving_average_decay: Optional[float] = None
+    moving_average_num_updates: bool = True   # d = min(decay, (1 + n) / (10 + n)), n = global step; False: d = decay
 
     def __post_init__(self):
         if self.math not in ("fast", "ieee"):
@@ -211,10 +216,32 @@ class OptimizerConfig:
             raise ValueError("initial_accumulator_value must be positive (Adagrad divides by its square root)")
         if not isinstance(self.schedule, LrSchedule):
             raise ValueError(f"schedule must be an LrSchedule, got {type(self.schedule).__name__}")
+        d = self.moving_average_decay
+        if d is not None:
+            if isinstance(d, bool) or not isinstance(d, (int, float)) or not 0.0 < d < 1.0:
+                raise ValueError(f"moving_average_decay must lie in (0, 1), got {d!r}")
+            object.__setattr__(self, "moving_average_decay", float(d))
+        object.__setattr__(self, "moving_average_num_updates", bool(self.moving_average_num_updates))
 
     def lr_at(self, step: int) -> float:
         """The learning rate of a push applied at global step `step` (LrSchedule.lr_at with lr0 = lr)."""
         return self.schedule.lr_at(step, self.lr)
+
+    @property
+    def moving_averages(self) -> bool:
+        return self.moving_average_decay is not None
+
+    def ema_decay_at(self, n: int) -> float:
+        """The moving-average decay of the optimizer step that brings the global step to `n` (the step included, as
+        TF1's `num_updates` after the apply op the average depends on): min(decay, (1 + n) / (10 + n)) in fp64,
+        rounded once to fp32 (what the ps computes in fp32), or the decay without num_updates."""
+        if self.moving_average_decay is None:
+            raise ValueError("moving averages are off (moving_average_decay is None)")
+        d = self.moving_average_decay
+        if self.moving_average_num_updates:
+            n = int(n)
+            d = min(d, (1.0 + n) / (10.0 + n))
+        return _f32(d)
 
     @property
     def native_kind(self) -> int:
@@ -305,6 +332,9 @@ class EngineConfig:
             if not opt.schedule.constant:
                 raise ValueError("push_mode='atomic' folds a constant -lr into the worker's push; a learning-rate "
                                  "schedule needs push_mode='mailbox'")
+            if opt.moving_averages:
+                raise ValueError("push_mode='atomic' has no ps-side apply to update moving averages after; "
+                                 "moving_average_decay needs push_mode='mailbox'")
             if self.dtype != "fp32":
                 raise ValueError("push_mode='atomic' updates only the fp32 master copy; use dtype fp32")
             if self.backend != "cuda":

@@ -59,8 +59,10 @@ def serve_geometry(n_items: int, ps_ctas: int, shares_gpu: bool, engine: str) ->
     return n, 1
 
 
-def shard_carver(shard: ShardLayout, n_workers: int, nslots: int) -> Carver:
-    """Byte layout of one PS shard segment (both sides derive pointers from the exported table)."""
+def shard_carver(shard: ShardLayout, n_workers: int, nslots: int, moving_averages: bool = False) -> Carver:
+    """Byte layout of one PS shard segment (both sides derive pointers from the exported table). `moving_averages`:
+    the shadow variables of ExponentialMovingAverage (region "ema", last and empty when off, so that no other region
+    moves)."""
     a = shard.arena_elems
     ni = max(shard.n_items, 1)
     nf = max(shard.n_flags, 1)
@@ -78,6 +80,7 @@ def shard_carver(shard: ShardLayout, n_workers: int, nslots: int) -> Carver:
     c.add("ctrl", CTRL_WORDS * 4)
     c.add("inbox_table", N.MAX_WORKERS * 8)
     c.add("stats", PS_STATS_CTAS * 9 * 8)   # per-CTA serve statistics and SM ids (DM_PS_STATS=1)
+    c.add("ema", a * 4 if moving_averages else 0)
     return c
 
 
@@ -116,7 +119,7 @@ class ParameterServer:
         kind = "cuda" if cfg.backend == "cuda" else "shm"
         if kind == "cuda":
             N.check(self.lib.dm_set_device(self.device), "set device")
-        carver = shard_carver(self.shard, self.n_workers, cfg.nslots)
+        carver = shard_carver(self.shard, self.n_workers, cfg.nslots, opt.moving_averages)
         self.seg = Segment.create(kind, carver.total, device=self.device, table=carver.table(), tag=f"ps{task_index}")
         self._init_tables()
         desc = self.seg.export()
@@ -175,6 +178,10 @@ class ParameterServer:
         P.nesterov = int(opt.use_nesterov)
         opt.schedule.fill_native(P)   # non-constant: the scheduled serve kernels / the cpu loop's rate table
         P.ieee_math = 1 if opt.math == "ieee" else 0
+        # moving averages: the averaging serve kernels / the cpu loop's shadow update
+        P.ema = s.addr("ema") if opt.moving_averages else None
+        P.ema_decay = opt.moving_average_decay or 0.0
+        P.ema_num_updates = int(opt.moving_average_num_updates)
         P.mailbox, P.arena_elems = s.addr("mailbox"), sh.arena_elems
         P.flags, P.next_seq, P.consumed = s.addr("flags"), s.addr("next_seq"), s.addr("consumed")
         P.global_step = s.addr("ctrl", 4 * CTRL_GLOBAL_STEP)

@@ -182,6 +182,13 @@ class Worker:
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: learning-rate "
                                    f"schedule {ps_sched} lr={ps_opt.get('lr')}, this worker has {self.opt.schedule} "
                                    f"lr={self.opt.lr}")
+            # the ps keeps (and updates) the moving averages; the chief writes them and evaluate / checkpoints read
+            # them, so both sides must agree on whether they exist and how they move
+            ps_ema = (ps_opt.get("moving_average_decay"), ps_opt.get("moving_average_num_updates", True))
+            my_ema = (self.opt.moving_average_decay, self.opt.moving_average_num_updates)
+            if ps_ema != my_ema:
+                raise RuntimeError(f"ps {k} was started with a different engine configuration: moving averages "
+                                   f"(decay, num_updates) {ps_ema}, this worker has {my_ema}")
             sh = self.layout.shards[k]
             if (desc["arena_elems"] != sh.arena_elems or desc["n_items"] != sh.n_items
                     or desc.get("n_flags", sh.n_flags) != sh.n_flags or desc.get("engine", self.engine) != self.engine):
@@ -367,7 +374,16 @@ class Worker:
             return flat.view(vl.rows, vl.ld)[:, :vl.cols].clone()
         return flat.clone()
 
+    def _require_moving_averages(self) -> None:
+        if not self.opt.moving_averages:
+            raise ValueError("moving averages are off in this run (OptimizerConfig.moving_average_decay is None / "
+                             "no --moving_average_decay): there are no shadow variables")
+
     def write_variables(self, params: Dict[str, torch.Tensor], region: str = "params") -> None:
+        """Write variables into a region of the ps shards: "params", the slots "adam_m" / "adam_v", or "ema" (the
+        moving averages, only when they are on)."""
+        if region == "ema":
+            self._require_moving_averages()
         for name, t in params.items():
             vl = self.layout.by_name[name]
             if tuple(t.shape) != tuple(vl.spec.shape):
@@ -380,6 +396,9 @@ class Worker:
                     self._copy_to_ps(k, "shadow", off, flat.to(torch.bfloat16))
 
     def read_variables(self, region: str = "params") -> Dict[str, torch.Tensor]:
+        """Every variable, [out, in] / [out], from a region of the ps shards (see write_variables)."""
+        if region == "ema":
+            self._require_moving_averages()
         out = {}
         for name, vl in self.layout.by_name.items():
             if len({(pc.ps, pc.offset) for pc in vl.pieces}) == 1:   # one owner (whole variable, or all slices there)
@@ -413,7 +432,8 @@ class Worker:
         self._copy_to_ps(k, "item_state", 0, state.to(torch.int32))
 
     def read_sched_steps(self, k: int) -> List[int]:
-        """Every item's learning-rate schedule step (PsItemState::sched_step) on ps shard k."""
+        """Every item's learning-rate schedule step (PsItemState::sched_step, also the moving averages' num_updates)
+        on ps shard k."""
         st = self.read_item_state(k).view(-1, 4)[: self.layout.shards[k].n_items, 3]
         return [int(x) & 0xFFFFFFFF for x in st]
 
@@ -436,6 +456,8 @@ class Worker:
         m0, v0 = self.opt.slot_init()   # Adagrad's accumulator and RMSProp's ms do not start at 0
         self.write_variables({k: torch.full_like(v, m0) for k, v in params.items()}, "adam_m")
         self.write_variables({k: torch.full_like(v, v0) for k, v in params.items()}, "adam_v")
+        if self.opt.moving_averages:   # shadows start at the initial values (TF1 slot_creator, initialized_value())
+            self.write_variables(params, "ema")
         self.rdv.put("init/done", {"seed": seed, "by": self.task_index})
 
     def variables_are_live(self) -> bool:
@@ -618,6 +640,19 @@ class Worker:
                             p.launch(st)
                 finally:
                     N.check(self.lib.dm_exec_end_group_capture(self._exec, g), "end group capture")
+        if self.opt.moving_averages:
+            # evaluate(moving_averages=True) runs the fused engine's host-logits + accuracy-kernel path
+            self._alloc_eval_buffers()
+
+    def _alloc_eval_buffers(self) -> None:
+        """Buffers of the host-logits evaluation path (allocated while building the step: nothing is allocated once a
+        persistent ps kernel may be resident)."""
+        Cn = self.spec.num_classes
+        self._ev_rows = 4096
+        self._ev_dev = torch.zeros(2 * self._ev_rows, Cn, dtype=torch.float32, device=f"cuda:{self.device}")
+        self._ev_cnt = torch.zeros(1, dtype=torch.int32, device=f"cuda:{self.device}")
+        self._ev_pin = torch.zeros(2 * self._ev_rows, Cn, dtype=torch.float32).pin_memory()
+        self._ev_cnt_pin = torch.zeros(1, dtype=torch.int32).pin_memory()
 
     # ------------------------------------------------------------------------------------------
     # fused engine construction
@@ -731,12 +766,7 @@ class Worker:
         self._fx_stage_y = torch.zeros(1, self.B_pad, Cn, dtype=torch.float32)
         self._fx_tickets: Dict[int, StepOutput] = {}
         self._fx_ticket = 0
-        # evaluation buffers (allocated now: nothing is allocated once a persistent ps kernel may be resident)
-        self._ev_rows = 4096
-        self._ev_dev = torch.zeros(2 * self._ev_rows, Cn, dtype=torch.float32, device=f"cuda:{self.device}")
-        self._ev_cnt = torch.zeros(1, dtype=torch.int32, device=f"cuda:{self.device}")
-        self._ev_pin = torch.zeros(2 * self._ev_rows, Cn, dtype=torch.float32).pin_memory()
-        self._ev_cnt_pin = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self._alloc_eval_buffers()
         self.kernels_per_step = 1
         torch.cuda.synchronize(self.device)
 
@@ -1008,16 +1038,21 @@ class Worker:
     # evaluation (forward only, accuracy kernel / torch on cpu)
     # ------------------------------------------------------------------------------------------
     @nvtx_annotate("dm.worker.evaluate")
-    def evaluate(self, images: torch.Tensor, labels: torch.Tensor) -> Tuple[float, float]:
+    def evaluate(self, images: torch.Tensor, labels: torch.Tensor,
+                 moving_averages: bool = False) -> Tuple[float, float]:
         """(mean loss, accuracy) of the current PS variables on a host dataset; GPU path uses the hand-written
-        accuracy reduction kernel (SURVEY K12) on torch-computed logits of the pulled variables."""
-        if self.cfg.backend == "cuda" and self.engine == "fused":
+        accuracy reduction kernel (SURVEY K12) on torch-computed logits of the pulled variables.
+        `moving_averages`: evaluate the shadow variables instead (TF1's `ema.variables_to_restore()` model), on
+        either engine through the host-logits path below."""
+        if moving_averages:
+            self._require_moving_averages()
+        if self.cfg.backend == "cuda" and (self.engine == "fused" or moving_averages):
             # Evaluation is not part of a training step: logits of the pulled variables are computed with torch on the
             # host (no torch CUDA kernel is launched — a lazily loaded kernel could deadlock against a resident
             # persistent ps kernel of an in-process cluster), the correct-prediction count with the hand-written,
             # pre-loaded accuracy reduction (SURVEY K12) on pre-allocated device buffers.
             self.drain()
-            params = self.read_variables()
+            params = self.read_variables("ema" if moving_averages else "params")
             logits, _ = mlp.forward_logits(self.spec, params, images.float())
             logits = logits.float().contiguous()
             labels_f = labels.float().contiguous()
@@ -1065,7 +1100,7 @@ class Worker:
                 loss_sum += float(res[:1].view(torch.float32).item())
                 correct += int(res[2].item())
             return loss_sum / n_chunks, correct / (n_chunks * self.batch)
-        params = self.read_variables()
+        params = self.read_variables("ema" if moving_averages else "params")
         logits, _ = mlp.forward_logits(self.spec, params, images.float())
         correct = mlp.accuracy_count(logits, labels)
         loss = float(mlp.loss_from_logits(self.spec, logits, labels.float()))

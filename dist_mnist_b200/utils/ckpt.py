@@ -12,7 +12,7 @@ Files: `<dir>/model.ckpt-<global_step>.pt` plus a TF-style `<dir>/checkpoint` in
 from __future__ import annotations
 
 import os
-from typing import Optional
+from typing import Dict, Optional
 
 import torch
 
@@ -34,7 +34,9 @@ def save_checkpoint(worker, directory: str) -> str:
                       "beta2": worker.opt.beta2, "eps": worker.opt.eps, "momentum": worker.opt.momentum,
                       "use_nesterov": worker.opt.use_nesterov, "decay": worker.opt.decay,
                       "initial_accumulator_value": worker.opt.initial_accumulator_value,
-                      "schedule": worker.opt.schedule.as_dict()},
+                      "schedule": worker.opt.schedule.as_dict(),
+                      "moving_average_decay": worker.opt.moving_average_decay,
+                      "moving_average_num_updates": worker.opt.moving_average_num_updates},
         "variables": worker.read_variables("params"),       # [out, in] layout, see models/mlp.py
         "adam_m": worker.read_variables("adam_m"),
         "adam_v": worker.read_variables("adam_v"),
@@ -43,6 +45,8 @@ def save_checkpoint(worker, directory: str) -> str:
         "num_ps": worker.cluster.num_ps,
         "dw_tile_n": worker.layout.dw_tile_n,    # item tables (hence item_state) depend on the dW tile width
     }
+    if worker.opt.moving_averages:   # the shadow variables (TF1 saves `<var>/ExponentialMovingAverage`)
+        state["ema"] = worker.read_variables("ema")
     name = f"model.ckpt-{gstep}.pt"
     path = os.path.join(directory, name)
     tmp = path + ".tmp"
@@ -85,9 +89,17 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
     kind = state.get("optimizer", {}).get("kind")
     if kind != worker.opt.kind and (kind in TF1_SLOT_KINDS or worker.opt.kind in TF1_SLOT_KINDS):
         raise RuntimeError(f"checkpoint {path} holds {kind!r} optimizer slots, this run uses {worker.opt.kind!r}")
+    # moving averages: restored when this run keeps them (TF1's Saver restores only the variables its graph has, so
+    # saved shadows are ignored without them), and a run that keeps them cannot start from a checkpoint without them
+    # (TF1 fails on the missing `.../ExponentialMovingAverage` variables)
+    if worker.opt.moving_averages and "ema" not in state:
+        raise RuntimeError(f"checkpoint {path} has no moving averages, this run keeps them "
+                           f"(moving_average_decay={worker.opt.moving_average_decay})")
     worker.write_variables(state["variables"], "params")
     worker.write_variables(state["adam_m"], "adam_m")
     worker.write_variables(state["adam_v"], "adam_v")
+    if worker.opt.moving_averages:
+        worker.write_variables(state["ema"], "ema")
     # per-item optimizer state (Adam step count / beta powers) is only meaningful for the same item table; with a
     # different shard count, placement or dW tile width the variables and Adam slots are restored and the
     # per-item step counters restart (bias correction re-warms, as after a TF slot-variable reset)
@@ -100,3 +112,22 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
     worker.set_sched_step(int(state["global_step"]))
     worker.write_global_step(int(state["global_step"]))
     return int(state["global_step"])
+
+
+def load_variables(path: str, moving_averages: bool = False) -> Dict[str, torch.Tensor]:
+    """The model variables of a checkpoint file (or of the latest checkpoint of a directory), by name in the [out, in]
+    layout of models/mlp.py, for evaluating a finished run offline. `moving_averages`: the shadow variables instead,
+    as TF1's `saver = tf.train.Saver(ema.variables_to_restore())` loads them into the model variables."""
+    if os.path.isdir(path):
+        latest = latest_checkpoint(path)
+        if latest is None:
+            raise FileNotFoundError(f"no checkpoint in {path}")
+        path = latest
+    state = torch.load(path, map_location="cpu", weights_only=False)
+    if state.get("format_version") != FORMAT_VERSION:
+        raise RuntimeError(f"unsupported checkpoint format in {path}")
+    if not moving_averages:
+        return state["variables"]
+    if "ema" not in state:
+        raise RuntimeError(f"checkpoint {path} has no moving averages (the run had no moving_average_decay)")
+    return state["ema"]
