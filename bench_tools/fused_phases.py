@@ -1,13 +1,15 @@
 """In-kernel phase stamps of the fused step kernel (DM_FUSED_DEBUG_TS=1): clock64() of cluster 0 / CTA 0 at
 step start, forward accumulator ready, after the reduce-scatter barrier, head done, after the all-gather barrier,
-dW accumulator ready, tile pushed, step end — for the first 8 steps of the last launch. lanes=1 and lanes=8."""
+dW accumulator ready, tile pushed, step end — for the first 8 steps of the last launch. lanes=1 and lanes=8.
+
+    python bench_tools/fused_phases.py [off | global_norm | norm | value]   (gradient clipping, default off)"""
 import os
 import sys
 
 import torch
 
 from dist_mnist_b200.models import mlp
-from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
+from dist_mnist_b200.parallel.config import EngineConfig, GradClip, OptimizerConfig
 from dist_mnist_b200.session import InProcessCluster
 from dist_mnist_b200.utils import data
 
@@ -42,7 +44,11 @@ def main():
     os.environ["DM_FUSED_DEBUG_TS"] = "1"
     ds = data.synthetic_mnist(8192, seed=0)
     spec = mlp.book_model(100)
-    opt = OptimizerConfig("adam", 1e-4)
+    kind = sys.argv[1] if len(sys.argv) > 1 else "off"
+    clip = (GradClip() if kind == "off" else GradClip("value", value_min=-0.01, value_max=0.01) if kind == "value"
+            else GradClip(kind, clip_norm=0.1))
+    opt = OptimizerConfig("adam", 1e-4, clip=clip)
+    print(f"gradient clipping: {kind}")
     for lanes in (1, 8):
         cfg = EngineConfig(backend="cuda", lanes=lanes, nslots=2 * lanes, pipeline_slots=max(4, 2 * lanes))
         with InProcessCluster(spec, opt, cfg, batch_size=32) as cl:

@@ -37,8 +37,9 @@ def card_info(dev: int) -> dict:
     return info
 
 
-def run(lanes: int, steps: int, warmup: int, batch: int, dev: int = 0) -> dict:
-    """One long fused launch beside the resident ps; returns the residency record as a dict."""
+def run(lanes: int, steps: int, warmup: int, batch: int, dev: int = 0, clip=None) -> dict:
+    """One long fused launch beside the resident ps; returns the residency record as a dict. `clip`: a GradClip, which
+    runs the gradient-clipping instantiation of the fused kernel."""
     import torch
 
     import bench
@@ -50,7 +51,7 @@ def run(lanes: int, steps: int, warmup: int, batch: int, dev: int = 0) -> dict:
 
     args = bench.parse_args(["--gpus", "1", "--lanes", str(lanes), "--batch_size", str(batch)])
     spec = mlp.get_model(args.model, args.hidden_units)
-    opt = OptimizerConfig(args.optimizer, args.learning_rate)
+    opt = OptimizerConfig(args.optimizer, args.learning_rate, **({"clip": clip} if clip is not None else {}))
     cfg = bench.engine_config(args)
     torch.cuda.set_device(dev)
     lib = N.lib()

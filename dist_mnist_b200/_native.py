@@ -28,6 +28,7 @@ APPLY_PER_PUSH, APPLY_MERGED = 0, 1
 DT_F32, DT_BF16 = 0, 1
 LR_CONSTANT, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_NATURAL_EXP, LR_POLYNOMIAL, LR_COSINE, LR_PIECEWISE = range(7)
 MAX_LR_BOUNDARIES = 8   # protocol.h kMaxLrBoundaries
+CLIP_OFF, CLIP_GLOBAL_NORM, CLIP_NORM, CLIP_VALUE = range(4)   # protocol.h GradClipKind
 
 
 class PushTarget(C.Structure):
@@ -157,6 +158,27 @@ class FusedParams(C.Structure):
         ("lane_rec", C.c_void_p),
         ("exit_counter", C.c_void_p),
         ("clear_stop", C.c_uint32), ("wait_acks", C.c_uint32),
+        ("clip_kind", C.c_int), ("clip_norm", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
+    ]
+
+
+GRAD_CLIP_MAX_VARS, GRAD_CLIP_MAX_SHARDS, GRAD_CLIP_BLOCKS = 8, 16, 132   # protocol.h kGradClip*
+
+
+class GradClipVar(C.Structure):
+    _fields_ = [("local", C.c_void_p), ("mailbox", C.c_void_p), ("mailbox_slot_stride", C.c_uint64),
+                ("rows", C.c_uint32), ("cols", C.c_uint32), ("ld", C.c_uint32), ("pad_", C.c_uint32)]
+
+
+class GradClipParams(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int), ("clip_norm", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
+        ("n_vars", C.c_int), ("n_shards", C.c_int), ("nslots", C.c_uint32), ("gpu_scope", C.c_uint32),
+        ("seq_ptr", C.c_void_p), ("partials", C.c_void_p),
+        ("var", GradClipVar * GRAD_CLIP_MAX_VARS),
+        ("flags", C.c_void_p * GRAD_CLIP_MAX_SHARDS),
+        ("flag_slot_stride", C.c_uint32 * GRAD_CLIP_MAX_SHARDS),
+        ("n_flags", C.c_uint32 * GRAD_CLIP_MAX_SHARDS),
     ]
 
 
@@ -169,6 +191,7 @@ _MIRRORS = {
     "PushTarget": PushTarget, "GemmParams": GemmParams, "HeadParams": HeadParams, "StepResult": StepResult,
     "PsItem": PsItem, "PsItemState": PsItemState, "PsServeParams": PsServeParams,
     "FusedSlice": FusedSlice, "FusedShard": FusedShard, "FusedParams": FusedParams, "FusedMaps": FusedMaps,
+    "GradClipVar": GradClipVar, "GradClipParams": GradClipParams,
 }
 
 WORKER_DEAD = 0xFFFFFFFF   # protocol.h kWorkerDead
@@ -273,6 +296,8 @@ def _declare(l: C.CDLL) -> None:
         "dm_exec_destroy": (i, [vp]),
         "dm_launch_fused": (i, [vp, vp, i, vp]),
         "dm_fused_max_lanes": (i, [i, i, C.POINTER(i)]),
+        "dm_fused_max_lanes_clip": (i, [i, i, C.POINTER(i)]),
+        "dm_launch_grad_clip": (i, [C.c_void_p, i, C.c_void_p]),
         "dm_fused_smem_bytes": (i, [i]),
         "dm_nvls_probe": (i, [i, sz, i, C.c_char_p, sz]),
         "dm_fexec_last_error": (C.c_char_p, []),

@@ -26,7 +26,8 @@ import torch
 
 from .cluster import ClusterSpec, Rendezvous, default_device_index
 from .models import mlp
-from .parallel.config import LR_SCHEDULES, SCHEDULE_PARAMS, EngineConfig, LrSchedule, OptimizerConfig
+from .parallel.config import (CLIP_KINDS, CLIP_PARAMS, LR_SCHEDULES, SCHEDULE_PARAMS, EngineConfig, GradClip,
+                              LrSchedule, OptimizerConfig)
 from .parallel.ps import ParameterServer
 from .parallel.worker import Worker
 from .session import train_loop
@@ -92,6 +93,24 @@ def lr_schedule_from_args(args) -> LrSchedule:
     return LrSchedule(kind, **{_SCHED_FLAGS[flag]: v for flag, v in given.items()})
 
 
+# gradient-clip flag -> GradClip parameter
+_CLIP_FLAGS = {"clip_norm": "clip_norm", "clip_value_min": "value_min", "clip_value_max": "value_max"}
+
+
+def grad_clip_from_args(args) -> GradClip:
+    """The gradient clip of `--clip_gradients` and its parameters; a parameter flag the chosen kind does not use, or any
+    of them without --clip_gradients, is an error."""
+    kind = args.clip_gradients
+    given = {flag: getattr(args, flag) for flag in _CLIP_FLAGS if getattr(args, flag) is not None}
+    for flag in given:
+        kinds = CLIP_PARAMS[_CLIP_FLAGS[flag]]
+        if kind is None:
+            raise ValueError(f"--{flag} needs --clip_gradients (gradient clipping is off)")
+        if kind not in kinds:
+            raise ValueError(f"--{flag} does not apply to --clip_gradients {kind} (only {', '.join(kinds)})")
+    return GradClip(kind, **{_CLIP_FLAGS[flag]: v for flag, v in given.items()})
+
+
 def optimizer_config_from_args(args) -> OptimizerConfig:
     """The optimizer every task derives from the command line; a hyper-parameter flag the chosen optimizer does not
     use is an error."""
@@ -105,7 +124,8 @@ def optimizer_config_from_args(args) -> OptimizerConfig:
                            initial_accumulator_value=args.initial_accumulator_value,
                            schedule=lr_schedule_from_args(args),
                            moving_average_decay=args.moving_average_decay,
-                           moving_average_num_updates=args.moving_average_num_updates != "none")
+                           moving_average_num_updates=args.moving_average_num_updates != "none",
+                           clip=grad_clip_from_args(args))
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -162,6 +182,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--moving_average_num_updates", choices=["global_step", "none"], default=None,
                    help="global_step (default): decay = min(D, (1 + step) / (10 + step)), TF1's num_updates=global_step;"
                         " none: decay = D")
+    # gradient clipping on the worker before the push (TF1's compute_gradients -> clip_by_* -> apply_gradients)
+    p.add_argument("--clip_gradients", choices=list(CLIP_KINDS), default=None,
+                   help="global_norm: tf.clip_by_global_norm; norm: tf.clip_by_norm per variable; value: "
+                        "tf.clip_by_value (unset: off; fused engine and cpu backend)")
+    p.add_argument("--clip_norm", type=float, default=None, help="global_norm / norm (required): finite, > 0")
+    p.add_argument("--clip_value_min", type=float, default=None, help="value (required): finite, <= --clip_value_max")
+    p.add_argument("--clip_value_max", type=float, default=None, help="value (required): finite")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")

@@ -26,6 +26,8 @@ cudaError_t preload_head_kernels();
 cudaError_t preload_ps_kernels();
 cudaError_t preload_p2p_kernels();
 cudaError_t launch_head(const HeadParams& p, cudaStream_t stream);
+cudaError_t preload_grad_clip_kernels();
+cudaError_t launch_grad_clip(const GradClipParams& p, int stage, cudaStream_t stream);
 cudaError_t launch_accuracy(const float* logits, const float* labels, int B, int C, uint32_t* correct,
                             cudaStream_t stream);
 cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cudaStream_t stream);
@@ -73,6 +75,8 @@ int dm_sizeof(const char* name) {
   if (!strcmp(name, "FusedShard")) return sizeof(FusedShard);
   if (!strcmp(name, "FusedParams")) return sizeof(FusedParams);
   if (!strcmp(name, "FusedMaps")) return sizeof(FusedMaps);
+  if (!strcmp(name, "GradClipVar")) return sizeof(GradClipVar);
+  if (!strcmp(name, "GradClipParams")) return sizeof(GradClipParams);
   return -1;
 }
 
@@ -258,6 +262,7 @@ int dm_prepare_kernels(int dev) {
   // CUDA loads kernels lazily; a first launch while a persistent PS kernel is resident can deadlock on the
   // context-wide synchronisation the load needs — so load everything up front.
   DM_CUDA(dm::preload_head_kernels());
+  DM_CUDA(dm::preload_grad_clip_kernels());
   DM_CUDA(dm::preload_ps_kernels());
   DM_CUDA(dm::preload_p2p_kernels());
   DM_CUDA(dm::prepare_fused_kernel());
@@ -278,6 +283,11 @@ int dm_fused_max_lanes(int dev, int batch, int* out) {
   DM_CUDA(dm::fused_max_lanes(batch, out));
   return 0;
 }
+int dm_fused_max_lanes_clip(int dev, int batch, int* out) {
+  DM_CUDA(cudaSetDevice(dev));
+  DM_CUDA(dm::fused_max_lanes_clip(batch, out));
+  return 0;
+}
 int dm_fused_smem_bytes(int batch) { return static_cast<int>(dm::fused_smem_bytes(batch)); }
 
 int dm_launch_gemm(const void* tmA, const void* tmB, const void* params, int dtype, int a_mn, int b_mn, int splits,
@@ -288,6 +298,13 @@ int dm_launch_gemm(const void* tmA, const void* tmB, const void* params, int dty
   memcpy(&b, tmB, sizeof(b));
   memcpy(&p, params, sizeof(p));
   DM_CUDA(dm::launch_gemm(a, b, p, dtype, a_mn != 0, b_mn != 0, splits, static_cast<cudaStream_t>(stream)));
+  return 0;
+}
+// Graph engine gradient clipping tail (clip_sm90.cu): stage 0 sums of squares, 1 clip into the mailbox, 2 flags
+int dm_launch_grad_clip(const void* params, int stage, void* stream) {
+  dm::GradClipParams p;
+  memcpy(&p, params, sizeof(p));
+  DM_CUDA(dm::launch_grad_clip(p, stage, static_cast<cudaStream_t>(stream)));
   return 0;
 }
 int dm_launch_head(const void* params, void* stream) {

@@ -17,9 +17,10 @@ struct FusedMaps {
 
 // Batch B <= 32 runs the one-tile instantiation of the kernel, 32 < B <= 256 the multi-tile one; the functions that
 // take B answer for the instantiation that batch runs.
-cudaError_t prepare_fused_kernel();   // both instantiations: shared-memory opt-in + force-load
+cudaError_t prepare_fused_kernel();   // every instantiation: shared-memory opt-in + force-load
 size_t fused_smem_bytes(int B);
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream);
 cudaError_t fused_max_lanes(int B, int* out);
+cudaError_t fused_max_lanes_clip(int B, int* out);   // the same for the gradient-clipping instantiations
 
 }  // namespace dm

@@ -46,6 +46,7 @@
 // (gemm_sm90.cu, head_sm90.cu) chained in a CUDA graph.
 #include "common.cuh"
 #include "fused.h"
+#include "grad_clip.cuh"
 
 namespace dm {
 
@@ -93,6 +94,13 @@ constexpr uint32_t kFsMultiSmemBytes = kOffAccScal + 2 * 4 + 1024;
 static_assert(kFsMultiSmemBytes <= 227 * 1024, "shared memory budget (multi-tile)");
 template <int kMaxTiles>
 constexpr uint32_t fs_smem_bytes() { return kMaxTiles == 1 ? kFsSmemBytes : kFsMultiSmemBytes; }
+// Gradient clipping (fused_step_kernel<*, true>): the per-variable sums of squares of a step sit in the alignment gap
+// before the staging tile, so that the clip instantiations have the shared-memory footprint (and the residency beside
+// the ps serve kernel) of the unclipped ones.
+constexpr int kFsClipVars = 4;                                        // hid_w, hid_b, sm_w, sm_b
+constexpr uint32_t kOffClipWarp = (kOffRawBl + 64 + 15) & ~15u;       // [4][4]      warp partials of this CTA
+constexpr uint32_t kOffClipPart = kOffClipWarp + 4 * kFsClipVars * 4; // [8][4]      CTA partials (DSMEM all-gather)
+static_assert(kOffClipPart + kFusedCluster * kFsClipVars * 4 <= kOffStage, "the clip partials fit before the staging tile");
 
 // pre^T block [64 x 32] += W [64 x k8] . x [32 x k8]^T, both operands from shared memory (tf32)
 __device__ __forceinline__ void fs_mma_m64n32(float (&d)[4][4], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
@@ -171,7 +179,14 @@ __device__ __forceinline__ void fs_wait_acks(const FusedParams& p, uint32_t need
 }
 
 // kMaxTiles == 1: B <= 32, one row tile per step. kMaxTiles > 1: T = ceil(B / 32) row tiles per step (see the header).
-template <int kMaxTiles>
+// kClip: the pushed gradient is clipped first (FusedParams::clip_kind, TF1's clip_by_global_norm / clip_by_norm per
+// variable / clip_by_value). In the last row tile every CTA sums the squares of the gradient elements it pushes, per
+// variable: hid_w over its staging tile, sm_w / hid_b over its 16 hidden units, sm_b on CTA 0. The 4 partials go to
+// every CTA through DSMEM, one more cluster barrier (the norm barrier) follows, and every CTA adds the 8 x 4 partials
+// in the same order, so all agree on the scale bit for bit. The staging tile is then scaled in place before warp 4
+// stores it, and the small gradients are pushed after the norm barrier (still before barrier #3). CLIP_VALUE clamps
+// element-wise and needs neither the sums nor the barrier.
+template <int kMaxTiles, bool kClip>
 __global__ void __launch_bounds__(kFsThreads, 1)
 fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant__ FusedParams p) {
   constexpr bool kMulti = kMaxTiles > 1;
@@ -357,6 +372,9 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
           __syncwarp();
         }
       }
+      if constexpr (kClip) {
+        if (p.clip_kind != CLIP_VALUE) cluster_sync_all();   // the norm barrier (see the head warpgroup)
+      }
       // ---- the gradient push: the epilogue warps have staged the dW tile (swizzled, fence.proxy.async'ed) ----
       named_bar_sync(2, 160);
       {
@@ -435,6 +453,69 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
     float* acc = reinterpret_cast<float*>(smem + kOffAcc);   // multi-tile running sums (see kOffAcc)
     float* acc_dbl = reinterpret_cast<float*>(smem + kOffAccDbl);
     float* acc_scal = reinterpret_cast<float*>(smem + kOffAccScal);
+    // kClip: this thread's small gradients out of the landing zones (the same sums, in the same order, as the unclipped
+    // push): sm_w value vg of unit u, value vg + 8 of it or hid_b (vg == 3), and sm_b (CTA 0, et < C). They are read
+    // once for the norms and again for the push, so that no register holds them across the dW GEMM.
+    auto small_grads = [&](float& s0, float& s1, float& sbl) {
+      const int u = et & 15, vg = et >> 4;
+      s0 = 0.f;
+      s1 = 0.f;
+#pragma unroll
+      for (int s = 0; s < kFusedCluster; ++s) {
+        s0 += sg[(s * 16 + u) * kFsPart + vg];
+        if (vg < 4) s1 += sg[(s * 16 + u) * kFsPart + vg + 8];
+      }
+      sbl = 0.f;
+      if (rank == 0 && et < C) {
+#pragma unroll
+        for (int src = 0; src < kFusedCluster; ++src) sbl += dbl[src * kFsMaxC + et];
+      }
+    };
+    // kClip: the per-warp sum of v into warp partial `var` of this CTA (hid_w 0, hid_b 1, sm_w 2, sm_b 3)
+    float* clip_warp = reinterpret_cast<float*>(smem + kOffClipWarp);
+    auto clip_warp_sum = [&](float v, int var) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) clip_warp[q * kFsClipVars + var] = v;
+    };
+    // kClip: the clip factor of each variable (hid_w, hid_b, sm_w, sm_b) once every warp has stored its partials of
+    // the small variables (after barrier #2) and this thread's sum of squares of its hid_w elements is `ssq_w`.
+    // CLIP_GLOBAL_NORM: the common scale; CLIP_NORM: max(norm, clip_norm) per variable; CLIP_VALUE: unused.
+    auto clip_factors = [&](float ssq_w) -> float4 {
+      float4 fac = make_float4(1.f, 1.f, 1.f, 1.f);
+      if (p.clip_kind == CLIP_VALUE) return fac;
+      const float* cw = clip_warp;
+      const float* cp = reinterpret_cast<const float*>(smem + kOffClipPart);
+      clip_warp_sum(ssq_w, 0);
+      named_bar_sync(1, 128);
+      if (et < kFsClipVars) {
+        const float c = (cw[et] + cw[kFsClipVars + et]) + (cw[2 * kFsClipVars + et] + cw[3 * kFsClipVars + et]);
+#pragma unroll
+        for (uint32_t d = 0; d < kFusedCluster; ++d)
+          st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffClipPart + (rank * kFsClipVars + et) * 4u, d), c);
+      }
+      cluster_sync_all();   // the norm barrier: every CTA's partials have landed in every CTA
+      float tot[kFsClipVars];
+#pragma unroll
+      for (int v = 0; v < kFsClipVars; ++v) {
+        float a = 0.f;
+#pragma unroll
+        for (int src = 0; src < kFusedCluster; ++src) a += cp[src * kFsClipVars + v];
+        tot[v] = a;
+      }
+      const float cn = p.clip_norm;
+      if (p.clip_kind == CLIP_GLOBAL_NORM) {
+        const float sc = clip_global_scale(((tot[0] + tot[1]) + tot[2]) + tot[3], cn);
+        fac = make_float4(sc, sc, sc, sc);
+      } else {
+        fac = make_float4(clip_norm_divisor(tot[0], cn), clip_norm_divisor(tot[1], cn), clip_norm_divisor(tot[2], cn),
+                          clip_norm_divisor(tot[3], cn));
+      }
+      return fac;
+    };
+    auto clip_value = [&](float g, float f) -> float {
+      return clip_element(p.clip_kind, g, f, p.clip_norm, p.clip_min, p.clip_max);
+    };
 
     for (uint32_t jl = 0; cur != kFusedNoStep; ++jl) {
       const uint32_t seq = p.seq_base + cur + 1u;
@@ -663,7 +744,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
         if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 6] = clock64();
 
         // ---- small gradients: sum the 8 sources for my 16 hidden units and push them ----
-        if (last) {
+        if (!kClip && last) {
           const FsPush pw_l = fs_resolve(p.shard[p.shard_wl].push, push_seq);
           const FsPush pb_h = fs_resolve(p.shard[p.shard_bh].push, push_seq);
           const int u = et & 15, vg = et >> 4;   // values vg (0..7) and vg + 8 (8..11) of unit u
@@ -688,11 +769,29 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, s);
           }
         }
+        // kClip: only their squares count now (warp partials of hid_b / sm_w / sm_b); they are pushed once the clip is
+        // known, after the norm barrier
+        if (kClip && last && p.clip_kind != CLIP_VALUE) {
+          const int u = et & 15, vg = et >> 4;
+          const int unit = static_cast<int>(rank) * 16 + u;
+          float s0, s1, sbl, ssq_bh = 0.f, ssq_wl = 0.f, ssq_bl = 0.f;
+          small_grads(s0, s1, sbl);
+          if (unit < H) {
+            if (vg < C) ssq_wl = s0 * s0;
+            if (vg < 3 && vg + 8 < C) ssq_wl += s1 * s1;
+            if (vg == 3) ssq_bh = s1 * s1;
+          }
+          if (rank == 0 && et < C) ssq_bl = sbl * sbl;
+          clip_warp_sum(ssq_bh, 1);
+          clip_warp_sum(ssq_wl, 2);
+          clip_warp_sum(ssq_bl, 3);
+        }
 
         // ---- dW^T tile of my K-slice: wgmma -> registers -> swizzled staging tile; warp 4 TMA-stores it (the push) ----
         fence_proxy_async_smem_cta();   // generic-proxy (DSMEM) writes of dpre^T -> tensor-core reads
         mbar_wait(bar_xmn, (jl * static_cast<uint32_t>(T) + static_cast<uint32_t>(t)) & 1u);
         if (dbg && et == 0 && jl < 4) p.debug_ts[jl * kTs + 7] = clock64();
+        float4 cfac = make_float4(1.f, 1.f, 1.f, 1.f);   // kClip: clip_factors of this step
         if (nkc > 0) {
           // D[feature f][hidden h] = sum_b x[b][f] dpre^T[h][b]: M = my features (m64 blocks), N = 128 hidden units,
           // K = 32 batch rows. A = x^T from registers, read out of the K-major x tile ([b][f], 128-byte swizzled);
@@ -752,6 +851,66 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
                 }
             }
           }
+          if constexpr (kClip) {
+            if (last) {
+              // Only the elements the TMA store pushes (hidden rows < H, features < I) count toward the norms. The loop
+              // above has written the step's dW (summed over the row tiles) into the staging tile, which is read and
+              // scaled in place as float4s by a rolled loop: an unrolled pass over the wgmma fragments instead costs
+              // more than twice the step time at batch 32 (measured), from the code it adds to the step loop.
+              const int n4 = nkc * static_cast<int>(kFsWChunk / 16);
+              named_bar_sync(1, 128);   // every thread's part of the tile is in place (the passes below cross threads)
+              if (p.clip_kind != CLIP_VALUE) {   // (value clamps each element: no sums, no norm barrier)
+                float ssq_w = 0.f;
+                for (int i4 = et; i4 < n4; i4 += 128) {
+                  const int i = i4 / static_cast<int>(kFsWChunk / 16), o = (i4 % static_cast<int>(kFsWChunk / 16)) * 16;
+                  const int h = o >> 7, fl = (((o >> 4) & 7) ^ (h & 7)) << 2;   // inverse of sw128_offset
+                  const float4 v = *reinterpret_cast<const float4*>(smem + kOffStage + i * kFsWChunk + o);
+                  if (h < H && (sl.kc_begin + i) * 32 + fl < p.I) {   // I % 4 == 0: a float4 is in or out as a whole
+                    ssq_w = fmaf(v.x, v.x, ssq_w);
+                    ssq_w = fmaf(v.y, v.y, ssq_w);
+                    ssq_w = fmaf(v.z, v.z, ssq_w);
+                    ssq_w = fmaf(v.w, v.w, ssq_w);
+                  }
+                }
+                cfac = clip_factors(ssq_w);
+              }
+              for (int i4 = et; i4 < n4; i4 += 128) {
+                const int i = i4 / static_cast<int>(kFsWChunk / 16), o = (i4 % static_cast<int>(kFsWChunk / 16)) * 16;
+                float4* st = reinterpret_cast<float4*>(smem + kOffStage + i * kFsWChunk + o);
+                float4 v = *st;
+                v.x = clip_value(v.x, cfac.x);
+                v.y = clip_value(v.y, cfac.x);
+                v.z = clip_value(v.z, cfac.x);
+                v.w = clip_value(v.w, cfac.x);
+                *st = v;
+              }
+            }
+          }
+        }
+        if constexpr (kClip) {
+          if (last) {
+            if (nkc == 0) cfac = clip_factors(0.f);   // no dW tile, the same norm barrier
+            // the small gradients, clipped, after the norm barrier and before barrier #3 (the publisher's flags)
+            const FsPush pw_l = fs_resolve(p.shard[p.shard_wl].push, push_seq);
+            const FsPush pb_h = fs_resolve(p.shard[p.shard_bh].push, push_seq);
+            const int u = et & 15, vg = et >> 4;
+            float cg0, cg1, cgl;
+            small_grads(cg0, cg1, cgl);
+            const int unit = static_cast<int>(rank) * 16 + u;
+            if (unit < H) {
+              if (vg < C)
+                fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg) * H + unit,
+                              clip_value(cg0, cfac.z));
+              if (vg < 3 && vg + 8 < C)
+                fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg + 8) * H + unit,
+                              clip_value(cg1, cfac.z));
+              if (vg == 3) fs_push_value(p.shard[p.shard_bh].push, pb_h.base + p.off_bh + unit, clip_value(cg1, cfac.y));
+            }
+            if (rank == 0 && et < C) {
+              const FsPush pb_l = fs_resolve(p.shard[p.shard_bl].push, push_seq);
+              fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, clip_value(cgl, cfac.w));
+            }
+          }
         }
         if (last) {
           fence_proxy_async_smem_cta();  // staging writes -> visible to the TMA engine (shared memory only: does not
@@ -790,25 +949,27 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-template <int kMaxTiles>
+template <int kMaxTiles, bool kClip>
 static cudaError_t prepare_fused_instance() {
-  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(fs_smem_bytes<kMaxTiles>()));
   if (e != cudaSuccess) return e;
   cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles>);   // force-load (see preload_ps_kernels)
+  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip>);   // force-load (see preload_ps_kernels)
 }
 
 cudaError_t prepare_fused_kernel() {
-  const cudaError_t e = prepare_fused_instance<1>();
-  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles>();
+  cudaError_t e = prepare_fused_instance<1, false>();
+  if (e == cudaSuccess) e = prepare_fused_instance<kFsMaxTiles, false>();
+  if (e == cudaSuccess) e = prepare_fused_instance<1, true>();
+  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, true>();
 }
 
 static bool fused_multi_tile(int B) { return B > 32; }
 
 size_t fused_smem_bytes(int B) { return fused_multi_tile(B) ? fs_smem_bytes<kFsMaxTiles>() : fs_smem_bytes<1>(); }
 
-// One launch config for both instantiations: `lanes` clusters of 8 CTAs.
+// One launch config for every instantiation: `lanes` clusters of 8 CTAs.
 static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t stream, cudaLaunchAttribute* attr) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(kFusedCluster, lanes, 1);
@@ -826,22 +987,35 @@ static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t str
 
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
   if (lanes < 1 || p.B < 1 || p.B > 32 * kFsMaxTiles || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 ||
-      (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1)
+      (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1 || p.clip_kind < CLIP_OFF ||
+      p.clip_kind > CLIP_VALUE)
     return cudaErrorInvalidValue;
   for (int r = 0; r < kFusedCluster; ++r)
     if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
+  const bool clip = p.clip_kind != CLIP_OFF;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
-  if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles>, maps, p);
-  return cudaLaunchKernelEx(&cfg, fused_step_kernel<1>, maps, p);
+  if (clip) {
+    if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles, true>, maps, p);
+    return cudaLaunchKernelEx(&cfg, fused_step_kernel<1, true>, maps, p);
+  }
+  if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles, false>, maps, p);
+  return cudaLaunchKernelEx(&cfg, fused_step_kernel<1, false>, maps, p);
 }
 
 // How many clusters of the fused kernel that runs batch B can be co-resident on the device (upper bound for `lanes`).
 cudaError_t fused_max_lanes(int B, int* out) {
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles>, &cfg);
-  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1>, &cfg);
+  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles, false>, &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1, false>, &cfg);
+}
+
+cudaError_t fused_max_lanes_clip(int B, int* out) {
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
+  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles, true>, &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1, true>, &cfg);
 }
 
 }  // namespace dm

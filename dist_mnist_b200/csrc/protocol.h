@@ -294,6 +294,42 @@ struct FusedParams {
   uint32_t clear_stop;     // 1: the last cluster to exit zeroes *stop_word (last launch of a run)
   uint32_t wait_acks;      // 1: the last cluster to exit returns only after every shard has acknowledged every push made
                            //    so far (the launch then covers the ps-side apply of its last step: timed regions)
+  // gradient clipping before the push (TF1 clip_by_global_norm / clip_by_norm per variable / clip_by_value; appended,
+  // so that no earlier field moves). CLIP_OFF runs the unclipped instantiations.
+  int clip_kind;           // GradClipKind
+  float clip_norm;         // CLIP_GLOBAL_NORM, CLIP_NORM: > 0
+  float clip_min, clip_max;  // CLIP_VALUE
+};
+enum GradClipKind : int {
+  CLIP_OFF = 0,
+  CLIP_GLOBAL_NORM = 1,
+  CLIP_NORM = 2,
+  CLIP_VALUE = 3,
+};
+
+// Gradient clipping tail of the graph engine (clip_sm90.cu): the step's epilogues push into worker-local buffers, these
+// kernels clip them into this worker's mailbox slot on every shard and release the slot's flags.
+constexpr int kGradClipMaxVars = 8;
+constexpr int kGradClipMaxShards = 16;
+constexpr int kGradClipBlocks = 132;     // blocks of the sum-of-squares and apply kernels (partials: [blocks][vars])
+struct GradClipVar {
+  float* local;                  // the variable in this slot's local gradient buffer (arena layout of its shard)
+  float* mailbox;                // the variable in slot 0 of this worker's mailbox on its shard
+  uint64_t mailbox_slot_stride;  // elements between mailbox slots (the shard's arena)
+  uint32_t rows, cols, ld, pad_;
+};
+struct GradClipParams {
+  int kind;                      // GradClipKind (not CLIP_OFF)
+  float clip_norm, clip_min, clip_max;
+  int n_vars, n_shards;
+  uint32_t nslots;               // mailbox slots: the slot of push seq is seq % nslots
+  uint32_t gpu_scope;            // 1: every shard is on this GPU (gpu-scope fence suffices)
+  const uint32_t* seq_ptr;       // this ring slot's current push sequence number
+  float* partials;               // [kGradClipBlocks][kGradClipMaxVars] worker-local scratch
+  GradClipVar var[kGradClipMaxVars];
+  uint32_t* flags[kGradClipMaxShards];          // slot-0 flags of this worker on each shard
+  uint32_t flag_slot_stride[kGradClipMaxShards];
+  uint32_t n_flags[kGradClipMaxShards];
 };
 
 }  // namespace dm

@@ -222,3 +222,36 @@ def manual_loss_and_grads(spec: MLPSpec, params: Dict[str, torch.Tensor], x: tor
         if i > 0:
             d = (d @ params[wn]) * (acts[i] > 0).to(d.dtype)
     return loss, grads, logits
+
+
+def clip_gradients(grads: Dict[str, torch.Tensor], clip) -> Dict[str, torch.Tensor]:
+    """TF1's gradient clipping in fp32 (the reference of every engine's clip), applied to the gradients of the mean
+    loss over the whole batch, keyed by variable name. `clip` is a `parallel.config.GradClip`:
+
+    * "global_norm" (`tf.clip_by_global_norm`): n = sqrt(sum over the variables of sum(g*g)),
+      scale = clip_norm * min(1/n, 1/clip_norm) (NaN when n is inf or NaN), g' = g * scale. An unclipped step is still
+      multiplied by clip_norm * fl(1/clip_norm), which need not be 1.
+    * "norm" (`tf.clip_by_norm`, each variable on its own): l2 = sum(g*g), norm = sqrt(l2) if l2 > 0 else l2,
+      g' = (g * clip_norm) / max(norm, clip_norm).
+    * "value" (`tf.clip_by_value`): g' = max(min(g, value_max), value_min)."""
+    f32 = torch.float32
+    g32 = {k: g.detach().to(f32) for k, g in grads.items()}
+    if clip.kind == "value":
+        lo, hi = torch.tensor(clip.value_min, dtype=f32), torch.tensor(clip.value_max, dtype=f32)
+        return {k: torch.maximum(torch.minimum(g, hi), lo) for k, g in g32.items()}
+    c = torch.tensor(clip.clip_norm, dtype=f32)
+    if clip.kind == "global_norm":
+        total = torch.zeros((), dtype=f32)
+        for g in g32.values():
+            total = total + (g * g).sum()
+        n = torch.sqrt(total)
+        scale = c * torch.minimum(1.0 / n, 1.0 / c) + (n - n)
+        return {k: g * scale for k, g in g32.items()}
+    if clip.kind == "norm":
+        out = {}
+        for k, g in g32.items():
+            l2 = (g * g).sum()
+            norm = torch.sqrt(l2) if bool(l2 > 0) else l2
+            out[k] = (g * c) / torch.maximum(norm, c)
+        return out
+    raise ValueError(f"unknown gradient clip {clip.kind!r}")

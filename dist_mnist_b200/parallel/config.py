@@ -173,6 +173,75 @@ def _f32(x: float) -> float:
     return struct.unpack("f", struct.pack("f", x))[0]
 
 
+CLIP_KINDS = ("global_norm", "norm", "value")
+_NATIVE_CLIPS = {None: N.CLIP_OFF, "global_norm": N.CLIP_GLOBAL_NORM, "norm": N.CLIP_NORM, "value": N.CLIP_VALUE}
+# clip parameter -> the kinds that use it
+CLIP_PARAMS = {"clip_norm": ("global_norm", "norm"), "value_min": ("value",), "value_max": ("value",)}
+
+
+@dataclass(frozen=True)
+class GradClip:
+    """Gradient clipping on the worker, between TF1's `opt.compute_gradients(loss)` and `opt.apply_gradients(...)`:
+    "global_norm" is `tf.clip_by_global_norm(grads, clip_norm)`, "norm" is `tf.clip_by_norm(g, clip_norm)` applied to
+    every model variable separately, "value" is `tf.clip_by_value(g, value_min, value_max)`. `kind` None = off.
+
+    The clip applies to the gradient of the mean loss over the whole batch, the one that is pushed. The ps never sees
+    it: it combines with every optimizer, schedule, moving average, apply mode and sharding. `mlp.clip_gradients` is
+    the fp32 reference. A parameter the kind does not use is an error."""
+    kind: Optional[str] = None
+    clip_norm: Optional[float] = None
+    value_min: Optional[float] = None
+    value_max: Optional[float] = None
+
+    def __post_init__(self):
+        if self.kind not in _NATIVE_CLIPS:
+            raise ValueError(f"unknown gradient clip {self.kind!r} ({' | '.join(CLIP_KINDS)})")
+        for name, kinds in CLIP_PARAMS.items():
+            v = getattr(self, name)
+            if v is None:
+                if self.kind in kinds:
+                    raise ValueError(f"gradient clip {self.kind!r} needs {name}")
+                continue
+            if self.kind not in kinds:
+                what = "gradient clipping is off" if self.kind is None else f"gradient clip {self.kind!r}"
+                raise ValueError(f"{what}: {name} does not apply (only {', '.join(kinds)})")
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+                raise ValueError(f"{name} must be a finite number, got {v!r}")
+            object.__setattr__(self, name, float(v))
+        if self.clip_norm is not None and not self.clip_norm > 0:
+            raise ValueError(f"clip_norm must be > 0, got {self.clip_norm!r}")
+        if self.kind == "value" and not self.value_min <= self.value_max:
+            raise ValueError(f"value_min ({self.value_min}) must not exceed value_max ({self.value_max})")
+
+    @property
+    def enabled(self) -> bool:
+        return self.kind is not None
+
+    @property
+    def native_kind(self) -> int:
+        return _NATIVE_CLIPS[self.kind]
+
+    def apply(self, grads):
+        """The reference clip (mlp.clip_gradients) of a {variable name: gradient} dict; unchanged when off."""
+        from ..models import mlp
+
+        return mlp.clip_gradients(grads, self) if self.enabled else grads
+
+    def fill_native(self, P) -> None:
+        """Write this clip into a FusedParams."""
+        P.clip_kind = self.native_kind
+        P.clip_norm = self.clip_norm or 0.0
+        P.clip_min = self.value_min or 0.0
+        P.clip_max = self.value_max or 0.0
+
+    def as_dict(self) -> dict:
+        return asdict(self)
+
+    @classmethod
+    def from_dict(cls, d: Optional[dict]) -> "GradClip":
+        return cls(**d) if d else cls()
+
+
 @dataclass(frozen=True)
 class OptimizerConfig:
     """Reference: `tf.train.AdamOptimizer(FLAGS.learning_rate)` with TF defaults (DS:102); SGD is the
@@ -199,6 +268,9 @@ class OptimizerConfig:
     # variable's initial value and moves by shadow -= (shadow - p) * (1 - d). None = off.
     moving_average_decay: Optional[float] = None
     moving_average_num_updates: bool = True   # d = min(decay, (1 + n) / (10 + n)), n = global step; False: d = decay
+    # gradient clipping on the worker before the push (TF1 clip_by_global_norm / clip_by_norm / clip_by_value); the
+    # ps does not use it, and workers of one session may clip differently
+    clip: GradClip = GradClip()
 
     def __post_init__(self):
         if self.math not in ("fast", "ieee"):
@@ -216,6 +288,8 @@ class OptimizerConfig:
             raise ValueError("initial_accumulator_value must be positive (Adagrad divides by its square root)")
         if not isinstance(self.schedule, LrSchedule):
             raise ValueError(f"schedule must be an LrSchedule, got {type(self.schedule).__name__}")
+        if not isinstance(self.clip, GradClip):
+            raise ValueError(f"clip must be a GradClip, got {type(self.clip).__name__}")
         d = self.moving_average_decay
         if d is not None:
             if isinstance(d, bool) or not isinstance(d, (int, float)) or not 0.0 < d < 1.0:
@@ -335,6 +409,9 @@ class EngineConfig:
             if opt.moving_averages:
                 raise ValueError("push_mode='atomic' has no ps-side apply to update moving averages after; "
                                  "moving_average_decay needs push_mode='mailbox'")
+            if opt.clip.enabled:
+                raise ValueError("push_mode='atomic' applies every gradient tile as it is produced, before a clip "
+                                 "could know its scale; gradient clipping needs push_mode='mailbox'")
             if self.dtype != "fp32":
                 raise ValueError("push_mode='atomic' updates only the fp32 master copy; use dtype fp32")
             if self.backend != "cuda":

@@ -108,6 +108,19 @@ def usable_cores() -> int:
     return n
 
 
+class _GradClipPlan:
+    """One kernel of the graph engine's gradient-clipping tail (csrc/clip_sm90.cu): stage 0 sums of squares, 1 the
+    clipped copy into the mailbox, 2 the release of the flags."""
+
+    def __init__(self, params: N.GradClipParams, stage: int):
+        self.params, self.stage = params, stage
+        self.name = ("clip_ssq", "clip_apply", "clip_release")[stage]
+
+    def launch(self, stream: Optional[int] = None) -> None:
+        s = N.current_stream_ptr() if stream is None else stream
+        N.check(N.lib().dm_launch_grad_clip(C.addressof(self.params), self.stage, s), f"launch {self.name}")
+
+
 class Worker:
     def __init__(self, cluster: ClusterSpec, task_index: int, spec: MLPSpec, opt: OptimizerConfig,
                  cfg: EngineConfig, batch_size: int = 32, device: int = 0, rdv: Optional[Rendezvous] = None,
@@ -171,11 +184,12 @@ class Worker:
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: {desc}")
             # the ps applies the rule, the chief initialises its slots: with Momentum / Adagrad / RMSProp on either
             # side both must run the same optimizer (an Adam / SGD pairing is not checked, as before)
-            ps_opt = desc.get("optimizer") or {}
-            if ((ps_opt.get("kind") in TF1_SLOT_KINDS or self.opt.kind in TF1_SLOT_KINDS)
-                    and ps_opt != self.opt.as_dict()):
+            # (gradient clipping runs on the worker alone: workers may clip differently from the ps flags and each other)
+            ps_opt = {n: v for n, v in (desc.get("optimizer") or {}).items() if n != "clip"}
+            my_opt = {n: v for n, v in self.opt.as_dict().items() if n != "clip"}
+            if ((ps_opt.get("kind") in TF1_SLOT_KINDS or self.opt.kind in TF1_SLOT_KINDS) and ps_opt != my_opt):
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: optimizer "
-                                   f"{ps_opt}, this worker has {self.opt.as_dict()}")
+                                   f"{ps_opt}, this worker has {my_opt}")
             # the ps evaluates the learning-rate schedule; a worker that reports lr_at(global_step) must agree on it
             ps_sched = LrSchedule.from_dict(ps_opt.get("schedule"))
             if ps_sched != self.opt.schedule or (not ps_sched.constant and ps_opt.get("lr") != self.opt.lr):
@@ -494,6 +508,50 @@ class Worker:
                           and self.cluster.num_workers == 1)
         return t
 
+    def _clip_target(self, k: int, seq_ptr: int, local: Dict[int, torch.Tensor],
+                     flags: Dict[int, torch.Tensor]) -> N.PushTarget:
+        """Graph engine with gradient clipping: the push target of shard k redirected into this ring slot's local
+        gradient buffer (arena layout of the shard; slot stride 0) with worker-local flags. The epilogues run unchanged
+        (the head still waits for the mailbox slot it will reuse); the clip tail moves the clipped gradient into the
+        mailbox and releases the ps's flags."""
+        t = self._push_target(k, seq_ptr)
+        t.base, t.slot_stride = local[k].data_ptr(), 0
+        t.flags, t.flag_slot_stride = flags[k].data_ptr(), 0
+        return t
+
+    def _clip_tail(self, seq_ptr: int, local: Dict[int, torch.Tensor], partials: torch.Tensor) -> List["_GradClipPlan"]:
+        """The clip tail of one ring slot's step graph (csrc/clip_sm90.cu): sums of squares (not for "value"), the
+        clipped copy into the mailbox slot of push *seq_ptr, the release of that slot's flags on every shard."""
+        clip, ns, w = self.opt.clip, self.cfg.nslots, self.task_index
+        P = N.GradClipParams()
+        P.kind, P.clip_norm = clip.native_kind, clip.clip_norm or 0.0
+        P.clip_min, P.clip_max = clip.value_min or 0.0, clip.value_max or 0.0
+        P.nslots, P.seq_ptr, P.partials = ns, seq_ptr, partials.data_ptr()
+        variables = list(self.layout.by_name.values())
+        if len(variables) > N.GRAD_CLIP_MAX_VARS or len(self.inbox_order) > N.GRAD_CLIP_MAX_SHARDS:
+            raise ValueError(f"gradient clipping on the graph engine handles at most {N.GRAD_CLIP_MAX_VARS} variables "
+                             f"and {N.GRAD_CLIP_MAX_SHARDS} ps shards")
+        P.n_vars = len(variables)
+        for i, vl in enumerate(variables):
+            arena = self.ps_desc[vl.ps]["arena_elems"]
+            v = P.var[i]
+            v.local = local[vl.ps].data_ptr() + vl.offset * 4
+            v.mailbox = self.ps_segs[vl.ps].addr("mailbox", (w * ns * arena + vl.offset) * 4)
+            v.mailbox_slot_stride = arena
+            v.rows, v.cols, v.ld = vl.rows, vl.cols, vl.ld if len(vl.spec.shape) == 2 else vl.cols
+        P.n_shards = len(self.inbox_order)
+        scope = 1
+        for j, k in enumerate(self.inbox_order):
+            desc = self.ps_desc[k]
+            ni = max(desc.get("n_flags", desc["n_items"]), 1)
+            P.flags[j] = self.ps_segs[k].addr("flags", w * ns * ni * 4)
+            P.flag_slot_stride[j] = ni
+            P.n_flags[j] = self.layout.shards[k].n_flags
+            scope &= self._push_target(k, seq_ptr).gpu_scope
+        P.gpu_scope = scope
+        stages = (1, 2) if clip.kind == "value" else (0, 1, 2)
+        return [_GradClipPlan(P, st) for st in stages]
+
     def _weight_ptr(self, vl: VarLayout) -> int:
         seg = self.ps_segs[vl.ps]
         if self.cfg.dtype == "bf16":
@@ -545,9 +603,28 @@ class Worker:
             num_classes=spec.num_classes, loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT,
             act_bf16=cfg.dtype == "bf16", compute_grads=False, ldh=self.act[L - 1].shape[1]))
         torch.cuda.synchronize(self.device)
+        clip = self.opt.clip.enabled
+        # gradient clipping: per ring slot, a local gradient buffer per shard (the epilogues' push target), worker-local
+        # flags they release, and the clip tail's per-block partial sums (steps of different slots run concurrently)
+        self._clip_local, self._clip_flags, self._clip_partials = [], [], []
         for slot in range(cfg.ring_slots):
             act, dact = self._slot_act[slot], self._slot_dact[slot]
             seq_ptr = self.seg.addr("seq", 4 * (1 + slot))
+            if clip:
+                local = {k: torch.zeros(self.ps_desc[k]["arena_elems"], dtype=torch.float32, device=dev)
+                         for k in self.inbox_order}
+                lflags = {k: torch.zeros(max(lay.shards[k].n_flags, 1), dtype=torch.int32, device=dev)
+                          for k in self.inbox_order}
+                partials = torch.zeros(N.GRAD_CLIP_BLOCKS * N.GRAD_CLIP_MAX_VARS, dtype=torch.float32, device=dev)
+                self._clip_local.append(local)
+                self._clip_flags.append(lflags)
+                self._clip_partials.append(partials)
+
+                def push(k, seq_ptr=seq_ptr, local=local, lflags=lflags):
+                    return self._clip_target(k, seq_ptr, local, lflags)
+            else:
+                def push(k, seq_ptr=seq_ptr):
+                    return self._push_target(k, seq_ptr)
             stream = self.lib.dm_exec_capture_stream(self._exec, slot)
             xd, yd, rd, xs, ys = (C.c_void_p() for _ in range(5))
             N.check(self.lib.dm_exec_slot_info(self._exec, slot, C.byref(xd), C.byref(yd), C.byref(rd), C.byref(xs),
@@ -578,8 +655,7 @@ class Worker:
                 dpre_ptr=dact[L - 1].data_ptr(), result_ptr=rd.value, B=self.batch, B_pad=self.B_pad,
                 H=sizes[L - 1][0], num_classes=spec.num_classes,
                 loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT, act_bf16=cfg.dtype == "bf16",
-                push=self._push_target(wl.ps, seq_ptr), push_bh=self._push_target(hb.ps, seq_ptr),
-                push_bl=self._push_target(bl.ps, seq_ptr),
+                push=push(wl.ps), push_bh=push(hb.ps), push_bl=push(bl.ps),
                 off_w_last=wl.offset, off_b_last=bl.offset, off_b_hidden=hb.offset,
                 item_w_last_base=wl.item_base, item_b_last=bl.item_base, item_b_hidden_base=hb.item_base,
                 seq_ptr=seq_ptr, inbox_ptr=inbox_ptr, n_inbox=len(self.inbox_order), ps_global_step_ptr=gs_ptr,
@@ -587,7 +663,8 @@ class Worker:
             plans.append(head)
             # ---- backward of the hidden layers: dX (+ bias-grad push) *before* dW (fused push) of the same layer:
             #      dX pulls W_l from the PS a second time, and the PS applies a pushed dW_l within microseconds,
-            #      so pushing dW_l first would let this step's own update leak into its dX ----
+            #      so pushing dW_l first would let this step's own update leak into its dX (with clipping nothing
+            #      reaches the ps before the clip tail, and the order is kept as it is) ----
             for l in range(L - 2, -1, -1):
                 wn, bn = names[l]
                 wl = lay.by_name[wn]
@@ -600,11 +677,11 @@ class Worker:
                         w_ptr=self._weight_ptr(wl), dy_ptr=dact[l + 1].data_ptr(), out_ptr=dact[l].data_ptr(),
                         mask_ptr=act[l].data_ptr(), O=fout, I=fin, B=self.batch, B_pad=self.B_pad, dtype=self.dt,
                         ldw=wl.ld, lddy=dact[l + 1].shape[1], ldo=dact[l].shape[1],
-                        colsum=self._push_target(pb.ps, seq_ptr), colsum_offset=pb.offset, colsum_item_base=pb.item_base,
+                        colsum=push(pb.ps), colsum_offset=pb.offset, colsum_item_base=pb.item_base,
                         name=f"dx{l}"))
                 plans.append(gemm_ops.dw_plan(
                     dy_ptr=dact[l + 1].data_ptr(), x_ptr=in_ptr, O=fout, I=fin, B_pad=self.B_pad, dtype=self.dt,
-                    push=self._push_target(wl.ps, seq_ptr), push_offset=wl.offset, item_base=wl.item_base,
+                    push=push(wl.ps), push_offset=wl.offset, item_base=wl.item_base,
                     bn=lay.dw_tile_n, lddy=dact[l + 1].shape[1], ldx=ld_in, ldw=wl.ld, name=f"dw{l}"))
             if cfg.pdl:
                 # programmatic dependent launch inside the step graph: kernel k+1's prologue (and the head's
@@ -612,6 +689,9 @@ class Worker:
                 # its predecessor's outputs. The first kernel keeps a full dependency on the previous step.
                 for p in plans[1:]:
                     p.params.pdl = 1
+            if clip:
+                # after the step's last epilogue, without programmatic early launch: every push has landed locally
+                plans += self._clip_tail(seq_ptr, local, partials)
             self.kernels_per_step = len(plans)
             N.check(self.lib.dm_exec_begin_capture(self._exec, slot), "begin capture")
             try:
@@ -688,7 +768,8 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
-        N.check(self.lib.dm_fused_max_lanes(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
+        occupancy = self.lib.dm_fused_max_lanes_clip if self.opt.clip.enabled else self.lib.dm_fused_max_lanes
+        N.check(occupancy(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
         free = max_lanes.value
         if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
             # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots
@@ -755,6 +836,7 @@ class Worker:
         p.nslots = cfg.nslots
         p.ps_global_step = (self.ps_segs[self.gs_owner].addr("ctrl", 4 * CTRL_GLOBAL_STEP)
                             if cfg.push_mode == "atomic" else None)
+        self.opt.clip.fill_native(p)   # CLIP_OFF: the unclipped kernels
         if os.environ.get("DM_FUSED_DEBUG_TS") == "1":
             self._fx_dbg = torch.zeros(64, dtype=torch.int64, device=f"cuda:{self.device}")
             p.debug_ts = self._fx_dbg.data_ptr()
@@ -1004,6 +1086,7 @@ class Worker:
                         full[:, pc.c0:pc.c1] = src[:, pc.c0:pc.c1]
                 params[name] = full
         loss, grads, logits = mlp.manual_loss_and_grads(self.spec, params, x.float(), y.float())
+        grads = self.opt.clip.apply(grads)   # TF1's clip_by_* between compute_gradients and apply_gradients
         correct = mlp.accuracy_count(logits, y)
         self._seq_host += 1
         seq, ns = self._seq_host, self.cfg.nslots
