@@ -37,8 +37,8 @@ def _clip(name):
 
 
 def measure(batch: int, lanes: int, steps: int, warmup: int, clip_name: str, dev: int = 0, engine: str = "fused",
-            model: str = None) -> float:
-    """Device-timed steps/s of `steps` steps beside the resident ps."""
+            model: str = None, l2=None) -> float:
+    """Device-timed steps/s of `steps` steps beside the resident ps (`l2`: an L2Regularization, default off)."""
 
     import torch
 
@@ -51,7 +51,8 @@ def measure(batch: int, lanes: int, steps: int, warmup: int, clip_name: str, dev
 
     args = bench.parse_args(["--gpus", "1", "--lanes", str(lanes), "--batch_size", str(batch)])
     spec = mlp.get_model(model or args.model, args.hidden_units)
-    opt = OptimizerConfig(args.optimizer, args.learning_rate, clip=_clip(clip_name))
+    opt = OptimizerConfig(args.optimizer, args.learning_rate, clip=_clip(clip_name),
+                          **({"l2": l2} if l2 is not None else {}))
     cfg = dataclasses.replace(bench.engine_config(args), engine=engine)
     ds = data_utils.synthetic_mnist(data_utils.TRAIN_SIZE, seed=0)
     # (every tensor is made before the cluster starts: no new CUDA work while a persistent ps kernel is resident)

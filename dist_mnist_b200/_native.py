@@ -159,6 +159,7 @@ class FusedParams(C.Structure):
         ("exit_counter", C.c_void_p),
         ("clear_stop", C.c_uint32), ("wait_acks", C.c_uint32),
         ("clip_kind", C.c_int), ("clip_norm", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
+        ("l2_scale", C.c_float), ("l2_biases", C.c_uint32),
     ]
 
 
@@ -179,6 +180,8 @@ class GradClipParams(C.Structure):
         ("flags", C.c_void_p * GRAD_CLIP_MAX_SHARDS),
         ("flag_slot_stride", C.c_uint32 * GRAD_CLIP_MAX_SHARDS),
         ("n_flags", C.c_uint32 * GRAD_CLIP_MAX_SHARDS),
+        ("l2_w", C.c_void_p * GRAD_CLIP_MAX_VARS), ("l2_scale", C.c_float), ("l2_pad_", C.c_uint32),
+        ("l2_partials", C.c_void_p), ("result", C.c_void_p),
     ]
 
 
@@ -297,6 +300,7 @@ def _declare(l: C.CDLL) -> None:
         "dm_launch_fused": (i, [vp, vp, i, vp]),
         "dm_fused_max_lanes": (i, [i, i, C.POINTER(i)]),
         "dm_fused_max_lanes_clip": (i, [i, i, C.POINTER(i)]),
+        "dm_fused_max_lanes_l2": (i, [i, i, i, C.POINTER(i)]),
         "dm_launch_grad_clip": (i, [C.c_void_p, i, C.c_void_p]),
         "dm_fused_smem_bytes": (i, [i]),
         "dm_nvls_probe": (i, [i, sz, i, C.c_char_p, sz]),

@@ -26,8 +26,8 @@ import torch
 
 from .cluster import ClusterSpec, Rendezvous, default_device_index
 from .models import mlp
-from .parallel.config import (CLIP_KINDS, CLIP_PARAMS, LR_SCHEDULES, SCHEDULE_PARAMS, EngineConfig, GradClip,
-                              LrSchedule, OptimizerConfig)
+from .parallel.config import (CLIP_KINDS, CLIP_PARAMS, L2_VARIABLES, LR_SCHEDULES, SCHEDULE_PARAMS, EngineConfig,
+                              GradClip, L2Regularization, LrSchedule, OptimizerConfig)
 from .parallel.ps import ParameterServer
 from .parallel.worker import Worker
 from .session import train_loop
@@ -111,6 +111,14 @@ def grad_clip_from_args(args) -> GradClip:
     return GradClip(kind, **{_CLIP_FLAGS[flag]: v for flag, v in given.items()})
 
 
+def l2_regularization_from_args(args) -> L2Regularization:
+    """The L2 weight regularization of `--l2_regularization` and `--l2_variables`; the second without the first is an
+    error."""
+    if args.l2_variables is not None and args.l2_regularization is None:
+        raise ValueError("--l2_variables needs --l2_regularization (L2 regularization is off)")
+    return L2Regularization(args.l2_regularization, args.l2_variables or "weights")
+
+
 def optimizer_config_from_args(args) -> OptimizerConfig:
     """The optimizer every task derives from the command line; a hyper-parameter flag the chosen optimizer does not
     use is an error."""
@@ -125,7 +133,7 @@ def optimizer_config_from_args(args) -> OptimizerConfig:
                            schedule=lr_schedule_from_args(args),
                            moving_average_decay=args.moving_average_decay,
                            moving_average_num_updates=args.moving_average_num_updates != "none",
-                           clip=grad_clip_from_args(args))
+                           clip=grad_clip_from_args(args), l2=l2_regularization_from_args(args))
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -189,6 +197,12 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--clip_norm", type=float, default=None, help="global_norm / norm (required): finite, > 0")
     p.add_argument("--clip_value_min", type=float, default=None, help="value (required): finite, <= --clip_value_max")
     p.add_argument("--clip_value_max", type=float, default=None, help="value (required): finite")
+    # L2 weight regularization on the worker (TF1's loss + S * sum(tf.nn.l2_loss(v))), before the clip
+    p.add_argument("--l2_regularization", type=float, default=None,
+                   help="scale S of the L2 term added to the loss and S * w to the gradient: finite, >= 0 "
+                        "(unset or 0: off)")
+    p.add_argument("--l2_variables", choices=list(L2_VARIABLES), default=None,
+                   help="weights (default): every layer's weight matrix; all: the weights and the biases")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")

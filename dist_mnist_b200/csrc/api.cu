@@ -288,6 +288,12 @@ int dm_fused_max_lanes_clip(int dev, int batch, int* out) {
   DM_CUDA(dm::fused_max_lanes_clip(batch, out));
   return 0;
 }
+// the same for the L2-regularizing instantiations, with (clip != 0) or without gradient clipping
+int dm_fused_max_lanes_l2(int dev, int batch, int clip, int* out) {
+  DM_CUDA(cudaSetDevice(dev));
+  DM_CUDA(dm::fused_max_lanes_for(batch, clip != 0, true, out));
+  return 0;
+}
 int dm_fused_smem_bytes(int batch) { return static_cast<int>(dm::fused_smem_bytes(batch)); }
 
 int dm_launch_gemm(const void* tmA, const void* tmB, const void* params, int dtype, int a_mn, int b_mn, int splits,

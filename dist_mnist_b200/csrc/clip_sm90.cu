@@ -16,6 +16,12 @@
 //                             shard it pushes to is released with the step's push sequence number
 //
 // CLIP_VALUE needs no sums: the ssq kernel is not captured and the apply kernel clamps.
+//
+// L2 weight regularization (the <true> instantiations; GradClipParams::l2_scale != 0, with or without a clip) takes the
+// same route: the ssq kernel also sums w*w per block and, for the clip norms, squares g' = fl(g + fl(S * w)) instead of
+// g, where w is read from the owning shard (as the dX GEMM pulls W a second time); the apply kernel writes the clipped
+// g' (or g' itself under CLIP_OFF), and its block 0 adds S * sum(w*w) / 2 to the slot's StepResult loss, the partials
+// summed in a fixed order.
 #include "common.cuh"
 #include "grad_clip.cuh"
 
@@ -24,36 +30,73 @@ namespace dm {
 constexpr int kClipThreads = 256;
 constexpr int kClipBlocks = 132;
 
+// the block sum of v (warp shuffles, then the warps in order) into *out from thread 0
+template <typename F>
+__device__ __forceinline__ void clip_block_sum(float v, float* s_warp, F&& store) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float b = 0.f;
+#pragma unroll
+    for (int w = 0; w < kClipThreads / 32; ++w) b += s_warp[w];
+    store(b);
+  }
+  __syncthreads();
+}
+
+// g' = fl(g + fl(S * w)), as TF's L2LossGrad followed by the ADD_N of the two gradients
+__device__ __forceinline__ float l2_grad(float g, float s, float w) { return __fadd_rn(g, __fmul_rn(s, w)); }
+
+template <bool kL2>
 __global__ void __launch_bounds__(kClipThreads) grad_clip_ssq_kernel(const __grid_constant__ GradClipParams p) {
   __shared__ float s_warp[kClipThreads / 32];
   for (int v = 0; v < p.n_vars; ++v) {
     const GradClipVar& var = p.var[v];
     const uint64_t n = static_cast<uint64_t>(var.rows) * var.cols;
     float acc = 0.f;
-    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
-         i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
-      const float g = var.local[(i / var.cols) * var.ld + i % var.cols];
-      acc = fmaf(g, g, acc);
+    if constexpr (kL2) {
+      const float* w = p.l2_w[v];
+      const bool norms = p.kind == CLIP_GLOBAL_NORM || p.kind == CLIP_NORM;
+      float reg = 0.f;
+      for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
+           i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
+        const uint64_t e = (i / var.cols) * var.ld + i % var.cols;
+        float g = var.local[e];
+        if (w != nullptr) {
+          const float wv = w[e];
+          g = l2_grad(g, p.l2_scale, wv);
+          reg = fmaf(wv, wv, reg);
+        }
+        if (norms) acc = fmaf(g, g, acc);
+      }
+      clip_block_sum(reg, s_warp, [&](float b) { p.l2_partials[blockIdx.x * kGradClipMaxVars + v] = b; });
+    } else {
+      for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
+           i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
+        const float g = var.local[(i / var.cols) * var.ld + i % var.cols];
+        acc = fmaf(g, g, acc);
+      }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float b = 0.f;
-#pragma unroll
-      for (int w = 0; w < kClipThreads / 32; ++w) b += s_warp[w];
-      p.partials[blockIdx.x * kGradClipMaxVars + v] = b;
-    }
-    __syncthreads();
+    clip_block_sum(acc, s_warp, [&](float b) { p.partials[blockIdx.x * kGradClipMaxVars + v] = b; });
   }
 }
 
+template <bool kL2>
 __global__ void __launch_bounds__(kClipThreads) grad_clip_apply_kernel(const __grid_constant__ GradClipParams p) {
   __shared__ float s_fac[kGradClipMaxVars];
   const uint32_t seq = *reinterpret_cast<const volatile uint32_t*>(p.seq_ptr);
   const uint64_t slot = seq % p.nslots;
-  if (p.kind != CLIP_VALUE) {
+  if constexpr (kL2) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      float r = 0.f;
+      for (int v = 0; v < p.n_vars; ++v)
+        for (int b = 0; b < kClipBlocks; ++b) r += p.l2_partials[b * kGradClipMaxVars + v];
+      p.result->loss = __fadd_rn(p.result->loss, __fmul_rn(p.l2_scale, __fmul_rn(0.5f, r)));
+    }
+  }
+  if (kL2 ? (p.kind == CLIP_GLOBAL_NORM || p.kind == CLIP_NORM) : p.kind != CLIP_VALUE) {
     __shared__ float s_tot[kGradClipMaxVars];
     if (threadIdx.x < static_cast<unsigned>(p.n_vars)) {
       float t = 0.f;
@@ -75,14 +118,26 @@ __global__ void __launch_bounds__(kClipThreads) grad_clip_apply_kernel(const __g
   }
   for (int v = 0; v < p.n_vars; ++v) {
     const GradClipVar& var = p.var[v];
-    const float f = p.kind != CLIP_VALUE ? s_fac[v] : 1.f;
+    const float f = (kL2 ? (p.kind == CLIP_GLOBAL_NORM || p.kind == CLIP_NORM) : p.kind != CLIP_VALUE) ? s_fac[v] : 1.f;
     float* mb = var.mailbox + slot * var.mailbox_slot_stride;
     const uint64_t n = static_cast<uint64_t>(var.rows) * var.cols;
-    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
-         i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
-      const uint64_t e = (i / var.cols) * var.ld + i % var.cols;
-      mb[e] = clip_element(p.kind, var.local[e], f, p.clip_norm, p.clip_min, p.clip_max);
-      var.local[e] = 0.f;
+    if constexpr (kL2) {
+      const float* w = p.l2_w[v];
+      for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
+           i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
+        const uint64_t e = (i / var.cols) * var.ld + i % var.cols;
+        float g = var.local[e];
+        if (w != nullptr) g = l2_grad(g, p.l2_scale, w[e]);
+        mb[e] = p.kind == CLIP_OFF ? g : clip_element(p.kind, g, f, p.clip_norm, p.clip_min, p.clip_max);
+        var.local[e] = 0.f;
+      }
+    } else {
+      for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClipThreads + threadIdx.x; i < n;
+           i += static_cast<uint64_t>(gridDim.x) * kClipThreads) {
+        const uint64_t e = (i / var.cols) * var.ld + i % var.cols;
+        mb[e] = clip_element(p.kind, var.local[e], f, p.clip_norm, p.clip_min, p.clip_max);
+        var.local[e] = 0.f;
+      }
     }
   }
 }
@@ -99,19 +154,25 @@ __global__ void __launch_bounds__(kClipThreads) grad_clip_release_kernel(const _
 
 cudaError_t preload_grad_clip_kernels() {
   cudaFuncAttributes a;
-  cudaError_t e = cudaFuncGetAttributes(&a, grad_clip_ssq_kernel);   // force-load (see preload_ps_kernels)
-  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_apply_kernel);
+  cudaError_t e = cudaFuncGetAttributes(&a, grad_clip_ssq_kernel<false>);   // force-load (see preload_ps_kernels)
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_apply_kernel<false>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_ssq_kernel<true>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_apply_kernel<true>);
   return e != cudaSuccess ? e : cudaFuncGetAttributes(&a, grad_clip_release_kernel);
 }
 
 cudaError_t launch_grad_clip(const GradClipParams& p, int stage, cudaStream_t stream) {
+  const bool l2 = p.l2_scale != 0.f;
   if (p.n_vars < 1 || p.n_vars > kGradClipMaxVars || p.n_shards < 0 || p.n_shards > kGradClipMaxShards ||
-      p.nslots < 1 || p.kind < CLIP_GLOBAL_NORM || p.kind > CLIP_VALUE)
+      p.nslots < 1 || p.kind < (l2 ? CLIP_OFF : CLIP_GLOBAL_NORM) || p.kind > CLIP_VALUE ||
+      !(p.l2_scale >= 0.f && p.l2_scale < INFINITY) || (l2 && (p.l2_partials == nullptr || p.result == nullptr)))
     return cudaErrorInvalidValue;
   if (stage == 0) {
-    grad_clip_ssq_kernel<<<kClipBlocks, kClipThreads, 0, stream>>>(p);
+    if (l2) grad_clip_ssq_kernel<true><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
+    else grad_clip_ssq_kernel<false><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
   } else if (stage == 1) {
-    grad_clip_apply_kernel<<<kClipBlocks, kClipThreads, 0, stream>>>(p);
+    if (l2) grad_clip_apply_kernel<true><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
+    else grad_clip_apply_kernel<false><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
   } else if (stage == 2) {
     grad_clip_release_kernel<<<1, kClipThreads, 0, stream>>>(p);
   } else {

@@ -101,6 +101,11 @@ constexpr int kFsClipVars = 4;                                        // hid_w, 
 constexpr uint32_t kOffClipWarp = (kOffRawBl + 64 + 15) & ~15u;       // [4][4]      warp partials of this CTA
 constexpr uint32_t kOffClipPart = kOffClipWarp + 4 * kFsClipVars * 4; // [8][4]      CTA partials (DSMEM all-gather)
 static_assert(kOffClipPart + kFusedCluster * kFsClipVars * 4 <= kOffStage, "the clip partials fit before the staging tile");
+// L2 regularization (fused_step_kernel<*, *, true>): the sums of w*w of a step sit in the same gap, behind the clip
+// partials: per warp of this CTA {hid_w, small variables}, and the CTA partials that CTA 0's publisher adds up.
+constexpr uint32_t kOffL2Warp = kOffClipPart + kFusedCluster * kFsClipVars * 4;   // [4][2]  warp partials of this CTA
+constexpr uint32_t kOffL2Part = kOffL2Warp + 4 * 2 * 4;                           // [8]     CTA partials (CTA 0)
+static_assert(kOffL2Part + kFusedCluster * 4 <= kOffStage, "the L2 partials fit before the staging tile");
 
 // pre^T block [64 x 32] += W [64 x k8] . x [32 x k8]^T, both operands from shared memory (tf32)
 __device__ __forceinline__ void fs_mma_m64n32(float (&d)[4][4], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
@@ -186,7 +191,13 @@ __device__ __forceinline__ void fs_wait_acks(const FusedParams& p, uint32_t need
 // in the same order, so all agree on the scale bit for bit. The staging tile is then scaled in place before warp 4
 // stores it, and the small gradients are pushed after the norm barrier (still before barrier #3). CLIP_VALUE clamps
 // element-wise and needs neither the sums nor the barrier.
-template <int kMaxTiles, bool kClip>
+// kL2: L2 weight regularization (FusedParams::l2_scale, l2_biases), before the clip: the pushed gradient of a
+// regularized variable is fl(g + fl(S * w)), with w the copy this step pulled. W is read out of its forward tile and the
+// small variables out of their landing zones, so warp 4 issues the next step's pull only once the last row tile has
+// handed the staging tile over (named barrier 2) instead of after its barrier #1. Every CTA sums w*w over what it
+// owns (its W k-slice, W_last / b of its 16 hidden units, b_last on CTA 0) into one partial on CTA 0, whose publisher
+// adds the 8 partials in a fixed order and reports loss + S * sum / 2.
+template <int kMaxTiles, bool kClip, bool kL2>
 __global__ void __launch_bounds__(kFsThreads, 1)
 fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant__ FusedParams p) {
   constexpr bool kMulti = kMaxTiles > 1;
@@ -348,7 +359,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
         if (t == 0) nxt = ctl_next[(jl + 1) & 1];
         if (!last) {
           if (lane == 0) issue_x(cur, t + 1, kOffXk, bar_xk);   // x of the next tile (W stays for the whole step)
-        } else if (lane == 0 && !p.strict && nxt != kFusedNoStep) {
+        } else if (!kL2 && lane == 0 && !p.strict && nxt != kFusedNoStep) {
           issue_wx(nxt);                                    // W / x buffers are free: pull ahead
         }
         __syncwarp();
@@ -377,6 +388,11 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
       }
       // ---- the gradient push: the epilogue warps have staged the dW tile (swizzled, fence.proxy.async'ed) ----
       named_bar_sync(2, 160);
+      if constexpr (kL2) {
+        // the warpgroup has read W and the small variables for the L2 term (and fenced those generic reads before the
+        // hand-off): the pull-ahead may overwrite them now
+        if (lane == 0 && !p.strict && nxt != kFusedNoStep) issue_wx(nxt);
+      }
       {
         const PushTarget& tw = p.shard[sl.shard].push;
         const uint32_t slot = tw.mode == PUSH_MAILBOX ? seq % tw.nslots : 0u;
@@ -402,6 +418,13 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
       if (rank == 0 && lane == 0) {
 #pragma unroll
         for (int src = 0; src < kFusedCluster; ++src) { pend.loss += scal[src * 2]; pend.corr += scal[src * 2 + 1]; }
+        if constexpr (kL2) {
+          const float* l2p = reinterpret_cast<const float*>(smem + kOffL2Part);
+          float r = 0.f;
+#pragma unroll
+          for (int src = 0; src < kFusedCluster; ++src) r += l2p[src];
+          pend.loss = __fadd_rn(pend.loss, __fmul_rn(p.l2_scale, __fmul_rn(0.5f, r)));
+        }
       }
       if (lane == 0 && nxt != kFusedNoStep) issue_xmn(nxt, 0);   // (the dW MMAs that read the second x tile are complete)
       // Publishing costs several memory round trips (an NVLink round trip when the ps is remote): store completion,
@@ -456,6 +479,31 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
     // kClip: this thread's small gradients out of the landing zones (the same sums, in the same order, as the unclipped
     // push): sm_w value vg of unit u, value vg + 8 of it or hid_b (vg == 3), and sm_b (CTA 0, et < C). They are read
     // once for the norms and again for the push, so that no register holds them across the dW GEMM.
+    // kL2: g + S * w of one small-gradient element, w out of its landing zone; `r` adds up w * w
+    auto l2_add = [&](float g, float w, float& r) -> float {
+      r = fmaf(w, w, r);
+      return __fadd_rn(g, __fmul_rn(p.l2_scale, w));
+    };
+    // kL2: the L2 terms of this thread's small gradients (the elements the push below writes); returns the sum of w*w
+    auto l2_small = [&](float& s0, float& s1, float& sbl) -> float {
+      const int u = et & 15, vg = et >> 4;
+      const int unit = static_cast<int>(rank) * 16 + u;
+      float r = 0.f;
+      if (unit < H) {
+        if (vg < C) s0 = l2_add(s0, raw_wl[vg * H + unit], r);
+        if (vg < 3 && vg + 8 < C) s1 = l2_add(s1, raw_wl[(vg + 8) * H + unit], r);
+        if (vg == 3 && p.l2_biases) s1 = l2_add(s1, raw_b[unit], r);
+      }
+      if (rank == 0 && et < C && p.l2_biases) sbl = l2_add(sbl, raw_bl[et], r);
+      return r;
+    };
+    // kL2: the per-warp sum of v into L2 warp partial `var` of this CTA (hid_w 0, small variables 1)
+    float* l2_warp = reinterpret_cast<float*>(smem + kOffL2Warp);
+    auto l2_warp_sum = [&](float v, int var) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) l2_warp[q * 2 + var] = v;
+    };
     auto small_grads = [&](float& s0, float& s1, float& sbl) {
       const int u = et & 15, vg = et >> 4;
       s0 = 0.f;
@@ -470,6 +518,8 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 #pragma unroll
         for (int src = 0; src < kFusedCluster; ++src) sbl += dbl[src * kFsMaxC + et];
       }
+      if constexpr (kL2) return l2_small(s0, s1, sbl);
+      else return 0.f;
     };
     // kClip: the per-warp sum of v into warp partial `var` of this CTA (hid_w 0, hid_b 1, sm_w 2, sm_b 3)
     float* clip_warp = reinterpret_cast<float*>(smem + kOffClipWarp);
@@ -755,6 +805,14 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             if (vg < 4) s1 += sg[(s * 16 + u) * kFsPart + vg + 8];
           }
           const int unit = static_cast<int>(rank) * 16 + u;
+          float s = 0.f;
+          if constexpr (kL2) {
+            if (rank == 0 && et < C) {
+#pragma unroll
+              for (int src = 0; src < kFusedCluster; ++src) s += dbl[src * kFsMaxC + et];
+            }
+            l2_warp_sum(l2_small(s0, s1, s), 1);
+          }
           if (unit < H) {
             if (vg < C) fs_push_value(p.shard[p.shard_wl].push, pw_l.base + p.off_wl + static_cast<size_t>(vg) * H + unit, s0);
             if (vg < 3 && vg + 8 < C)
@@ -763,9 +821,10 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
           }
           if (rank == 0 && et < C) {
             const FsPush pb_l = fs_resolve(p.shard[p.shard_bl].push, push_seq);
-            float s = 0.f;
+            if constexpr (!kL2) {
 #pragma unroll
-            for (int src = 0; src < kFusedCluster; ++src) s += dbl[src * kFsMaxC + et];
+              for (int src = 0; src < kFusedCluster; ++src) s += dbl[src * kFsMaxC + et];
+            }
             fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, s);
           }
         }
@@ -851,6 +910,36 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
                 }
             }
           }
+          if constexpr (kL2) {
+            if (last) {
+              // g + S * w over the staging tile, rolled like the clip passes below. The forward's W tile has the
+              // staging tile's layout ([128 hidden rows][32 features] per chunk, SWIZZLE_128B), so element o of one is
+              // element o of the other. Only the elements the TMA store pushes count toward the sum of w*w.
+              const int n4 = nkc * static_cast<int>(kFsWChunk / 16);
+              named_bar_sync(1, 128);   // every thread's part of the tile is in place (the pass crosses threads)
+              const float S = p.l2_scale;
+              float r = 0.f;
+              for (int i4 = et; i4 < n4; i4 += 128) {
+                const int i = i4 / static_cast<int>(kFsWChunk / 16), o = (i4 % static_cast<int>(kFsWChunk / 16)) * 16;
+                const int h = o >> 7, fl = (((o >> 4) & 7) ^ (h & 7)) << 2;   // inverse of sw128_offset
+                const float4 w = *reinterpret_cast<const float4*>(smem + kOffW + i * kFsWChunk + o);
+                float4* st = reinterpret_cast<float4*>(smem + kOffStage + i * kFsWChunk + o);
+                float4 v = *st;
+                v.x = __fadd_rn(v.x, __fmul_rn(S, w.x));
+                v.y = __fadd_rn(v.y, __fmul_rn(S, w.y));
+                v.z = __fadd_rn(v.z, __fmul_rn(S, w.z));
+                v.w = __fadd_rn(v.w, __fmul_rn(S, w.w));
+                *st = v;
+                if (h < H && (sl.kc_begin + i) * 32 + fl < p.I) {   // I % 4 == 0: a float4 is in or out as a whole
+                  r = fmaf(w.x, w.x, r);
+                  r = fmaf(w.y, w.y, r);
+                  r = fmaf(w.z, w.z, r);
+                  r = fmaf(w.w, w.w, r);
+                }
+              }
+              l2_warp_sum(r, 0);
+            }
+          }
           if constexpr (kClip) {
             if (last) {
               // Only the elements the TMA store pushes (hidden rows < H, features < I) count toward the norms. The loop
@@ -895,7 +984,8 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             const FsPush pb_h = fs_resolve(p.shard[p.shard_bh].push, push_seq);
             const int u = et & 15, vg = et >> 4;
             float cg0, cg1, cgl;
-            small_grads(cg0, cg1, cgl);
+            const float l2_r = small_grads(cg0, cg1, cgl);
+            if constexpr (kL2) l2_warp_sum(l2_r, 1);
             const int unit = static_cast<int>(rank) * 16 + u;
             if (unit < H) {
               if (vg < C)
@@ -909,6 +999,17 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             if (rank == 0 && et < C) {
               const FsPush pb_l = fs_resolve(p.shard[p.shard_bl].push, push_seq);
               fs_push_value(p.shard[p.shard_bl].push, pb_l.base + p.off_bl + et, clip_value(cgl, cfac.w));
+            }
+          }
+        }
+        if constexpr (kL2) {
+          if (last) {
+            if (nkc == 0) l2_warp_sum(0.f, 0);   // no W k-slice
+            named_bar_sync(1, 128);              // every warp's L2 partials are in place
+            if (et == 0) {
+              const float r = ((l2_warp[0] + l2_warp[2]) + (l2_warp[4] + l2_warp[6])) +
+                              ((l2_warp[1] + l2_warp[3]) + (l2_warp[5] + l2_warp[7]));
+              st_shared_cluster_f32(mapa_shared_cluster(sbase + kOffL2Part + rank * 4u, 0), r);   // before barrier #3
             }
           }
         }
@@ -949,20 +1050,27 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-template <int kMaxTiles, bool kClip>
+template <int kMaxTiles, bool kClip, bool kL2>
 static cudaError_t prepare_fused_instance() {
-  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip, kL2>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(fs_smem_bytes<kMaxTiles>()));
   if (e != cudaSuccess) return e;
   cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip>);   // force-load (see preload_ps_kernels)
+  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip, kL2>);   // force-load (see preload_ps_kernels)
+}
+
+template <bool kClip, bool kL2>
+static cudaError_t prepare_fused_pair() {
+  cudaError_t e = prepare_fused_instance<1, kClip, kL2>();
+  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, kClip, kL2>();
 }
 
 cudaError_t prepare_fused_kernel() {
-  cudaError_t e = prepare_fused_instance<1, false>();
-  if (e == cudaSuccess) e = prepare_fused_instance<kFsMaxTiles, false>();
-  if (e == cudaSuccess) e = prepare_fused_instance<1, true>();
-  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, true>();
+  cudaError_t e = prepare_fused_pair<false, false>();
+  if (e == cudaSuccess) e = prepare_fused_pair<true, false>();
+  if (e == cudaSuccess) e = prepare_fused_pair<false, true>();
+  return e != cudaSuccess ? e : prepare_fused_pair<true, true>();
 }
 
 static bool fused_multi_tile(int B) { return B > 32; }
@@ -985,37 +1093,41 @@ static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t str
   return cfg;
 }
 
+using FusedKernel = void (*)(const FusedMaps, const FusedParams);
+
+// The instantiation batch B runs with or without the clip and the L2 term.
+static FusedKernel fused_kernel_for(int B, bool clip, bool l2) {
+  const bool multi = fused_multi_tile(B);
+  if (l2) {
+    if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, true> : fused_step_kernel<1, true, true>;
+    return multi ? fused_step_kernel<kFsMaxTiles, false, true> : fused_step_kernel<1, false, true>;
+  }
+  if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, false> : fused_step_kernel<1, true, false>;
+  return multi ? fused_step_kernel<kFsMaxTiles, false, false> : fused_step_kernel<1, false, false>;
+}
+
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
   if (lanes < 1 || p.B < 1 || p.B > 32 * kFsMaxTiles || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 ||
       (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1 || p.clip_kind < CLIP_OFF ||
-      p.clip_kind > CLIP_VALUE)
+      p.clip_kind > CLIP_VALUE || !(p.l2_scale >= 0.f && p.l2_scale < INFINITY) ||
+      (p.l2_scale != 0.f && p.shard[0].push.mode == PUSH_ATOMIC))
     return cudaErrorInvalidValue;
   for (int r = 0; r < kFusedCluster; ++r)
     if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
-  const bool clip = p.clip_kind != CLIP_OFF;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
-  if (clip) {
-    if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles, true>, maps, p);
-    return cudaLaunchKernelEx(&cfg, fused_step_kernel<1, true>, maps, p);
-  }
-  if (fused_multi_tile(p.B)) return cudaLaunchKernelEx(&cfg, fused_step_kernel<kFsMaxTiles, false>, maps, p);
-  return cudaLaunchKernelEx(&cfg, fused_step_kernel<1, false>, maps, p);
+  return cudaLaunchKernelEx(&cfg, fused_kernel_for(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f), maps, p);
 }
 
 // How many clusters of the fused kernel that runs batch B can be co-resident on the device (upper bound for `lanes`).
-cudaError_t fused_max_lanes(int B, int* out) {
-  cudaLaunchAttribute attr[1];
-  const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles, false>, &cfg);
-  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1, false>, &cfg);
-}
+cudaError_t fused_max_lanes(int B, int* out) { return fused_max_lanes_for(B, false, false, out); }
 
-cudaError_t fused_max_lanes_clip(int B, int* out) {
+cudaError_t fused_max_lanes_clip(int B, int* out) { return fused_max_lanes_for(B, true, false, out); }
+
+cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int* out) {
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  if (fused_multi_tile(B)) return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<kFsMaxTiles, true>, &cfg);
-  return cudaOccupancyMaxActiveClusters(out, fused_step_kernel<1, true>, &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_kernel_for(B, clip, l2), &cfg);
 }
 
 }  // namespace dm

@@ -299,6 +299,10 @@ struct FusedParams {
   int clip_kind;           // GradClipKind
   float clip_norm;         // CLIP_GLOBAL_NORM, CLIP_NORM: > 0
   float clip_min, clip_max;  // CLIP_VALUE
+  // L2 weight regularization (TF1 loss + l2_scale * sum l2_loss(v); appended): g' = fl(g + fl(l2_scale * w)) for the
+  // weights (and, with l2_biases, the biases) before the clip. 0 runs the unregularized instantiations.
+  float l2_scale;          // finite, >= 0
+  uint32_t l2_biases;      // 1: the biases are regularized too
 };
 enum GradClipKind : int {
   CLIP_OFF = 0,
@@ -330,6 +334,13 @@ struct GradClipParams {
   uint32_t* flags[kGradClipMaxShards];          // slot-0 flags of this worker on each shard
   uint32_t flag_slot_stride[kGradClipMaxShards];
   uint32_t n_flags[kGradClipMaxShards];
+  // L2 weight regularization (appended; the tail runs with l2_scale != 0 even when kind is CLIP_OFF): g' = fl(local +
+  // fl(l2_scale * w)) before the clip for every variable with an l2_w, and loss += l2_scale * sum(w*w) / 2
+  const float* l2_w[kGradClipMaxVars];          // the variable's fp32 values on its shard (nullptr: not regularized)
+  float l2_scale;
+  uint32_t l2_pad_;
+  float* l2_partials;                           // [kGradClipBlocks][kGradClipMaxVars] worker-local scratch: sums of w*w
+  StepResult* result;                           // this ring slot's step result (the head has written the data loss)
 };
 
 }  // namespace dm

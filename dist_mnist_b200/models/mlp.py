@@ -255,3 +255,28 @@ def clip_gradients(grads: Dict[str, torch.Tensor], clip) -> Dict[str, torch.Tens
             out[k] = (g * c) / torch.maximum(norm, c)
         return out
     raise ValueError(f"unknown gradient clip {clip.kind!r}")
+
+
+def l2_regularize(params: Dict[str, torch.Tensor], grads: Dict[str, torch.Tensor],
+                  reg) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """TF1's L2 weight regularization in fp32 (the reference of every engine's L2 term), keyed by variable name.
+    `reg` is a `parallel.config.L2Regularization` with scale S and variable set V: the weight matrices (2-D
+    variables) for "weights", every variable for "all".
+
+    Returns (reg_loss, grads'): reg_loss = S * sum over V of l2_loss(v), l2_loss(v) = sum(v*v) / 2 as in
+    `tf.nn.l2_loss`, the term added to the data loss; grads' = g + fl(S * w) for a variable in V (TF's `L2LossGrad`
+    followed by the ADD_N of the two gradients: the product and the sum each rounded, no FMA), g unchanged otherwise.
+    `w` is the variable as the step read it (the fp32 master copy under bf16), `g` the gradient of the mean data loss
+    over the whole batch."""
+    f32 = torch.float32
+    s = torch.tensor(reg.scale, dtype=f32)
+    total = torch.zeros((), dtype=f32)
+    out = {}
+    for name, g in grads.items():
+        g = g.detach().to(f32)
+        w = params[name].detach().to(f32)
+        if reg.variables == "all" or w.dim() == 2:
+            total = total + (w * w).sum() / 2
+            g = g + s * w
+        out[name] = g
+    return s * total, out

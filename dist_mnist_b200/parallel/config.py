@@ -242,6 +242,63 @@ class GradClip:
         return cls(**d) if d else cls()
 
 
+L2_VARIABLES = ("weights", "all")
+
+
+@dataclass(frozen=True)
+class L2Regularization:
+    """TF1's L2 weight regularization on the worker: `loss += scale * sum(tf.nn.l2_loss(v) for v in V)` before
+    `opt.compute_gradients(loss)` (equivalently `tf.contrib.layers.l2_regularizer(scale)`, or cifar10's
+    `wd * l2_loss(w)`). V is every layer's weight matrix ("weights") or the weights and the biases ("all", as in the
+    MNIST `convolutional.py` example). `scale` None or 0.0 = off.
+
+    The gradient pushed for a variable in V is fl(g + fl(scale * w)), with w the variable as the step read it; gradient
+    clipping applies to that sum. The ps never sees it: it combines with every optimizer, schedule, moving average,
+    apply mode and sharding. `mlp.l2_regularize` is the fp32 reference."""
+    scale: Optional[float] = None
+    variables: str = "weights"
+
+    def __post_init__(self):
+        if self.variables not in L2_VARIABLES:
+            raise ValueError(f"unknown L2 variable set {self.variables!r} ({' | '.join(L2_VARIABLES)})")
+        s = self.scale
+        if s is None:
+            return
+        if isinstance(s, bool) or not isinstance(s, (int, float)) or not math.isfinite(s) or s < 0:
+            raise ValueError(f"L2 regularization scale must be a finite number >= 0, got {s!r}")
+        object.__setattr__(self, "scale", float(s))
+
+    @property
+    def enabled(self) -> bool:
+        return bool(self.scale)
+
+    def apply(self, params, grads):
+        """(reg_loss, grads') of the reference (mlp.l2_regularize) for {variable name: tensor} dicts; (0.0, grads)
+        unchanged when off."""
+        from ..models import mlp
+
+        if not self.enabled:
+            return 0.0, grads
+        return mlp.l2_regularize(params, grads, self)
+
+    def loss(self, params) -> float:
+        """The regularization term scale * sum over V of l2_loss(v) (fp32 reference) of {variable name: tensor}, 0.0
+        when off."""
+        return float(self.apply(params, {k: v * 0 for k, v in params.items()})[0])
+
+    def fill_native(self, P) -> None:
+        """Write this regularization into a FusedParams (l2_scale 0: the unregularized kernels)."""
+        P.l2_scale = self.scale or 0.0
+        P.l2_biases = int(self.enabled and self.variables == "all")
+
+    def as_dict(self) -> dict:
+        return asdict(self)
+
+    @classmethod
+    def from_dict(cls, d: Optional[dict]) -> "L2Regularization":
+        return cls(**d) if d else cls()
+
+
 @dataclass(frozen=True)
 class OptimizerConfig:
     """Reference: `tf.train.AdamOptimizer(FLAGS.learning_rate)` with TF defaults (DS:102); SGD is the
@@ -271,6 +328,9 @@ class OptimizerConfig:
     # gradient clipping on the worker before the push (TF1 clip_by_global_norm / clip_by_norm / clip_by_value); the
     # ps does not use it, and workers of one session may clip differently
     clip: GradClip = GradClip()
+    # L2 weight regularization on the worker (TF1 scale * l2_loss(w) added to the loss); like the clip, the ps does not
+    # use it, and it is part of the model's loss, not of the optimizer state a checkpoint restores
+    l2: L2Regularization = L2Regularization()
 
     def __post_init__(self):
         if self.math not in ("fast", "ieee"):
@@ -290,6 +350,8 @@ class OptimizerConfig:
             raise ValueError(f"schedule must be an LrSchedule, got {type(self.schedule).__name__}")
         if not isinstance(self.clip, GradClip):
             raise ValueError(f"clip must be a GradClip, got {type(self.clip).__name__}")
+        if not isinstance(self.l2, L2Regularization):
+            raise ValueError(f"l2 must be an L2Regularization, got {type(self.l2).__name__}")
         d = self.moving_average_decay
         if d is not None:
             if isinstance(d, bool) or not isinstance(d, (int, float)) or not 0.0 < d < 1.0:
@@ -412,6 +474,10 @@ class EngineConfig:
             if opt.clip.enabled:
                 raise ValueError("push_mode='atomic' applies every gradient tile as it is produced, before a clip "
                                  "could know its scale; gradient clipping needs push_mode='mailbox'")
+            if opt.l2.enabled:
+                raise ValueError("push_mode='atomic' applies every gradient tile as it is produced (the graph engine's "
+                                 "dW epilogue red.add is the apply), with no place to add the L2 term; L2 "
+                                 "regularization needs push_mode='mailbox'")
             if self.dtype != "fp32":
                 raise ValueError("push_mode='atomic' updates only the fp32 master copy; use dtype fp32")
             if self.backend != "cuda":

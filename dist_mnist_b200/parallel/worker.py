@@ -184,9 +184,10 @@ class Worker:
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: {desc}")
             # the ps applies the rule, the chief initialises its slots: with Momentum / Adagrad / RMSProp on either
             # side both must run the same optimizer (an Adam / SGD pairing is not checked, as before)
-            # (gradient clipping runs on the worker alone: workers may clip differently from the ps flags and each other)
-            ps_opt = {n: v for n, v in (desc.get("optimizer") or {}).items() if n != "clip"}
-            my_opt = {n: v for n, v in self.opt.as_dict().items() if n != "clip"}
+            # (gradient clipping and L2 regularization run on the worker alone: workers may clip or regularize
+            # differently from the ps flags and each other)
+            ps_opt = {n: v for n, v in (desc.get("optimizer") or {}).items() if n not in ("clip", "l2")}
+            my_opt = {n: v for n, v in self.opt.as_dict().items() if n not in ("clip", "l2")}
             if ((ps_opt.get("kind") in TF1_SLOT_KINDS or self.opt.kind in TF1_SLOT_KINDS) and ps_opt != my_opt):
                 raise RuntimeError(f"ps {k} was started with a different engine configuration: optimizer "
                                    f"{ps_opt}, this worker has {my_opt}")
@@ -519,10 +520,13 @@ class Worker:
         t.flags, t.flag_slot_stride = flags[k].data_ptr(), 0
         return t
 
-    def _clip_tail(self, seq_ptr: int, local: Dict[int, torch.Tensor], partials: torch.Tensor) -> List["_GradClipPlan"]:
-        """The clip tail of one ring slot's step graph (csrc/clip_sm90.cu): sums of squares (not for "value"), the
-        clipped copy into the mailbox slot of push *seq_ptr, the release of that slot's flags on every shard."""
-        clip, ns, w = self.opt.clip, self.cfg.nslots, self.task_index
+    def _clip_tail(self, seq_ptr: int, local: Dict[int, torch.Tensor], partials: torch.Tensor,
+                   l2_partials: Optional[torch.Tensor], result_ptr: int) -> List["_GradClipPlan"]:
+        """The clip / L2 tail of one ring slot's step graph (csrc/clip_sm90.cu): sums of squares (not for "value"
+        alone), the clipped (and L2-regularized) copy into the mailbox slot of push *seq_ptr, the release of that slot's
+        flags on every shard. With L2 the first kernel also sums w*w, and the second adds the L2 term to the step's
+        loss at `result_ptr`."""
+        clip, l2, ns, w = self.opt.clip, self.opt.l2, self.cfg.nslots, self.task_index
         P = N.GradClipParams()
         P.kind, P.clip_norm = clip.native_kind, clip.clip_norm or 0.0
         P.clip_min, P.clip_max = clip.value_min or 0.0, clip.value_max or 0.0
@@ -539,6 +543,11 @@ class Worker:
             v.mailbox = self.ps_segs[vl.ps].addr("mailbox", (w * ns * arena + vl.offset) * 4)
             v.mailbox_slot_stride = arena
             v.rows, v.cols, v.ld = vl.rows, vl.cols, vl.ld if len(vl.spec.shape) == 2 else vl.cols
+            if l2.enabled and (l2.variables == "all" or len(vl.spec.shape) == 2):
+                # w as the owning shard holds it at the end of the step (the fp32 master copy under bf16)
+                P.l2_w[i] = self.ps_segs[vl.ps].addr("params", vl.offset * 4)
+        if l2.enabled:
+            P.l2_scale, P.l2_partials, P.result = l2.scale, l2_partials.data_ptr(), result_ptr
         P.n_shards = len(self.inbox_order)
         scope = 1
         for j, k in enumerate(self.inbox_order):
@@ -549,7 +558,7 @@ class Worker:
             P.n_flags[j] = self.layout.shards[k].n_flags
             scope &= self._push_target(k, seq_ptr).gpu_scope
         P.gpu_scope = scope
-        stages = (1, 2) if clip.kind == "value" else (0, 1, 2)
+        stages = (1, 2) if clip.kind == "value" and not l2.enabled else (0, 1, 2)
         return [_GradClipPlan(P, st) for st in stages]
 
     def _weight_ptr(self, vl: VarLayout) -> int:
@@ -603,9 +612,10 @@ class Worker:
             num_classes=spec.num_classes, loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT,
             act_bf16=cfg.dtype == "bf16", compute_grads=False, ldh=self.act[L - 1].shape[1]))
         torch.cuda.synchronize(self.device)
-        clip = self.opt.clip.enabled
-        # gradient clipping: per ring slot, a local gradient buffer per shard (the epilogues' push target), worker-local
-        # flags they release, and the clip tail's per-block partial sums (steps of different slots run concurrently)
+        clip = self.opt.clip.enabled or self.opt.l2.enabled
+        # gradient clipping / L2 regularization: per ring slot, a local gradient buffer per shard (the epilogues' push
+        # target), worker-local flags they release, and the tail's per-block partial sums (steps of different slots run
+        # concurrently)
         self._clip_local, self._clip_flags, self._clip_partials = [], [], []
         for slot in range(cfg.ring_slots):
             act, dact = self._slot_act[slot], self._slot_dact[slot]
@@ -615,7 +625,7 @@ class Worker:
                          for k in self.inbox_order}
                 lflags = {k: torch.zeros(max(lay.shards[k].n_flags, 1), dtype=torch.int32, device=dev)
                           for k in self.inbox_order}
-                partials = torch.zeros(N.GRAD_CLIP_BLOCKS * N.GRAD_CLIP_MAX_VARS, dtype=torch.float32, device=dev)
+                partials = torch.zeros(2, N.GRAD_CLIP_BLOCKS * N.GRAD_CLIP_MAX_VARS, dtype=torch.float32, device=dev)
                 self._clip_local.append(local)
                 self._clip_flags.append(lflags)
                 self._clip_partials.append(partials)
@@ -691,7 +701,7 @@ class Worker:
                     p.params.pdl = 1
             if clip:
                 # after the step's last epilogue, without programmatic early launch: every push has landed locally
-                plans += self._clip_tail(seq_ptr, local, partials)
+                plans += self._clip_tail(seq_ptr, local, partials[0], partials[1], rd.value)
             self.kernels_per_step = len(plans)
             N.check(self.lib.dm_exec_begin_capture(self._exec, slot), "begin capture")
             try:
@@ -768,8 +778,12 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
-        occupancy = self.lib.dm_fused_max_lanes_clip if self.opt.clip.enabled else self.lib.dm_fused_max_lanes
-        N.check(occupancy(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
+        if self.opt.l2.enabled:
+            N.check(self.lib.dm_fused_max_lanes_l2(self.device, self.batch, int(self.opt.clip.enabled),
+                                                   C.byref(max_lanes)), "fused occupancy")
+        else:
+            occupancy = self.lib.dm_fused_max_lanes_clip if self.opt.clip.enabled else self.lib.dm_fused_max_lanes
+            N.check(occupancy(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
         free = max_lanes.value
         if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
             # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots
@@ -837,6 +851,7 @@ class Worker:
         p.ps_global_step = (self.ps_segs[self.gs_owner].addr("ctrl", 4 * CTRL_GLOBAL_STEP)
                             if cfg.push_mode == "atomic" else None)
         self.opt.clip.fill_native(p)   # CLIP_OFF: the unclipped kernels
+        self.opt.l2.fill_native(p)     # l2_scale 0: the unregularized kernels
         if os.environ.get("DM_FUSED_DEBUG_TS") == "1":
             self._fx_dbg = torch.zeros(64, dtype=torch.int64, device=f"cuda:{self.device}")
             p.debug_ts = self._fx_dbg.data_ptr()
@@ -1086,6 +1101,9 @@ class Worker:
                         full[:, pc.c0:pc.c1] = src[:, pc.c0:pc.c1]
                 params[name] = full
         loss, grads, logits = mlp.manual_loss_and_grads(self.spec, params, x.float(), y.float())
+        if self.opt.l2.enabled:   # TF1's scale * l2_loss(w) in the loss: the reported loss and the clipped gradient
+            reg_loss, grads = self.opt.l2.apply(params, grads)
+            loss = loss + reg_loss
         grads = self.opt.clip.apply(grads)   # TF1's clip_by_* between compute_gradients and apply_gradients
         correct = mlp.accuracy_count(logits, y)
         self._seq_host += 1
