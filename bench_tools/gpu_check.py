@@ -402,8 +402,8 @@ def _ref_apply(opt, p, m, v, g, lr, t):
 
 
 def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step: int = 0) -> bool:
-    """The serve kernel's Momentum / Adagrad / RMSProp instantiations (`opt`: an OptimizerConfig; `opt.math` picks the
-    fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
+    """The serve kernel's Momentum / Adagrad / RMSProp / Adadelta / FTRL / ProximalAdagrad / ProximalGradientDescent
+    instantiations (`opt`: an OptimizerConfig; `opt.math` picks the fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
     against the TF1 formulas in fp64 (parameters and both slot buffers within 1e-5 relative error; the bf16 shadow,
     global_step and the acks exact). `resident`: one pushed push per worker and pass (lookahead 1) and one vectorisable
     item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass.
@@ -463,7 +463,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     P.n_items, P.n_workers, P.nslots, P.opt, P.apply_mode = n_items, n_workers, nslots, opt.native_kind, apply_mode
     P.n_flags = n_items
     P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
-    P.momentum, P.decay, P.nesterov = opt.momentum or 0.0, opt.decay or 0.0, int(opt.use_nesterov)
+    opt.fill_native_rule(P)
     P.ieee_math = 1 if opt.math == "ieee" else 0
     opt.schedule.fill_native(P)
     ema = params.clone() if opt.moving_averages else None
@@ -513,6 +513,10 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
             and acks == [n_push] * n_workers and int(exitc.item()) == n_ctas)
     name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''} momentum={opt.momentum} math={opt.math} "
             f"mode={apply_mode} resident={resident}")
+    if opt.kind in ("adadelta", "ftrl", "proximal_adagrad", "proximal_sgd"):
+        name += (f" rho={opt.rho} l1={opt.l1_regularization_strength} l2={opt.l2_regularization_strength} "
+                 f"shrinkage={opt.l2_shrinkage_regularization_strength} lr_power={opt.learning_rate_power} "
+                 f"accum0={opt.initial_accumulator_value}")
     extra = ""
     if not opt.schedule.constant or ema is not None:
         steps_now = sorted({int(x) & 0xFFFFFFFF for x in state.view(torch.int32).view(n_items, 4)[:, 3].tolist()})

@@ -21,10 +21,18 @@ from dist_mnist_b200.session import InProcessCluster
 from dist_mnist_b200.utils import data
 
 
+def _prox_shrink(prox, a, l1, l2):
+    """ApplyProximalAdagrad / ApplyProximalGradientDescent's proximal step at step size `a` (a tensor)."""
+    if l1 > 0:
+        return prox.sign() * (prox.abs() - a * l1).clamp_min(0) / (1 + l2 * a)
+    return prox / (1 + l2 * a)
+
+
 def tf1_apply(opt, p, m, v, g):
-    """One TF1 `training_ops` step of Momentum / Adagrad / RMSProp (not centered) on tensors, in their own dtype:
-    `m` is the slot kept in adam_m (momentum accumulator, RMSProp mom), `v` the one in adam_v (Adagrad accumulator,
-    RMSProp ms). Returns the new (p, m, v)."""
+    """One TF1 `training_ops` step of Momentum / Adagrad / RMSProp (not centered) / Adadelta / FTRL (V2 with
+    l2_shrinkage) / ProximalAdagrad / ProximalGradientDescent on tensors, in their own dtype: `m` is the slot kept in
+    adam_m (momentum accumulator, RMSProp mom, Adadelta accum_update, FTRL linear), `v` the one in adam_v (Adagrad,
+    FTRL and ProximalAdagrad accumulator, RMSProp ms, Adadelta accum). Returns the new (p, m, v)."""
     if opt.kind == "momentum":
         m = opt.momentum * m + g
         p = p - (g * opt.lr + m * opt.momentum * opt.lr) if opt.use_nesterov else p - opt.lr * m
@@ -35,6 +43,28 @@ def tf1_apply(opt, p, m, v, g):
         v = v + (g * g - v) * (1 - opt.decay)
         m = opt.momentum * m + opt.lr * g / (v + opt.eps).sqrt()
         p = p - m
+    elif opt.kind == "adadelta":
+        rho = opt.rho
+        v = v * rho + g * g * (1 - rho)
+        upd = (m + opt.eps).sqrt() * (v + opt.eps).rsqrt() * g
+        p = p - upd * opt.lr
+        m = m * rho + upd * upd * (1 - rho)
+    elif opt.kind == "proximal_adagrad":
+        v = v + g * g
+        a = opt.lr * v.rsqrt()
+        p = _prox_shrink(p - g * a, a, opt.l1_regularization_strength, opt.l2_regularization_strength)
+    elif opt.kind == "proximal_sgd":
+        a = torch.full_like(p, opt.lr)
+        p = _prox_shrink(p - g * a, a, opt.l1_regularization_strength, opt.l2_regularization_strength)
+    elif opt.kind == "ftrl":
+        l1, l2, lrp = opt.l1_regularization_strength, opt.l2_regularization_strength, opt.learning_rate_power
+        gs = g + 2 * opt.l2_shrinkage_regularization_strength * p
+        n = v + g * g
+        pn, pa = (n.sqrt(), v.sqrt()) if lrp == -0.5 else (n.pow(-lrp), v.pow(-lrp))
+        m = m + (gs - (pn - pa) / opt.lr * p)
+        y = pn / opt.lr + 2 * l2
+        p = torch.where(m.abs() > l1, (m.sign() * l1 - m) / y, torch.zeros_like(p))
+        v = n
     else:
         raise ValueError(opt.kind)
     return p, m, v

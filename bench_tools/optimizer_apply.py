@@ -1,5 +1,6 @@
-"""What each ps optimizer costs in the flagship configuration: Adam, SGD, Momentum, Nesterov momentum, Adagrad and
-RMSProp, one after the other, in bench.py's single-GPU setup (ps and worker sharing the GPU, fused engine, default
+"""What each ps optimizer costs in the flagship configuration: Adam, SGD, Momentum, Nesterov momentum, Adagrad,
+RMSProp, Adadelta, FTRL (at lr_power -0.5, the square-root path, and as `ftrl_pow` at -0.25, the general power),
+ProximalAdagrad and ProximalGradientDescent, one after the other, in bench.py's single-GPU setup (ps and worker sharing the GPU, fused engine, default
 lanes, device-resident data).
 
 Per optimizer, two in-process clusters: one for the device-timed steps/s of `Worker.run_resident` (the serve kernel's
@@ -12,8 +13,10 @@ and at a constant rate, alternated in the same call: the cost of the rate table 
 `--moving_average_decay D` likewise measures every optimizer with moving averages of that decay (the averaging serve
 kernels) and without, alternated in the same call: the cost of the shadow load, update and store.
 
+`--rounds N` repeats the whole sequence N times, so that every rule is measured N times, alternated with the others.
+
     python bench_tools/optimizer_apply.py [--steps 20000] [--warmup 50] [--only rmsprop,adam] [--lr_schedule KIND]
-                                          [--moving_average_decay D]
+                                          [--moving_average_decay D] [--rounds N]
 """
 from __future__ import annotations
 
@@ -26,7 +29,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-RULES = ["adam", "sgd", "momentum", "nesterov", "adagrad", "rmsprop"]
+RULES = ["adam", "sgd", "momentum", "nesterov", "adagrad", "rmsprop", "adadelta", "ftrl", "ftrl_pow", "proximal_adagrad",
+         "proximal_sgd"]
 
 
 def schedule(kind: str, lr: float):
@@ -47,6 +51,9 @@ def optimizer(rule: str, lr: float, sched: str = "constant", ema=None):
 
     if rule == "nesterov":
         return OptimizerConfig("momentum", lr, use_nesterov=True, schedule=schedule(sched, lr),
+                               moving_average_decay=ema)
+    if rule == "ftrl_pow":
+        return OptimizerConfig("ftrl", lr, learning_rate_power=-0.25, schedule=schedule(sched, lr),
                                moving_average_decay=ema)
     return OptimizerConfig(rule, lr, schedule=schedule(sched, lr), moving_average_decay=ema)
 
@@ -112,6 +119,7 @@ def main(argv=None) -> int:
                     help="also run every optimizer under this learning-rate schedule, alternated with constant")
     ap.add_argument("--moving_average_decay", type=float, default=None,
                     help="also run every optimizer with moving averages of this decay, alternated with none")
+    ap.add_argument("--rounds", type=int, default=1, help="repeat the whole sequence of optimizers this many times")
     a = ap.parse_args(argv)
     import torch
 
@@ -131,7 +139,7 @@ def main(argv=None) -> int:
     emas = [a.moving_average_decay, None] if a.moving_average_decay is not None else [None]
     card = card_info(0)
     rows = []
-    for r in rules:
+    for r in [r for _ in range(a.rounds) for r in rules]:
         for sc, ema in [(sc, e) for sc in scheds for e in emas]:
             timed = run_one(r, a.steps, a.warmup, stats=False, sched=sc, ema=ema)
             counted = run_one(r, a.steps, a.warmup, stats=True, sched=sc, ema=ema)
@@ -141,7 +149,7 @@ def main(argv=None) -> int:
                    "steps_per_s_with_counters": counted["steps_per_s"], "card": card}
             rows.append(row)
             print(json.dumps(row), flush=True)
-    print(f"card {card}; {a.steps} timed steps per optimizer, schedule and averaging")
+    print(f"card {card}; {a.steps} timed steps per optimizer, schedule and averaging; {a.rounds} round(s)")
     print(f"{'optimizer':>10} {'lr_schedule':>18} {'ema decay':>10} {'steps/s':>9} {'apply cycles/push':>18} "
           f"{'pushes/pass':>12} {'ps busy':>8}")
     for row in rows:

@@ -51,8 +51,12 @@ def engine_config_from_args(args, backend: str) -> EngineConfig:
 
 
 # optimizer flag -> the optimizers that use it
+_PROXIMAL_OPTS = ("ftrl", "proximal_adagrad", "proximal_sgd")
 _OPT_FLAGS = {"momentum": ("momentum", "rmsprop"), "use_nesterov": ("momentum",), "rmsprop_decay": ("rmsprop",),
-              "initial_accumulator_value": ("adagrad",), "epsilon": ("adam", "rmsprop")}
+              "initial_accumulator_value": ("adagrad", "ftrl", "proximal_adagrad"),
+              "epsilon": ("adam", "rmsprop", "adadelta"), "rho": ("adadelta",),
+              "l1_regularization_strength": _PROXIMAL_OPTS, "l2_regularization_strength": _PROXIMAL_OPTS,
+              "l2_shrinkage_regularization_strength": ("ftrl",), "learning_rate_power": ("ftrl",)}
 
 
 # learning-rate schedule flag -> LrSchedule parameter
@@ -129,7 +133,11 @@ def optimizer_config_from_args(args) -> OptimizerConfig:
         raise ValueError("--moving_average_num_updates needs --moving_average_decay (moving averages are off)")
     return OptimizerConfig(args.optimizer, args.learning_rate, eps=args.epsilon, math=args.adam_math,
                            momentum=args.momentum, use_nesterov=args.use_nesterov, decay=args.rmsprop_decay,
-                           initial_accumulator_value=args.initial_accumulator_value,
+                           initial_accumulator_value=args.initial_accumulator_value, rho=args.rho,
+                           l1_regularization_strength=args.l1_regularization_strength,
+                           l2_regularization_strength=args.l2_regularization_strength,
+                           l2_shrinkage_regularization_strength=args.l2_shrinkage_regularization_strength,
+                           learning_rate_power=args.learning_rate_power,
                            schedule=lr_schedule_from_args(args),
                            moving_average_decay=args.moving_average_decay,
                            moving_average_num_updates=args.moving_average_num_updates != "none",
@@ -152,19 +160,34 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--job_name", type=str, default=None, help="worker or ps")
     p.add_argument("--task_index", type=int, default=None)
     # ---- new-engine flags ----
-    p.add_argument("--optimizer", choices=["adam", "sgd", "momentum", "adagrad", "rmsprop"], default="adam",
-                   help="reference uses Adam (DS:102); momentum / adagrad / rmsprop are TF1's MomentumOptimizer, "
-                        "AdagradOptimizer and (non-centered) RMSPropOptimizer, applied on the ps")
+    p.add_argument("--optimizer", choices=["adam", "sgd", "momentum", "adagrad", "rmsprop", "adadelta", "ftrl",
+                                           "proximal_adagrad", "proximal_sgd"], default="adam",
+                   help="reference uses Adam (DS:102); momentum / adagrad / rmsprop / adadelta / ftrl / "
+                        "proximal_adagrad / proximal_sgd are TF1's MomentumOptimizer, AdagradOptimizer, (non-centered) "
+                        "RMSPropOptimizer, AdadeltaOptimizer, FtrlOptimizer, ProximalAdagradOptimizer and "
+                        "ProximalGradientDescentOptimizer, applied on the ps")
     p.add_argument("--adam_math", choices=["fast", "ieee"], default="fast",
-                   help="ps-side arithmetic of Adam, Adagrad and RMSProp (cuda): MUFU sqrt/reciprocal (default) or "
-                        "correctly rounded like TF's Apply* kernels")
+                   help="ps-side arithmetic of every optimizer with a square root or a power (cuda): MUFU "
+                        "sqrt/reciprocal/power (default) or correctly rounded like TF's Apply* kernels")
     # optimizer hyper-parameters: unset = the chosen optimizer's TF1 default; one it does not use is an error
     p.add_argument("--momentum", type=float, default=None, help="momentum (0.9) and rmsprop (0.0)")
     p.add_argument("--use_nesterov", action="store_true", help="momentum: Nesterov momentum")
     p.add_argument("--rmsprop_decay", type=float, default=None, help="rmsprop: decay of the mean square (0.9)")
     p.add_argument("--initial_accumulator_value", type=float, default=None,
-                   help="adagrad: starting value of the accumulator (0.1)")
-    p.add_argument("--epsilon", type=float, default=None, help="adam (1e-8) and rmsprop (1e-10)")
+                   help="adagrad, ftrl and proximal_adagrad: starting value of the accumulator (0.1)")
+    p.add_argument("--epsilon", type=float, default=None, help="adam (1e-8), rmsprop (1e-10) and adadelta (1e-8)")
+    p.add_argument("--rho", type=float, default=None, help="adadelta: decay of both accumulators (0.95)")
+    p.add_argument("--l1_regularization_strength", type=float, default=None,
+                   help="ftrl, proximal_adagrad and proximal_sgd: l1 strength of the ps-side proximal step, which "
+                        "sets weights to exact zeros (0.0)")
+    p.add_argument("--l2_regularization_strength", type=float, default=None,
+                   help="ftrl, proximal_adagrad and proximal_sgd: l2 strength of the ps-side proximal step (0.0). This "
+                        "is the optimizer's own term, not the worker-side --l2_regularization loss term; both may be "
+                        "given")
+    p.add_argument("--l2_shrinkage_regularization_strength", type=float, default=None,
+                   help="ftrl: magnitude shrinkage added to the gradient, TF's FTRL V2 (0.0: off)")
+    p.add_argument("--learning_rate_power", type=float, default=None,
+                   help="ftrl: power of the per-coordinate rate, <= 0 (-0.5)")
     # learning-rate schedule over the global step (TF1's tf.train.*_decay / piecewise_constant), evaluated on the ps
     # when a push is applied; a parameter flag the schedule does not use is an error
     p.add_argument("--lr_schedule", choices=list(LR_SCHEDULES), default="constant",

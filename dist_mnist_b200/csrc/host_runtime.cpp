@@ -48,7 +48,14 @@ struct CpuPs {
   std::atomic<uint64_t> applied{0};
 };
 
-// TF1 Apply{Momentum,Adagrad,RMSProp} with IEEE arithmetic (ps_apply_sm90.cu tf1_step)
+// ApplyProximalAdagrad / ApplyProximalGradientDescent's proximal step at step size a (ps_apply_sm90.cu prox_shrink)
+float prox_shrink_cpu(float prox, float a, float l1, float l2) {
+  const float num = l1 > 0.f ? std::copysign(std::fmax(std::fabs(prox) - a * l1, 0.f), prox) : prox;
+  return num / (1.f + l2 * a);
+}
+
+// TF1 Apply{Momentum,Adagrad,RMSProp,Adadelta,FtrlV2,ProximalAdagrad,ProximalGradientDescent} with IEEE arithmetic and
+// the C library's float functions (ps_apply_sm90.cu tf1_step)
 void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, float& v, float g) {
   if (P.opt == dm::OPT_MOMENTUM) {
     m = P.momentum * m + g;
@@ -57,19 +64,42 @@ void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, floa
   } else if (P.opt == dm::OPT_ADAGRAD) {
     v += g * g;
     p -= lr * g / std::sqrt(v);
-  } else {   // OPT_RMSPROP
+  } else if (P.opt == dm::OPT_RMSPROP) {
     v += (g * g - v) * (1.f - P.decay);
     m = P.momentum * m + lr * g / std::sqrt(v + P.eps);
     p -= m;
+  } else if (P.opt == dm::OPT_ADADELTA) {   // v = accum, m = accum_update, rho = P.decay
+    v = v * P.decay + g * g * (1.f - P.decay);
+    const float upd = std::sqrt(m + P.eps) * (1.f / std::sqrt(v + P.eps)) * g;
+    p -= upd * lr;
+    m = m * P.decay + upd * upd * (1.f - P.decay);
+  } else if (P.opt == dm::OPT_PROXIMAL_ADAGRAD) {   // v = accumulator
+    v += g * g;
+    const float a = lr * (1.f / std::sqrt(v));
+    p = prox_shrink_cpu(p - g * a, a, P.l1, P.l2);
+  } else if (P.opt == dm::OPT_PROXIMAL_SGD) {
+    p = prox_shrink_cpu(p - lr * g, lr, P.l1, P.l2);
+  } else {   // OPT_FTRL: v = accum, m = linear
+    const float gs = g + 2.f * P.l2_shrinkage * p;
+    const float n = v + g * g;
+    const bool half = P.lr_power == -0.5f;
+    const float pn = half ? std::sqrt(n) : std::pow(n, -P.lr_power);
+    const float pa = half ? std::sqrt(v) : std::pow(v, -P.lr_power);
+    m += gs - (pn - pa) / lr * p;
+    const float y = pn / lr + 2.f * P.l2;
+    p = std::fabs(m) > P.l1 ? (std::copysign(P.l1, m) - m) / y : 0.f;
+    v = n;
   }
 }
 
 void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItemState st, uint32_t mask,
                     const uint32_t* seqs) {
   const uint64_t wstride = static_cast<uint64_t>(P.nslots) * P.arena_elems;
-  const bool tf1 = P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
-  const bool use_m = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_RMSPROP;
-  const bool use_v = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP;
+  const bool tf1 = P.opt != dm::OPT_ADAM && P.opt != dm::OPT_SGD;
+  const bool use_m = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_RMSPROP ||
+                     P.opt == dm::OPT_ADADELTA || P.opt == dm::OPT_FTRL;
+  const bool use_v = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP ||
+                     P.opt == dm::OPT_ADADELTA || P.opt == dm::OPT_FTRL || P.opt == dm::OPT_PROXIMAL_ADAGRAD;
   // rate of the k-th push of the pass (workers in order), lr(sched_step + k); a merged step uses lr(sched_step)
   float lrs[dm::kMaxWorkers];
   for (int k = 0; k < __builtin_popcount(mask); ++k)

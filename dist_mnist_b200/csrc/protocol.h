@@ -149,8 +149,19 @@ struct PsItemState {  // persisted across serve-kernel launches and checkpointed
 };
 
 // TF1 `training_ops` rules applied per push (or per round, APPLY_MERGED). Slot buffers: adam_m = Adam m / momentum
-// accumulator / RMSProp mom; adam_v = Adam v / Adagrad accumulator / RMSProp ms.
-enum OptimizerKind : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_MOMENTUM = 2, OPT_ADAGRAD = 3, OPT_RMSPROP = 4 };
+// accumulator / RMSProp mom / Adadelta accum_update / FTRL linear; adam_v = Adam v / Adagrad accumulator / RMSProp ms /
+// Adadelta accum / FTRL accum / ProximalAdagrad accumulator. ProximalGradientDescent has no slot.
+enum OptimizerKind : int {
+  OPT_SGD = 0,
+  OPT_ADAM = 1,
+  OPT_MOMENTUM = 2,
+  OPT_ADAGRAD = 3,
+  OPT_RMSPROP = 4,
+  OPT_ADADELTA = 5,
+  OPT_FTRL = 6,
+  OPT_PROXIMAL_ADAGRAD = 7,
+  OPT_PROXIMAL_SGD = 8,
+};
 enum ApplyMode : int {
   APPLY_PER_PUSH = 0,  // reference semantics: every worker push is its own optimizer step
   APPLY_MERGED = 1,    // pushes that are ready at the same poll are summed and applied as one step
@@ -198,7 +209,7 @@ struct PsServeParams {
   // hyper-parameters of the rules after Adam / SGD (appended, so that no earlier field moves); `eps` above is also
   // RMSProp's epsilon
   float momentum;              // OPT_MOMENTUM, OPT_RMSPROP
-  float decay;                 // OPT_RMSPROP (TF1 `decay`, rho)
+  float decay;                 // OPT_RMSPROP (TF1 `decay`), OPT_ADADELTA (TF1 `rho`)
   uint32_t nesterov;           // OPT_MOMENTUM: 1 = use_nesterov
   uint32_t pad_;
   // learning-rate schedule (TF1 tf.train.*_decay / piecewise_constant; appended, so that no earlier field moves).
@@ -221,6 +232,12 @@ struct PsServeParams {
   float* ema;                  // [arena] shadow variables of the fp32 parameters; null = off (unaveraged kernels)
   float ema_decay;
   uint32_t ema_num_updates;    // 1: d warms up with n (TF1 num_updates=global_step); 0: d = ema_decay
+  // hyper-parameters of FTRL and the proximal rules (appended, so that no earlier field moves); `eps` above is also
+  // Adadelta's epsilon, `decay` its rho
+  float l1;                    // OPT_FTRL, OPT_PROXIMAL_ADAGRAD, OPT_PROXIMAL_SGD: l1_regularization_strength (>= 0)
+  float l2;                    //   the same three: l2_regularization_strength (>= 0)
+  float l2_shrinkage;          // OPT_FTRL: l2_shrinkage_regularization_strength (>= 0; 0 = ApplyFtrl, else ApplyFtrlV2)
+  float lr_power;              // OPT_FTRL: learning_rate_power (<= 0; -0.5 takes the square-root path)
 };
 enum LrScheduleKind : int {
   LR_CONSTANT = 0,

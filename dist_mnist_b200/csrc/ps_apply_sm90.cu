@@ -5,8 +5,9 @@
 // shard (params + Adam slots + global_step, DS:88-91,102-103), polls the per-item flags that workers
 // publish with st.release.sys after their in-kernel P2P gradient stores, reduces whatever is ready
 // (many-to-one) and applies the optimizer in the same pass (ApplyAdam / SGD, SURVEY K7; or TF1's
-// ApplyMomentum / ApplyAdagrad / ApplyRMSProp in their own instantiations), bumps
-// global_step (K8) and acknowledges into the worker's inbox over NVLink. No host, NCCL or gRPC in the loop.
+// ApplyMomentum / ApplyAdagrad / ApplyRMSProp / ApplyAdadelta / ApplyFtrl(V2) / ApplyProximalAdagrad /
+// ApplyProximalGradientDescent in their own instantiations), bumps global_step (K8) and acknowledges into the
+// worker's inbox over NVLink. No host, NCCL or gRPC in the loop.
 //
 // Work decomposition: items (2-D blocks of the arena) are dealt round-robin to CTAs; a CTA never shares
 // an item, so item state (Adam step count / beta powers) needs no synchronisation. Pushes of one worker
@@ -65,6 +66,36 @@ __device__ __forceinline__ float div_sqrt(float a, float x) {   // a / sqrt(x)
   if constexpr (kIeee) return __fdiv_rn(a, __fsqrt_rn(x));
   else return a * rsqrt_approx(x);
 }
+// Adadelta, FTRL and the proximal rules (Apply{Adadelta,Ftrl,FtrlV2,ProximalAdagrad,ProximalGradientDescent}): fast =
+// the MUFU helpers above (and __powf for FTRL's general power), IEEE = correctly rounded sqrt / divide (rsqrt as 1 /
+// sqrt) and powf.
+template <bool kIeee>
+__device__ __forceinline__ float sqrt_m(float x) {
+  if constexpr (kIeee) return __fsqrt_rn(x);
+  else return sqrt_approx(x);
+}
+template <bool kIeee>
+__device__ __forceinline__ float rsqrt_m(float x) {
+  if constexpr (kIeee) return __fdiv_rn(1.f, __fsqrt_rn(x));
+  else return rsqrt_approx(x);
+}
+template <bool kIeee>
+__device__ __forceinline__ float div_m(float a, float b) {
+  if constexpr (kIeee) return __fdiv_rn(a, b);
+  else return a * rcp_approx(b);
+}
+template <bool kIeee>
+__device__ __forceinline__ float pow_m(float x, float y) {
+  if constexpr (kIeee) return powf(x, y);
+  else return __powf(x, y);
+}
+// The proximal step of ApplyProximalAdagrad / ApplyProximalGradientDescent at step size `a`:
+//   l1 > 0: sign(prox) max(|prox| - a l1, 0) / (1 + l2 a) ; else prox / (1 + l2 a)
+template <bool kIeee>
+__device__ __forceinline__ float prox_shrink(float prox, float a, float l1, float l2) {
+  const float num = l1 > 0.f ? copysignf(fmaxf(fabsf(prox) - a * l1, 0.f), prox) : prox;
+  return div_m<kIeee>(num, fmaf(l2, a, 1.f));
+}
 // kSched: the step's rate is `lr_sched`; else P.lr (read from the parameter block as the measured instantiations do)
 template <int kOpt, bool kIeee, bool kSched>
 __device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, const PsServeParams& P,
@@ -79,18 +110,55 @@ __device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, 
     // accum <- accum + g^2 ; p <- p - lr g / sqrt(accum)   (no epsilon)
     v = fmaf(g, g, v);
     p = p - div_sqrt<kIeee>(lr * g, v);
-  } else {
-    static_assert(kOpt == OPT_RMSPROP, "unknown optimizer family");
+  } else if constexpr (kOpt == OPT_RMSPROP) {
     // ms <- ms + (g^2 - ms)(1 - decay) ; mom <- momentum mom + lr g / sqrt(ms + eps) ; p <- p - mom
     v = fmaf(fmaf(g, g, -v), 1.f - P.decay, v);
     m = fmaf(P.momentum, m, div_sqrt<kIeee>(lr * g, v + P.eps));
     p = p - m;
+  } else if constexpr (kOpt == OPT_ADADELTA) {
+    // accum <- rho accum + (1 - rho) g^2 ; update = sqrt(accum_update + eps) rsqrt(accum + eps) g ; p <- p - lr update ;
+    // accum_update <- rho accum_update + (1 - rho) update^2   (rho rides in P.decay; v = accum, m = accum_update)
+    const float rho = P.decay;
+    v = fmaf(v, rho, g * g * (1.f - rho));
+    const float upd = sqrt_m<kIeee>(m + P.eps) * rsqrt_m<kIeee>(v + P.eps) * g;
+    p = fmaf(-upd, lr, p);
+    m = fmaf(m, rho, upd * upd * (1.f - rho));
+  } else if constexpr (kOpt == OPT_PROXIMAL_ADAGRAD) {
+    // accum <- accum + g^2 ; a = lr rsqrt(accum) ; p <- shrink(p - g a, a)
+    v = fmaf(g, g, v);
+    const float a = lr * rsqrt_m<kIeee>(v);
+    p = prox_shrink<kIeee>(fmaf(-g, a, p), a, P.l1, P.l2);
+  } else if constexpr (kOpt == OPT_PROXIMAL_SGD) {
+    // p <- shrink(p - lr g, lr)   (no square root: one instantiation, IEEE divide)
+    p = prox_shrink<true>(fmaf(-lr, g, p), lr, P.l1, P.l2);
+  } else {
+    static_assert(kOpt == OPT_FTRL, "unknown optimizer family");
+    // ApplyFtrlV2 (l2_shrinkage 0: ApplyFtrl, gs = g exactly). v = accum, m = linear.
+    //   n = accum + g^2 ; linear += gs - (n^-lr_power - accum^-lr_power) / lr p ;
+    //   p <- |linear| > l1 ? (sign(linear) l1 - linear) / (n^-lr_power / lr + 2 l2) : 0 ; accum <- n
+    const float gs = fmaf(2.f * P.l2_shrinkage, p, g);
+    const float n = fmaf(g, g, v);
+    float pn, pa;
+    if (P.lr_power == -0.5f) {   // TF's special case: sqrt
+      pn = sqrt_m<kIeee>(n);
+      pa = sqrt_m<kIeee>(v);
+    } else {
+      pn = pow_m<kIeee>(n, -P.lr_power);
+      pa = pow_m<kIeee>(v, -P.lr_power);
+    }
+    m = m + (gs - div_m<kIeee>(pn - pa, lr) * p);
+    const float y = div_m<kIeee>(pn, lr) + 2.f * P.l2;
+    p = fabsf(m) > P.l1 ? div_m<kIeee>(copysignf(P.l1, m) - m, y) : 0.f;
+    v = n;
   }
 }
 
 // Optimizer family of a serve-kernel instantiation. Adam and SGD share the two instantiations that were measured (P.opt
 // picks the rule at run time; their SASS is unchanged by the other families); every other kind gets its own.
 constexpr int kFamAdamSgd = -1;
+// Adadelta, FTRL, ProximalAdagrad and ProximalGradientDescent: their gradient chunks are set apart (kChFtrlProx), so
+// that the chunks of the families before them stay as measured.
+constexpr bool is_ftrl_prox(int kFam) { return kFam >= OPT_ADADELTA; }
 
 // Apply every pending push to one item. s_pend[0..n_pend) lists the mailbox slots (element offset of the slot
 // inside P.mailbox) in application order — round k = the k-th pending push of every worker, oldest round first —
@@ -109,6 +177,24 @@ struct ResidentState {
 struct ResidentEma {
   float e[kQuads][4];
 };
+// Gradient loads in flight in the instantiations of Adadelta, FTRL and the proximal rules: the largest chunk at which
+// ptxas reports no spill under __launch_bounds__(kPsThreads, 1) (see kCh in apply_item).
+//   constant rate: fast FTRL 8; every other one spills at 8 and takes 7.
+//   scheduled:     fast FTRL and fast Adadelta 8; every other one spills at 8 and takes 7.
+//   averaging:     fast ProximalAdagrad 7; Adadelta and FTRL (both) spill at 7 and take 6; IEEE ProximalAdagrad and
+//                  ProximalGradientDescent spill at 6 and take 5.
+template <int kFam, bool kIeee, bool kSched, bool kEma>
+constexpr int kChFtrlProx() {
+  if constexpr (kEma) {
+    if constexpr (kFam == OPT_PROXIMAL_ADAGRAD) return kIeee ? kChunk - 3 : kChunk - 1;
+    else if constexpr (kFam == OPT_PROXIMAL_SGD) return kChunk - 3;
+    else return kChunk - 2;
+  } else if constexpr (kSched) {
+    return (!kIeee && (kFam == OPT_FTRL || kFam == OPT_ADADELTA)) ? kChunk : kChunk - 1;
+  } else {
+    return (!kIeee && kFam == OPT_FTRL) ? kChunk : kChunk - 1;
+  }
+}
 // Gradient loads in flight in the averaging instantiations (see kCh in apply_item).
 template <int kFam, bool kIeee>
 constexpr int kChEma() {
@@ -132,8 +218,11 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
   const int step = vec ? 4 : 1;
   const bool adam = kFam == kFamAdamSgd && P.opt == OPT_ADAM;
   // the slot buffers this rule reads and writes
-  const bool use_m = kFam == kFamAdamSgd ? adam : (kFam == OPT_MOMENTUM || kFam == OPT_RMSPROP);
-  const bool use_v = kFam == kFamAdamSgd ? adam : (kFam == OPT_ADAGRAD || kFam == OPT_RMSPROP);
+  const bool use_m = kFam == kFamAdamSgd ? adam : (kFam == OPT_MOMENTUM || kFam == OPT_RMSPROP ||
+                                                   kFam == OPT_ADADELTA || kFam == OPT_FTRL);
+  const bool use_v = kFam == kFamAdamSgd ? adam : (kFam == OPT_ADAGRAD || kFam == OPT_RMSPROP ||
+                                                   kFam == OPT_ADADELTA || kFam == OPT_FTRL ||
+                                                   kFam == OPT_PROXIMAL_ADAGRAD);
   const bool merged = P.apply_mode == APPLY_MERGED;
   for (int e0 = tid * step; e0 < total; e0 += kPsThreads * step * kQuads) {
     uint64_t a[kQuads];
@@ -207,7 +296,10 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
     // The averaging instantiations hold 8 shadows more per thread (kChEma): Momentum and fast RMSProp do not spill at
     // 7; Adagrad (both), IEEE RMSProp and fast Adam / SGD spill at 7 and take 6; IEEE Adam / SGD spills at 6 and
     // takes 5.
-    constexpr int kCh = kEma ? kChEma<kFam, kIeee>() : kChNoEma;
+    // Adadelta, FTRL and the proximal rules: kChFtrlProx.
+    constexpr int kCh = is_ftrl_prox(kFam) ? kChFtrlProx<kFam, kIeee, kSched, kEma>()
+                        : kEma             ? kChEma<kFam, kIeee>()
+                                           : kChNoEma;
     int r0 = 0;   // kSched, merged: position of the first push of the current round
     for (int i0 = 0; i0 < n_pend; i0 += kCh) {
       float g[kCh][kQuads][4];
@@ -321,7 +413,8 @@ __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_co
   constexpr bool kEma = false;
 #include "ps_serve_body.cuh"
 }
-// Momentum / Adagrad / RMSProp: ps_serve_kernel<kOpt, kIeee>.
+// Every other family (Momentum, Adagrad, RMSProp, Adadelta, FTRL, ProximalAdagrad, ProximalGradientDescent):
+// ps_serve_kernel<kOpt, kIeee>.
 template <int kOpt, bool kIeee>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
   constexpr int kFam = kOpt;
@@ -385,6 +478,17 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
       case OPT_RMSPROP:
         if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, true>, p);
         return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, false>, p);
+      case OPT_ADADELTA:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADADELTA, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADADELTA, false>, p);
+      case OPT_FTRL:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_FTRL, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_FTRL, false>, p);
+      case OPT_PROXIMAL_ADAGRAD:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
+      case OPT_PROXIMAL_SGD:
+        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_SGD, true>, p);
       default:
         return cudaErrorInvalidValue;
     }
@@ -403,6 +507,17 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
       case OPT_RMSPROP:
         if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, true>, p);
         return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, false>, p);
+      case OPT_ADADELTA:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADADELTA, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADADELTA, false>, p);
+      case OPT_FTRL:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_FTRL, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_FTRL, false>, p);
+      case OPT_PROXIMAL_ADAGRAD:
+        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
+      case OPT_PROXIMAL_SGD:
+        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_SGD, true>, p);
       default:
         return cudaErrorInvalidValue;
     }
@@ -420,6 +535,17 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
     case OPT_RMSPROP:
       if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, true>, p);
       return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, false>, p);
+    case OPT_ADADELTA:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADADELTA, true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADADELTA, false>, p);
+    case OPT_FTRL:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_FTRL, true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_FTRL, false>, p);
+    case OPT_PROXIMAL_ADAGRAD:
+      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
+    case OPT_PROXIMAL_SGD:   // no square root: one instantiation (IEEE divide) serves both math modes
+      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_SGD, true>, p);
     default:
       return cudaErrorInvalidValue;
   }
@@ -542,6 +668,27 @@ cudaError_t preload_ps_kernels() {
   if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
+  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, dense_apply_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, shadow_refresh_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, wait_ack_kernel)) != cudaSuccess) return e;

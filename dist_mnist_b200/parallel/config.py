@@ -19,15 +19,24 @@ def _env_flag(name: str, default: bool) -> bool:
 
 
 _NATIVE_KINDS = {"adam": N.OPT_ADAM, "sgd": N.OPT_SGD, "momentum": N.OPT_MOMENTUM, "adagrad": N.OPT_ADAGRAD,
-                 "rmsprop": N.OPT_RMSPROP}
+                 "rmsprop": N.OPT_RMSPROP, "adadelta": N.OPT_ADADELTA, "ftrl": N.OPT_FTRL,
+                 "proximal_adagrad": N.OPT_PROXIMAL_ADAGRAD, "proximal_sgd": N.OPT_PROXIMAL_SGD}
 # the kinds after Adam / SGD: their slot buffers hold other state, so ps, chief and checkpoints must agree on the kind
-TF1_SLOT_KINDS = ("momentum", "adagrad", "rmsprop")
+TF1_SLOT_KINDS = ("momentum", "adagrad", "rmsprop", "adadelta", "ftrl", "proximal_adagrad", "proximal_sgd")
+_PROXIMAL = ("ftrl", "proximal_adagrad", "proximal_sgd")
+_FTRL_PROX_HPARAMS = ("rho", "l1_regularization_strength", "l2_regularization_strength",
+                      "l2_shrinkage_regularization_strength", "learning_rate_power")
 # hyper-parameters beyond lr / beta1 / beta2 / eps, the kinds that use each, and the TF1 default per kind
 # (TF1's MomentumOptimizer has no default momentum; 0.9 here)
 _EXTRA_DEFAULTS = {
     "momentum": {"momentum": 0.9, "rmsprop": 0.0},
     "decay": {"rmsprop": 0.9},
-    "initial_accumulator_value": {"adagrad": 0.1},
+    "initial_accumulator_value": {"adagrad": 0.1, "ftrl": 0.1, "proximal_adagrad": 0.1},
+    "rho": {"adadelta": 0.95},
+    "l1_regularization_strength": {k: 0.0 for k in _PROXIMAL},
+    "l2_regularization_strength": {k: 0.0 for k in _PROXIMAL},
+    "l2_shrinkage_regularization_strength": {"ftrl": 0.0},
+    "learning_rate_power": {"ftrl": -0.5},
 }
 
 
@@ -303,22 +312,33 @@ class L2Regularization:
 class OptimizerConfig:
     """Reference: `tf.train.AdamOptimizer(FLAGS.learning_rate)` with TF defaults (DS:102); SGD is the
     north-star "async-SGD" variant. "momentum", "adagrad" and "rmsprop" are TF1's `MomentumOptimizer`,
-    `AdagradOptimizer` and (non-centered) `RMSPropOptimizer`, applied on the ps with the `training_ops` formulas.
+    `AdagradOptimizer` and (non-centered) `RMSPropOptimizer`, applied on the ps with the `training_ops` formulas;
+    "adadelta", "ftrl", "proximal_adagrad" and "proximal_sgd" likewise are `AdadeltaOptimizer`, `FtrlOptimizer` (V2
+    when l2_shrinkage_regularization_strength > 0), `ProximalAdagradOptimizer` and `ProximalGradientDescentOptimizer`.
+    Their l1 / l2 strengths are the ps-side proximal terms of those optimizers, not the worker-side loss term `l2`.
 
     A hyper-parameter left at None takes the kind's TF1 default; giving one that the kind does not use is an error."""
-    kind: str = "adam"          # "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop"
+    kind: str = "adam"          # "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop" | "adadelta" | "ftrl" |
+                                # "proximal_adagrad" | "proximal_sgd"
     lr: float = 1e-4            # --learning_rate default (DS:15)
     beta1: float = 0.9
     beta2: float = 0.999
-    eps: Optional[float] = None   # Adam 1e-8 (also kept for the kinds without an epsilon), RMSProp 1e-10
-    math: str = "fast"          # ps-side arithmetic of every rule with a square root (Adam, Adagrad, RMSProp) on the
+    eps: Optional[float] = None   # Adam and Adadelta 1e-8 (also kept for the kinds without an epsilon), RMSProp 1e-10
+    math: str = "fast"          # ps-side arithmetic of every rule with a square root (all but SGD, Momentum and
+                                # ProximalGradientDescent; FTRL's general power too) on the
                                 # cuda backend: "fast" (MUFU, <= 2 ulp, the measured configuration) | "ieee" (correctly
                                 # rounded sqrt and divide, like TF's Apply* kernels; ~4x the per-push apply cost for
                                 # Adam). The cpu backend is always IEEE.
     momentum: Optional[float] = None    # "momentum" (0.9), "rmsprop" (0.0)
     use_nesterov: bool = False          # "momentum"
     decay: Optional[float] = None       # "rmsprop" (0.9)
-    initial_accumulator_value: Optional[float] = None   # "adagrad" (0.1): Adagrad's slot starts here, not at 0
+    initial_accumulator_value: Optional[float] = None   # "adagrad", "ftrl", "proximal_adagrad" (0.1): the
+                                                        # accumulator slot starts here, not at 0
+    rho: Optional[float] = None                         # "adadelta" (0.95)
+    l1_regularization_strength: Optional[float] = None  # "ftrl", "proximal_adagrad", "proximal_sgd" (0.0)
+    l2_regularization_strength: Optional[float] = None  # the same three (0.0)
+    l2_shrinkage_regularization_strength: Optional[float] = None   # "ftrl" (0.0; > 0: ApplyFtrlV2)
+    learning_rate_power: Optional[float] = None         # "ftrl" (-0.5)
     schedule: LrSchedule = LrSchedule()   # learning-rate schedule over the global step (default: constant `lr`)
     # TF1 `tf.train.ExponentialMovingAverage(decay, num_updates=global_step).apply(tf.trainable_variables())`, run on
     # the ps after every optimizer step (zero_debias=False): every model variable gets a shadow that starts at the
@@ -344,8 +364,23 @@ class OptimizerConfig:
                 raise ValueError(f"optimizer {self.kind!r} has no hyper-parameter {name!r}")
         if self.use_nesterov and self.kind != "momentum":
             raise ValueError(f"use_nesterov applies to the momentum optimizer, not {self.kind!r}")
-        if self.kind == "adagrad" and not self.initial_accumulator_value > 0:
-            raise ValueError("initial_accumulator_value must be positive (Adagrad divides by its square root)")
+        if self.kind in ("adagrad", "proximal_adagrad") and not self.initial_accumulator_value > 0:
+            raise ValueError(f"initial_accumulator_value must be positive ({self.kind} divides by its square root)")
+        if self.kind in ("adadelta",) + _PROXIMAL:   # every hyper-parameter finite
+            for name in ("lr", "eps", "initial_accumulator_value") + _FTRL_PROX_HPARAMS:
+                x = getattr(self, name)
+                if x is not None and (isinstance(x, bool) or not isinstance(x, (int, float)) or not math.isfinite(x)):
+                    raise ValueError(f"{name} must be a finite number, got {x!r}")
+            if self.kind != "adadelta" and not self.lr > 0:   # TF's Apply{Ftrl,Proximal*} kernels: "lr is not positive"
+                raise ValueError(f"optimizer {self.kind!r} needs a positive learning rate, got {self.lr!r}")
+        for name in ("l1_regularization_strength", "l2_regularization_strength", "l2_shrinkage_regularization_strength"):
+            if getattr(self, name) is not None and getattr(self, name) < 0:
+                raise ValueError(f"{name} must be >= 0, got {getattr(self, name)!r}")
+        if self.kind == "ftrl":
+            if self.initial_accumulator_value < 0:
+                raise ValueError(f"initial_accumulator_value must be >= 0 for ftrl, got {self.initial_accumulator_value!r}")
+            if self.learning_rate_power > 0:
+                raise ValueError(f"learning_rate_power must be <= 0, got {self.learning_rate_power!r}")
         if not isinstance(self.schedule, LrSchedule):
             raise ValueError(f"schedule must be an LrSchedule, got {type(self.schedule).__name__}")
         if not isinstance(self.clip, GradClip):
@@ -386,13 +421,25 @@ class OptimizerConfig:
         raise ValueError(f"unknown optimizer {self.kind!r} ({' | '.join(_NATIVE_KINDS)})")
 
     def slot_init(self) -> Tuple[float, float]:
-        """Initial values of the two slot buffers (adam_m, adam_v): Adagrad's accumulator starts at
-        initial_accumulator_value and RMSProp's ms at 1 (TF1's `ones_initializer`); every other slot at 0."""
-        if self.kind == "adagrad":
+        """Initial values of the two slot buffers (adam_m, adam_v): the accumulator of Adagrad, FTRL and
+        ProximalAdagrad starts at initial_accumulator_value and RMSProp's ms at 1 (TF1's `ones_initializer`); every
+        other slot (FTRL's linear, both of Adadelta's) at 0."""
+        if self.kind in ("adagrad", "ftrl", "proximal_adagrad"):
             return 0.0, float(self.initial_accumulator_value)
         if self.kind == "rmsprop":
             return 0.0, 1.0
         return 0.0, 0.0
+
+    def fill_native_rule(self, P) -> None:
+        """Write the rule's hyper-parameters beyond lr / beta1 / beta2 / eps into a PsServeParams (Adadelta's rho rides
+        in `decay`)."""
+        P.momentum = self.momentum or 0.0
+        P.decay = self.rho if self.kind == "adadelta" else (self.decay or 0.0)
+        P.nesterov = int(self.use_nesterov)
+        P.l1 = self.l1_regularization_strength or 0.0
+        P.l2 = self.l2_regularization_strength or 0.0
+        P.l2_shrinkage = self.l2_shrinkage_regularization_strength or 0.0
+        P.lr_power = self.learning_rate_power or 0.0
 
     def as_dict(self) -> dict:
         d = asdict(self)

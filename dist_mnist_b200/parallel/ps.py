@@ -173,9 +173,7 @@ class ParameterServer:
         P.oneshot = 0
         P.opt, P.apply_mode = opt.native_kind, cfg.native_apply_mode
         P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
-        P.momentum = opt.momentum or 0.0
-        P.decay = opt.decay or 0.0
-        P.nesterov = int(opt.use_nesterov)
+        opt.fill_native_rule(P)   # momentum, decay (Adadelta's rho), nesterov, l1, l2, l2_shrinkage, lr_power
         opt.schedule.fill_native(P)   # non-constant: the scheduled serve kernels / the cpu loop's rate table
         P.ieee_math = 1 if opt.math == "ieee" else 0
         # moving averages: the averaging serve kernels / the cpu loop's shadow update

@@ -34,6 +34,11 @@ def save_checkpoint(worker, directory: str) -> str:
                       "beta2": worker.opt.beta2, "eps": worker.opt.eps, "momentum": worker.opt.momentum,
                       "use_nesterov": worker.opt.use_nesterov, "decay": worker.opt.decay,
                       "initial_accumulator_value": worker.opt.initial_accumulator_value,
+                      "rho": worker.opt.rho,
+                      "l1_regularization_strength": worker.opt.l1_regularization_strength,
+                      "l2_regularization_strength": worker.opt.l2_regularization_strength,
+                      "l2_shrinkage_regularization_strength": worker.opt.l2_shrinkage_regularization_strength,
+                      "learning_rate_power": worker.opt.learning_rate_power,
                       "schedule": worker.opt.schedule.as_dict(),
                       "moving_average_decay": worker.opt.moving_average_decay,
                       "moving_average_num_updates": worker.opt.moving_average_num_updates},
@@ -84,8 +89,8 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
         raise RuntimeError(f"unsupported checkpoint format in {path}")
     if tuple(state["hidden"]) != tuple(worker.spec.hidden):
         raise RuntimeError(f"checkpoint {path} is for hidden={state['hidden']}, model has {worker.spec.hidden}")
-    # adam_m / adam_v hold a different optimizer's state under Momentum / Adagrad / RMSProp (TF fails on the missing
-    # slot variables in this case)
+    # adam_m / adam_v hold a different optimizer's state under every kind but Adam and SGD (TF fails on the missing
+    # slot variables in this case); only the kind is read, so checkpoints without the later hyper-parameters restore
     kind = state.get("optimizer", {}).get("kind")
     if kind != worker.opt.kind and (kind in TF1_SLOT_KINDS or worker.opt.kind in TF1_SLOT_KINDS):
         raise RuntimeError(f"checkpoint {path} holds {kind!r} optimizer slots, this run uses {worker.opt.kind!r}")
