@@ -96,10 +96,8 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
                     const uint32_t* seqs) {
   const uint64_t wstride = static_cast<uint64_t>(P.nslots) * P.arena_elems;
   const bool tf1 = P.opt != dm::OPT_ADAM && P.opt != dm::OPT_SGD;
-  const bool use_m = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_MOMENTUM || P.opt == dm::OPT_RMSPROP ||
-                     P.opt == dm::OPT_ADADELTA || P.opt == dm::OPT_FTRL;
-  const bool use_v = P.opt == dm::OPT_ADAM || P.opt == dm::OPT_ADAGRAD || P.opt == dm::OPT_RMSPROP ||
-                     P.opt == dm::OPT_ADADELTA || P.opt == dm::OPT_FTRL || P.opt == dm::OPT_PROXIMAL_ADAGRAD;
+  const bool use_m = dm::opt_uses_m(P.opt);
+  const bool use_v = dm::opt_uses_v(P.opt);
   // rate of the k-th push of the pass (workers in order), lr(sched_step + k); a merged step uses lr(sched_step)
   float lrs[dm::kMaxWorkers];
   for (int k = 0; k < __builtin_popcount(mask); ++k)
@@ -119,17 +117,8 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
       if (use_v) v = P.adam_v[a];
       if (ema) e = P.ema[a];
       float b1p = st.beta1_pow, b2p = st.beta2_pow;
-      float gsum = 0.f;
-      uint32_t mm = mask;
-      int k = 0;
-      while (mm) {
-        const int w = __builtin_ffs(mm) - 1;
-        mm &= mm - 1;
-        const uint32_t slot = seqs[w] % P.nslots;
-        const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
-        if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
-        const float omd = ema ? ema_omd[k] : 0.f;
-        const float lr = lrs[k++];
+      // one optimizer step with gradient g at rate lr, then the moving average with 1 - d = omd
+      const auto apply_step = [&](float g, float lr, float omd) {
         if (tf1) {
           tf1_step_cpu(P, lr, p, m, v, g);
         } else if (P.opt == dm::OPT_ADAM) {
@@ -142,22 +131,20 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
           p -= lr * g;
         }
         if (ema) e -= (e - p) * omd;   // assign_moving_average
+      };
+      float gsum = 0.f;
+      uint32_t mm = mask;
+      int k = 0;
+      while (mm) {
+        const int w = __builtin_ffs(mm) - 1;
+        mm &= mm - 1;
+        const uint32_t slot = seqs[w] % P.nslots;
+        const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
+        if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
+        const float omd = ema ? ema_omd[k] : 0.f;
+        apply_step(g, lrs[k++], omd);
       }
-      if (P.apply_mode == dm::APPLY_MERGED) {
-        const float lr = lrs[0];
-        if (tf1) {
-          tf1_step_cpu(P, lr, p, m, v, gsum);
-        } else if (P.opt == dm::OPT_ADAM) {
-          b1p *= P.beta1; b2p *= P.beta2;
-          const float lr_t = lr * std::sqrt(1.f - b2p) / (1.f - b1p);
-          m = P.beta1 * m + (1.f - P.beta1) * gsum;
-          v = P.beta2 * v + (1.f - P.beta2) * gsum * gsum;
-          p -= lr_t * m / (std::sqrt(v) + P.eps);
-        } else {
-          p -= lr * gsum;
-        }
-        if (ema) e -= (e - p) * ema_omd[npush - 1];
-      }
+      if (P.apply_mode == dm::APPLY_MERGED) apply_step(gsum, lrs[0], ema ? ema_omd[npush - 1] : 0.f);
       P.params[a] = p;
       if (use_m) P.adam_m[a] = m;
       if (use_v) P.adam_v[a] = v;

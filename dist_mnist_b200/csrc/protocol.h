@@ -162,6 +162,14 @@ enum OptimizerKind : int {
   OPT_PROXIMAL_ADAGRAD = 7,
   OPT_PROXIMAL_SGD = 8,
 };
+// The slot buffers rule `opt` reads and writes (the serve kernel and the CPU serve loop load and store only these).
+constexpr bool opt_uses_m(int opt) {
+  return opt == OPT_ADAM || opt == OPT_MOMENTUM || opt == OPT_RMSPROP || opt == OPT_ADADELTA || opt == OPT_FTRL;
+}
+constexpr bool opt_uses_v(int opt) {
+  return opt == OPT_ADAM || opt == OPT_ADAGRAD || opt == OPT_RMSPROP || opt == OPT_ADADELTA || opt == OPT_FTRL ||
+         opt == OPT_PROXIMAL_ADAGRAD;
+}
 enum ApplyMode : int {
   APPLY_PER_PUSH = 0,  // reference semantics: every worker push is its own optimizer step
   APPLY_MERGED = 1,    // pushes that are ready at the same poll are summed and applied as one step

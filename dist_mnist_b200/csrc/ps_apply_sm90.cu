@@ -22,7 +22,6 @@ namespace dm {
 constexpr int kPsThreads = 512;
 constexpr int kMaxOwn = 32;   // items one CTA may own (their descriptors / state / cursors live in shared memory)
 constexpr int kQuads = 2;     // element quads per thread per pass
-constexpr int kChunk = 8;     // pending pushes whose gradient loads are in flight together
 constexpr int kMaxPending = 32;
 
 // MUFU approximations (<= 2 ulp): the Adam update is issue-bound on the one SM that owns an item (IEEE sqrt and
@@ -153,18 +152,15 @@ __device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, 
   }
 }
 
-// Optimizer family of a serve-kernel instantiation. Adam and SGD share the two instantiations that were measured (P.opt
-// picks the rule at run time; their SASS is unchanged by the other families); every other kind gets its own.
+// Optimizer family of a serve-kernel instantiation. Adam and SGD share theirs (P.opt picks the rule at run time); every
+// other kind gets its own.
 constexpr int kFamAdamSgd = -1;
-// Adadelta, FTRL, ProximalAdagrad and ProximalGradientDescent: their gradient chunks are set apart (kChFtrlProx), so
-// that the chunks of the families before them stay as measured.
-constexpr bool is_ftrl_prox(int kFam) { return kFam >= OPT_ADADELTA; }
 
 // Apply every pending push to one item. s_pend[0..n_pend) lists the mailbox slots (element offset of the slot
 // inside P.mailbox) in application order — round k = the k-th pending push of every worker, oldest round first —
 // and s_round[i] is the round of entry i. One optimizer step per push, or per round in APPLY_MERGED mode
 // (concurrent pushes of different workers are summed; consecutive pushes of one worker stay separate steps).
-// Parameters and Adam slots stay in registers for the whole pass; the gradient loads of kChunk pushes are issued
+// Parameters and Adam slots stay in registers for the whole pass; the gradient loads of kCh pushes are issued
 // together (a mailbox line costs an L2/HBM round trip of ~1-2 us: issuing them one push at a time made the
 // pass, and with it the push->ack latency that throttles the workers, proportional to 5 us x pending pushes).
 // Optimizer state of an item held in registers across passes (see ps_serve_kernel): valid when the CTA owns exactly one
@@ -177,52 +173,39 @@ struct ResidentState {
 struct ResidentEma {
   float e[kQuads][4];
 };
-// Gradient loads in flight in the instantiations of Adadelta, FTRL and the proximal rules: the largest chunk at which
-// ptxas reports no spill under __launch_bounds__(kPsThreads, 1) (see kCh in apply_item).
-//   constant rate: fast FTRL 8; every other one spills at 8 and takes 7.
-//   scheduled:     fast FTRL and fast Adadelta 8; every other one spills at 8 and takes 7.
-//   averaging:     fast ProximalAdagrad 7; Adadelta and FTRL (both) spill at 7 and take 6; IEEE ProximalAdagrad and
-//                  ProximalGradientDescent spill at 6 and take 5.
-template <int kFam, bool kIeee, bool kSched, bool kEma>
-constexpr int kChFtrlProx() {
-  if constexpr (kEma) {
-    if constexpr (kFam == OPT_PROXIMAL_ADAGRAD) return kIeee ? kChunk - 3 : kChunk - 1;
-    else if constexpr (kFam == OPT_PROXIMAL_SGD) return kChunk - 3;
-    else return kChunk - 2;
-  } else if constexpr (kSched) {
-    return (!kIeee && (kFam == OPT_FTRL || kFam == OPT_ADADELTA)) ? kChunk : kChunk - 1;
-  } else {
-    return (!kIeee && kFam == OPT_FTRL) ? kChunk : kChunk - 1;
-  }
-}
-// Gradient loads in flight in the averaging instantiations (see kCh in apply_item).
-template <int kFam, bool kIeee>
-constexpr int kChEma() {
-  if constexpr (kFam == kFamAdamSgd) return kIeee ? kChunk - 3 : kChunk - 2;
-  else return (kFam == OPT_ADAGRAD || kIeee) ? kChunk - 2 : kChunk - 1;
-}
+// Pending pushes whose gradient loads are in flight together, per instantiation: the largest chunk that ptxas compiles
+// without a spill under __launch_bounds__(kPsThreads, 1) (IEEE Adam / SGD at a constant rate keeps the fast one's 8 and
+// spills 28 bytes). Indexed [family row][kIeee][constant rate, scheduled, averaging]; the family rows are Adam / SGD,
+// then OPT_MOMENTUM .. OPT_PROXIMAL_SGD in enum order. 0: no such instantiation (see serve_kernel).
+constexpr int kServeChunk[8][2][3] = {
+    {{8, 7, 6}, {8, 6, 5}},   // Adam / SGD
+    {{7, 7, 7}, {0, 0, 0}},   // Momentum
+    {{7, 7, 6}, {7, 7, 6}},   // Adagrad
+    {{7, 7, 7}, {7, 7, 6}},   // RMSProp
+    {{7, 8, 6}, {7, 7, 6}},   // Adadelta
+    {{8, 8, 6}, {7, 7, 6}},   // FTRL
+    {{7, 7, 7}, {7, 7, 5}},   // ProximalAdagrad
+    {{0, 0, 0}, {7, 7, 5}},   // ProximalGradientDescent
+};
+constexpr int serve_family_row(int fam) { return fam == kFamAdamSgd ? 0 : fam - OPT_MOMENTUM + 1; }
 
 // kSched (the scheduled instantiations): the rate of the optimizer step whose pushes sit at positions i0..i1 of the
 // application order is s_lr[i0], the pass's rate table (lr(sched_step + i), built by the serve loop); else P.lr.
 // kEma (the averaging instantiations, which are also kSched): the item's moving averages P.ema stay in registers for
 // the pass like the parameters, and after the optimizer step that ends at position i every element's shadow moves
 // toward the new parameter by 1 - s_ema[i], the pass's decay table (ema_decay(sched_step + i + 1)).
-template <bool kIeee, int kFam, bool kSched = false, bool kEma = false>
+template <int kFam, bool kIeee, bool kSched, bool kEma>
 __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItemState st, const uint64_t* s_pend,
-                           const uint32_t* s_round, const int n_pend, ResidentState* res = nullptr,
-                           const float* s_lr = nullptr, const float* s_ema = nullptr,
-                           ResidentEma* res_ema = nullptr) {
+                           const uint32_t* s_round, const int n_pend, ResidentState* res, const float* s_lr,
+                           const float* s_ema, ResidentEma* res_ema) {
   const int tid = threadIdx.x;
   const int total = it.rows * it.cols;
   const bool vec = ((it.cols & 3) == 0) && ((it.ld & 3) == 0) && ((it.offset & 3) == 0);
   const int step = vec ? 4 : 1;
   const bool adam = kFam == kFamAdamSgd && P.opt == OPT_ADAM;
   // the slot buffers this rule reads and writes
-  const bool use_m = kFam == kFamAdamSgd ? adam : (kFam == OPT_MOMENTUM || kFam == OPT_RMSPROP ||
-                                                   kFam == OPT_ADADELTA || kFam == OPT_FTRL);
-  const bool use_v = kFam == kFamAdamSgd ? adam : (kFam == OPT_ADAGRAD || kFam == OPT_RMSPROP ||
-                                                   kFam == OPT_ADADELTA || kFam == OPT_FTRL ||
-                                                   kFam == OPT_PROXIMAL_ADAGRAD);
+  const bool use_m = kFam == kFamAdamSgd ? adam : opt_uses_m(kFam);
+  const bool use_v = kFam == kFamAdamSgd ? adam : opt_uses_v(kFam);
   const bool merged = P.apply_mode == APPLY_MERGED;
   for (int e0 = tid * step; e0 < total; e0 += kPsThreads * step * kQuads) {
     uint64_t a[kQuads];
@@ -289,17 +272,8 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
       for (int j = 0; j < 4; ++j) gsum[q][j] = 0.f;
 
-    // the other families' straight-line update keeps more values live: a chunk of 8 spills there, 7 does not. The
-    // scheduled Adam / SGD instantiations (rate-table read, round start) spill at 8 too, and the IEEE one still at 7:
-    // 7 and 6 there; the scheduled Momentum / Adagrad / RMSProp ones do not spill at 7.
-    constexpr int kChNoEma = kFam != kFamAdamSgd ? kChunk - 1 : !kSched ? kChunk : kIeee ? kChunk - 2 : kChunk - 1;
-    // The averaging instantiations hold 8 shadows more per thread (kChEma): Momentum and fast RMSProp do not spill at
-    // 7; Adagrad (both), IEEE RMSProp and fast Adam / SGD spill at 7 and take 6; IEEE Adam / SGD spills at 6 and
-    // takes 5.
-    // Adadelta, FTRL and the proximal rules: kChFtrlProx.
-    constexpr int kCh = is_ftrl_prox(kFam) ? kChFtrlProx<kFam, kIeee, kSched, kEma>()
-                        : kEma             ? kChEma<kFam, kIeee>()
-                                           : kChNoEma;
+    constexpr int kCh = kServeChunk[serve_family_row(kFam)][kIeee][kEma ? 2 : kSched ? 1 : 0];
+    static_assert(kCh > 0, "no serve-kernel instantiation of this family and math");
     int r0 = 0;   // kSched, merged: position of the first push of the current round
     for (int i0 = 0; i0 < n_pend; i0 += kCh) {
       float g[kCh][kQuads][4];
@@ -405,41 +379,232 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
   }
 }
 
-// Adam / SGD: ps_serve_kernel<kIeee>, the two instantiations that were measured.
-template <bool kIeee>
+// kFam: optimizer family; kIeee: correctly rounded sqrt / divide. kSched: a non-constant learning-rate schedule
+// (P.lr_schedule != LR_CONSTANT). kEma: moving averages of the parameters (P.ema != null), under any schedule: the rate
+// table is compiled in as with kSched (scheduled_lr is lr0 for LR_CONSTANT), so one instantiation serves a constant rate
+// and every schedule. Everything a schedule adds sits behind `if constexpr (kSched)`, everything averaging adds behind
+// `if constexpr (kEma)`, so the constant-rate instantiations carry none of it.
+template <int kFam, bool kIeee, bool kSched, bool kEma>
 __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
-  constexpr int kFam = kFamAdamSgd;
-  constexpr bool kSched = false;
-  constexpr bool kEma = false;
-#include "ps_serve_body.cuh"
+  static_assert(kSched || !kEma, "the averaging instantiations read the rate table too");
+  // Everything the poll loop needs about this CTA's items lives in shared memory: the only global traffic of an
+  // idle poll is one acquire load of a flag word per (worker, look-ahead slot).
+  __shared__ PsItem s_item[kMaxOwn];
+  __shared__ PsItemState s_state[kMaxOwn];
+  __shared__ uint32_t s_next[kMaxOwn][kMaxWorkers];  // next expected push seq per (owned item, worker)
+  __shared__ uint64_t s_pend[kMaxPending];
+  __shared__ uint32_t s_round[kMaxPending];
+  __shared__ uint32_t s_npend;
+  __shared__ uint32_t s_any;
+  __shared__ uint32_t s_exit;
+  __shared__ float s_lr[kMaxPending];   // kSched: rate of the pass's i-th push, lr(sched_step + i)
+  __shared__ float s_ema[kMaxPending];  // kEma: decay of the step ending at the i-th push, ema_decay(sched_step + i + 1)
+  const int tid = threadIdx.x;
+  const int lane = tid & 31;
+  const int warp = tid >> 5;
+  uint32_t iter = 0;
+  int n_own = 0;
+  for (int item = blockIdx.x; item < P.n_items && n_own < kMaxOwn; item += gridDim.x) ++n_own;
+  for (int i = tid; i < n_own; i += kPsThreads) {
+    const int item = blockIdx.x + i * gridDim.x;
+    s_item[i] = P.items[item];
+    s_state[i] = P.item_state[item];
+  }
+  for (int i = tid; i < n_own * kMaxWorkers; i += kPsThreads) {
+    const int own = i / kMaxWorkers, w = i - own * kMaxWorkers;
+    s_next[own][w] = w < P.n_workers ? P.next_seq[static_cast<size_t>(w) * P.n_items + blockIdx.x + own * gridDim.x] : 0u;
+  }
+  __syncthreads();
+  // poll lanes, round-major: lane = k * n_workers + w checks push s_next[w] + k of worker w. Pushes of one worker
+  // are consumed in order, so only its contiguous ready prefix k = 0 .. cnt-1 is taken in a pass; lane order is
+  // then exactly the application order (round k = k-th pending push of every worker, oldest round first).
+  const int nw = P.n_workers;
+  int kdepth = max(1, min(min(P.nslots, 16), 32 / nw));
+  if (P.lookahead != 0u) kdepth = min(kdepth, static_cast<int>(P.lookahead));
+  const int pk = lane / nw, pw = lane - pk * nw;
+  const bool pvalid = pk < kdepth;
+  const uint64_t wstride = static_cast<uint64_t>(P.nslots) * P.arena_elems;
+
+  // Register-resident optimizer state: a CTA that owns exactly one vectorisable item of at most one sweep keeps the
+  // item's parameters and Adam slots in registers from pass to pass (it is the only writer while it runs; the host
+  // writes variables only while no serve kernel is resident). Results are still stored every pass — the workers pull
+  // the parameters, checkpoints read the slots — but the three load round trips (~1 us of a ~6.7 us pass) are gone.
+  ResidentState resident;
+  resident.loaded = false;
+  ResidentEma resident_ema;   // kEma: the shadows beside them
+  bool use_resident = false;
+  if (n_own == 1) {
+    const PsItem it0 = s_item[0];
+    use_resident = ((it0.cols & 3) == 0) && ((it0.ld & 3) == 0) && ((it0.offset & 3) == 0) &&
+                   (it0.rows * it0.cols <= kPsThreads * kQuads * 4);
+  }
+
+  // serve statistics (thread 0's view; the CTA barriers make it representative)
+  unsigned long long st_pass = 0, st_push = 0, st_apply = 0, st_book = 0, st_idle_n = 0, st_idle = 0, st_max = 0,
+                     st_poll = 0;
+  const bool stats_on = P.stats != nullptr;
+
+  for (;;) {
+    bool sweep_any = false;   // (uniform over the CTA: s_any is read after a barrier)
+    for (int own = 0; own < n_own; ++own) {
+      const int item = blockIdx.x + own * gridDim.x;
+      const long long c0 = stats_on ? clock64() : 0;
+      uint32_t p_seq = 0, p_cnt = 0, p_taken = 0;   // warp 0: this lane's push seq, its worker's prefix, all taken
+      bool p_take = false;
+      if (warp == 0) {
+        uint32_t ready = 0, slot = 0;
+        if (pvalid) {
+          p_seq = s_next[own][pw] + pk;
+          slot = p_seq % P.nslots;
+          const uint32_t f = ld_acquire_scoped_u32(
+              P.flags + (static_cast<size_t>(pw) * P.nslots + slot) * P.n_flags + s_item[own].flag_index, P.gpu_scope);
+          ready = (f == p_seq) ? 1u : 0u;
+        }
+        const uint32_t b = __ballot_sync(0xffffffffu, ready);
+        if (pvalid)
+          while (p_cnt < static_cast<uint32_t>(kdepth) && ((b >> (p_cnt * nw + pw)) & 1u)) ++p_cnt;
+        p_take = pvalid && static_cast<uint32_t>(pk) < p_cnt;
+        p_taken = __ballot_sync(0xffffffffu, p_take);
+        if (p_take) {
+          const int pos = __popc(p_taken & ((1u << lane) - 1u));
+          s_pend[pos] = static_cast<uint64_t>(pw) * wstride + static_cast<uint64_t>(slot) * P.arena_elems;
+          s_round[pos] = pk;
+        }
+        if (lane == 0) {
+          s_any = p_taken;
+          s_npend = __popc(p_taken);
+        }
+        if constexpr (kSched) {
+          // the pass's rate table (one fp32 evaluation per lane): the i-th push of the application order is applied
+          // at schedule step sched_step + i; published to apply_item by the barrier below
+          if (lane < __popc(p_taken)) s_lr[lane] = scheduled_lr(P, s_state[own].sched_step + lane);
+        }
+        if constexpr (kEma) {
+          // the pass's decay table: the step that ends at the i-th push leaves the item at sched_step + i + 1
+          // applied pushes, TF1's num_updates = global_step after the apply_gradients op the average follows
+          if (lane < __popc(p_taken)) s_ema[lane] = ema_decay(P, s_state[own].sched_step + lane + 1);
+        }
+      }
+      __syncthreads();
+      const long long c1 = stats_on ? clock64() : 0;
+      if (!s_any && stats_on) { ++st_idle_n; st_idle += c1 - c0; }
+      if (s_any) {
+        sweep_any = true;
+        const PsItemState st = s_state[own];
+        apply_item<kFam, kIeee, kSched, kEma>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
+                                              use_resident ? &resident : nullptr, s_lr, s_ema,
+                                              use_resident ? &resident_ema : nullptr);
+        __syncthreads();   // every thread's parameter stores precede warp 0's release operations below
+        const long long c2 = stats_on ? clock64() : 0;
+        if (stats_on) {
+          ++st_pass; st_push += s_npend; st_apply += c2 - c1; st_poll += c1 - c0;
+          st_max = max(st_max, static_cast<unsigned long long>(s_npend));
+        }
+        if (warp == 0) {
+          if (lane == 0) {
+            const uint32_t npush = __popc(p_taken);
+            const uint32_t rounds = (31u - __clz(p_taken)) / nw + 1u;   // lanes are round-major
+            const uint32_t nsteps = (P.apply_mode == APPLY_MERGED) ? rounds : npush;
+            PsItemState ns = st;
+            ns.t += nsteps;
+            for (uint32_t k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
+            // one schedule step per push, in both apply modes (also the num_updates of the averaging kernels)
+            if constexpr (kSched) ns.sched_step += npush;
+            s_state[own] = ns;
+            P.item_state[item] = ns;   // persisted for checkpoints / a relaunch (never read back in this loop)
+          }
+          if (p_take) {
+            const uint32_t slot = p_seq % P.nslots;
+            const uint32_t done = atomicAdd(&P.consumed[pw * P.nslots + slot], 1u) + 1u;
+            if (done == static_cast<uint32_t>(P.n_items)) {
+              // this worker's push `p_seq` is fully applied: one global step (reference DS:91,103)
+              P.consumed[pw * P.nslots + slot] = 0;
+              const uint32_t gs = atomicAdd(P.global_step, 1u) + 1u;
+              uint32_t* ib = P.inbox_table[pw];
+              if (ib != nullptr) {
+                red_max_relaxed_scoped_u32(ib + 1, gs, P.gpu_scope);
+                red_max_release_scoped_u32(ib, p_seq, P.gpu_scope);  // ack: the mailbox slot may be reused
+              }
+            }
+          }
+          if (pvalid && pk == 0 && p_cnt > 0) {
+            const uint32_t nx = p_seq + p_cnt;
+            s_next[own][pw] = nx;
+            P.next_seq[static_cast<size_t>(pw) * P.n_items + item] = nx;
+          }
+        }
+        if (stats_on) { __syncwarp(); st_book += clock64() - c2; }
+      }
+      __syncthreads();
+    }
+    // ---- exit protocol: host stop request, or every worker has left and all their pushes are applied ----
+    // (checked every 32nd poll round only: the check itself costs several system-scope loads, and the poll
+    //  loop's period is the PS's reaction latency)
+    if (tid == 0) {
+      uint32_t ex = 0;
+      // one-shot mode: everything that will ever be pushed was pushed before this launch (stream order), so a
+      // full sweep without work means the shard is up to date
+      if (P.oneshot && !sweep_any) ex = 1;
+      const bool check = !P.oneshot && (iter & 31u) == 0u;
+      if (check && *P.host_stop != 0u) ex = 1;
+      if (check && !ex) {
+        bool all_done = true;
+        for (int w = 0; w < P.n_workers && all_done; ++w) {
+          const uint32_t d = ld_acquire_sys_u32(P.worker_done + w);  // = last push seq + 1, 0 while active
+          if (d == 0) { all_done = false; break; }
+          if (d == kWorkerDead) continue;   // presumed dead: whatever it left half-pushed is dropped
+          for (int own = 0; own < n_own; ++own)
+            if (s_next[own][w] != d) { all_done = false; break; }
+        }
+        if (all_done) ex = 1;
+      }
+      s_exit = ex;
+    }
+    __syncthreads();
+    if (s_exit) break;
+    ++iter;
+  }
+  if (tid == 0) {
+    if (stats_on) {
+      unsigned long long* o = P.stats + static_cast<size_t>(blockIdx.x) * 8;
+      o[0] += st_pass; o[1] += st_push; o[2] += st_apply; o[3] += st_book; o[4] += st_idle_n; o[5] += st_idle;
+      o[6] = max(o[6], st_max); o[7] += st_poll;
+      P.stats[kPsStatsCtas * 8 + blockIdx.x] = sm_id();
+    }
+    atomicAdd(P.exit_counter, 1u);
+  }
 }
-// Every other family (Momentum, Adagrad, RMSProp, Adadelta, FTRL, ProximalAdagrad, ProximalGradientDescent):
-// ps_serve_kernel<kOpt, kIeee>.
-template <int kOpt, bool kIeee>
-__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_constant__ PsServeParams P) {
-  constexpr int kFam = kOpt;
-  constexpr bool kSched = false;
-  constexpr bool kEma = false;
-#include "ps_serve_body.cuh"
+
+using ServeKernel = void (*)(PsServeParams);
+template <int kFam, bool kIeee>
+ServeKernel serve_kernel_at(bool sched, bool ema) {
+  if (ema) return ps_serve_kernel<kFam, kIeee, true, true>;
+  if (sched) return ps_serve_kernel<kFam, kIeee, true, false>;
+  return ps_serve_kernel<kFam, kIeee, false, false>;
 }
-// Any family under a non-constant learning-rate schedule (P.lr_schedule != LR_CONSTANT): ps_serve_sched_kernel<kFam,
-// kIeee>. Separate instantiations keep the seven above, and with them every constant-rate run, exactly as measured.
-template <int kFamT, bool kIeee>
-__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_sched_kernel(const __grid_constant__ PsServeParams P) {
-  constexpr int kFam = kFamT;
-  constexpr bool kSched = true;
-  constexpr bool kEma = false;
-#include "ps_serve_body.cuh"
+template <int kFam>
+ServeKernel serve_kernel_of(bool ieee, bool sched, bool ema) {
+  // Momentum has no square root or divide: its one instantiation serves both math modes. ProximalGradientDescent has no
+  // square root: its one has the IEEE divide.
+  if constexpr (kFam == OPT_MOMENTUM) return serve_kernel_at<kFam, false>(sched, ema);
+  else if constexpr (kFam == OPT_PROXIMAL_SGD) return serve_kernel_at<kFam, true>(sched, ema);
+  else return ieee ? serve_kernel_at<kFam, true>(sched, ema) : serve_kernel_at<kFam, false>(sched, ema);
 }
-// Any family with moving averages of the parameters (P.ema != null), under any schedule: ps_serve_ema_kernel<kFam,
-// kIeee>. The rate table is compiled in as in the scheduled kernels (scheduled_lr is lr0 for LR_CONSTANT), so one
-// set serves a constant rate and every schedule; the fourteen above stay exactly as measured.
-template <int kFamT, bool kIeee>
-__global__ void __launch_bounds__(kPsThreads, 1) ps_serve_ema_kernel(const __grid_constant__ PsServeParams P) {
-  constexpr int kFam = kFamT;
-  constexpr bool kSched = true;
-  constexpr bool kEma = true;
-#include "ps_serve_body.cuh"
+// The serve-kernel instantiation for optimizer `opt` (OptimizerKind) in math mode `ieee`, with a non-constant schedule
+// (`sched`) and moving averages (`ema`, which takes the scheduled path whatever `sched` is); null for an unknown `opt`.
+ServeKernel serve_kernel(int opt, bool ieee, bool sched, bool ema) {
+  switch (opt) {
+    case OPT_SGD:
+    case OPT_ADAM: return serve_kernel_of<kFamAdamSgd>(ieee, sched, ema);
+    case OPT_MOMENTUM: return serve_kernel_of<OPT_MOMENTUM>(ieee, sched, ema);
+    case OPT_ADAGRAD: return serve_kernel_of<OPT_ADAGRAD>(ieee, sched, ema);
+    case OPT_RMSPROP: return serve_kernel_of<OPT_RMSPROP>(ieee, sched, ema);
+    case OPT_ADADELTA: return serve_kernel_of<OPT_ADADELTA>(ieee, sched, ema);
+    case OPT_FTRL: return serve_kernel_of<OPT_FTRL>(ieee, sched, ema);
+    case OPT_PROXIMAL_ADAGRAD: return serve_kernel_of<OPT_PROXIMAL_ADAGRAD>(ieee, sched, ema);
+    case OPT_PROXIMAL_SGD: return serve_kernel_of<OPT_PROXIMAL_SGD>(ieee, sched, ema);
+    default: return nullptr;
+  }
 }
 
 // `cluster` > 1: the grid is launched as clusters of that many CTAs. The kernel has no cluster-scope code; the
@@ -464,91 +629,9 @@ cudaError_t launch_ps_serve(const PsServeParams& p, int n_ctas, int cluster, cud
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = cluster > 1 ? 1 : 0;
-  if (p.ema != nullptr) {
-    switch (p.opt) {
-      case OPT_SGD:
-      case OPT_ADAM:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<kFamAdamSgd, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<kFamAdamSgd, false>, p);
-      case OPT_MOMENTUM:
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_MOMENTUM, false>, p);
-      case OPT_ADAGRAD:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADAGRAD, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADAGRAD, false>, p);
-      case OPT_RMSPROP:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_RMSPROP, false>, p);
-      case OPT_ADADELTA:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADADELTA, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_ADADELTA, false>, p);
-      case OPT_FTRL:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_FTRL, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_FTRL, false>, p);
-      case OPT_PROXIMAL_ADAGRAD:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
-      case OPT_PROXIMAL_SGD:
-        return cudaLaunchKernelEx(&cfg, ps_serve_ema_kernel<OPT_PROXIMAL_SGD, true>, p);
-      default:
-        return cudaErrorInvalidValue;
-    }
-  }
-  if (p.lr_schedule != LR_CONSTANT) {
-    switch (p.opt) {
-      case OPT_SGD:
-      case OPT_ADAM:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<kFamAdamSgd, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<kFamAdamSgd, false>, p);
-      case OPT_MOMENTUM:
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_MOMENTUM, false>, p);
-      case OPT_ADAGRAD:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADAGRAD, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADAGRAD, false>, p);
-      case OPT_RMSPROP:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_RMSPROP, false>, p);
-      case OPT_ADADELTA:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADADELTA, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_ADADELTA, false>, p);
-      case OPT_FTRL:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_FTRL, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_FTRL, false>, p);
-      case OPT_PROXIMAL_ADAGRAD:
-        if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
-      case OPT_PROXIMAL_SGD:
-        return cudaLaunchKernelEx(&cfg, ps_serve_sched_kernel<OPT_PROXIMAL_SGD, true>, p);
-      default:
-        return cudaErrorInvalidValue;
-    }
-  }
-  switch (p.opt) {
-    case OPT_SGD:
-    case OPT_ADAM:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<false>, p);
-    case OPT_MOMENTUM:   // no square root: one instantiation serves both math modes
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_MOMENTUM, false>, p);
-    case OPT_ADAGRAD:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADAGRAD, true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADAGRAD, false>, p);
-    case OPT_RMSPROP:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_RMSPROP, false>, p);
-    case OPT_ADADELTA:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADADELTA, true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_ADADELTA, false>, p);
-    case OPT_FTRL:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_FTRL, true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_FTRL, false>, p);
-    case OPT_PROXIMAL_ADAGRAD:
-      if (p.ieee_math) return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, true>, p);
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, false>, p);
-    case OPT_PROXIMAL_SGD:   // no square root: one instantiation (IEEE divide) serves both math modes
-      return cudaLaunchKernelEx(&cfg, ps_serve_kernel<OPT_PROXIMAL_SGD, true>, p);
-    default:
-      return cudaErrorInvalidValue;
-  }
+  const ServeKernel k = serve_kernel(p.opt, p.ieee_math != 0u, p.lr_schedule != LR_CONSTANT, p.ema != nullptr);
+  if (k == nullptr) return cudaErrorInvalidValue;
+  return cudaLaunchKernelEx(&cfg, k, p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -643,52 +726,16 @@ cudaError_t launch_worker_done(uint32_t* done_slot, const uint32_t* seq_ptr, cud
 namespace dm {
 // Force-load every kernel of this translation unit. With CUDA's lazy module loading the *first* launch of a
 // kernel may need a context-wide synchronisation; if that first launch happens while the persistent serve
-// kernel is resident (and the serve kernel is waiting for the new kernel's flags) the process deadlocks.
+// kernel is resident (and the serve kernel is waiting for the new kernel's flags) the process deadlocks. The serve
+// kernels are enumerated through serve_kernel, so every one that launch_ps_serve can pick is loaded here.
 cudaError_t preload_ps_kernels() {
   cudaFuncAttributes a;
   cudaError_t e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<kFamAdamSgd, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<kFamAdamSgd, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<kFamAdamSgd, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<kFamAdamSgd, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_MOMENTUM, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_RMSPROP, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_sched_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADADELTA, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_ADADELTA, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_FTRL, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_FTRL, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, false>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_ADAGRAD, true>)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, ps_serve_ema_kernel<OPT_PROXIMAL_SGD, true>)) != cudaSuccess) return e;
+  for (int opt = OPT_SGD; opt <= OPT_PROXIMAL_SGD; ++opt)
+    for (const bool ieee : {false, true})
+      for (const bool sched : {false, true})
+        for (const bool ema : {false, true})
+          if ((e = cudaFuncGetAttributes(&a, serve_kernel(opt, ieee, sched, ema))) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, dense_apply_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, shadow_refresh_kernel)) != cudaSuccess) return e;
   if ((e = cudaFuncGetAttributes(&a, wait_ack_kernel)) != cudaSuccess) return e;

@@ -66,7 +66,7 @@ def test_engine_flags_defaults_are_the_benchmarked_engine_and_lanes_1_is_the_ref
     assert (cfg.nslots, cfg.lanes, cfg.graph_steps) == (4, 4, 2)
 
 
-def test_adam_math_flag_selects_the_ieee_ps_kernel():
+def test_adam_math_flag_selects_the_ieee_serve_kernel_instantiation():
     import pytest
     from dist_mnist_b200 import _native as N
     from dist_mnist_b200.parallel.config import OptimizerConfig
@@ -78,12 +78,15 @@ def test_adam_math_flag_selects_the_ieee_ps_kernel():
     with pytest.raises(ValueError):
         OptimizerConfig("adam", 1e-4, math="exact")
     assert "ieee_math" in [f[0] for f in N.PsServeParams._fields_]
-    # both instantiations of the serve kernel are in the library
+    # both constant-rate Adam / SGD instantiations of the serve kernel (family -1, fast and IEEE) are in the library,
+    # among exactly 42: 14 (family, math) pairs, each at a constant rate, scheduled and averaging
+    import re
     import shutil
     import subprocess
     if shutil.which("cuobjdump"):
         syms = subprocess.run(["cuobjdump", "-elf", str(N.lib_path())], capture_output=True, text=True).stdout
-        assert "ps_serve_kernelILb0EE" in syms and "ps_serve_kernelILb1EE" in syms
+        assert "ps_serve_kernelILin1ELb0ELb0ELb0EE" in syms and "ps_serve_kernelILin1ELb1ELb0ELb0EE" in syms
+        assert len(set(re.findall(r"ps_serve_kernelI\w+?EEEv", syms))) == 42
 
 
 def test_package_is_runnable_as_a_module():
