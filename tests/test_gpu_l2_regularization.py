@@ -5,31 +5,9 @@ the unregularized one plus the fp64 L2 term; lock-step trajectories against fp32
 fused steps, 100 graph steps); bit-identical repeated runs; group graphs; and the fused lane cap beside the ps."""
 import pytest
 
+from bench_tools.fused_push_ref import pushed
+
 pytestmark = pytest.mark.gpu
-
-
-def _pushed(w, seq=1):
-    """The gradient this worker pushed with push `seq`, read out of its mailbox slot in the ps segments."""
-    import torch
-
-    ns = w.cfg.nslots
-    slot = seq % ns
-    out = {}
-    for name, vl in w.layout.by_name.items():
-        owners = list(dict.fromkeys((pc.ps, pc.offset) for pc in vl.pieces))
-        spans = {}
-        for k, off in owners:
-            base = (w.task_index * ns + slot) * w.ps_desc[k]["arena_elems"]
-            spans[(k, off)] = w._unpack(vl, w._copy_from_ps(k, "mailbox", base + off, vl.span, torch.float32))
-        if len(owners) == 1:
-            out[name] = spans[owners[0]]
-            continue
-        full = torch.empty(vl.rows, vl.cols)
-        for pc in vl.pieces:
-            if pc.c1 > pc.c0:
-                full[:, pc.c0:pc.c1] = spans[(pc.ps, pc.offset)][:, pc.c0:pc.c1]
-        out[name] = full
-    return out
 
 
 def _one_step(H, B, nps, sharding, l2, clip=None, model="book", engine="fused", dtype="fp32"):
@@ -56,7 +34,7 @@ def _one_step(H, B, nps, sharding, l2, clip=None, model="book", engine="fused", 
         assert w.engine == engine
         r = w.step(ds.images[:B], ds.labels[:B])
         w.wait_applied()
-        return r.loss, _pushed(w), params
+        return r.loss, pushed(w), params
 
 
 def _clip_ref(g, clip):
