@@ -51,6 +51,24 @@ unit roundoff), k the loss normalisation (1 / (B C) for the book loss, 1 / B for
 * correct count: exact over rows whose top two logits are further apart than 2 dz_b + EPS_F max|z_b|; each other row
   may go either way.
 
+Other activations (`--activation`, case builder and bound take `activation`; relu is the derivation above exactly)
+-----------------------------------------------------------------------------------------------------------------
+hv = f(pre) and dpre = dh * f'(hv), f' taken of the output as TF's *Grad ops take it (csrc/activation.cuh). With L_f
+the Lipschitz constant of f (1; selu sa = 1.7581; sigmoid 1/4) the kernel's hv errs by ey = L_f band + f's own
+rounding. CUDA 12.9's documented maximum errors are 2 ulp for expf and for tanhf and 0 for the IEEE divide, so f
+rounds by at most (2 ulp + 2 u) |y| for sigmoid and tanh, by 2^-22 K e^pre + u |y| on the negative branch of elu (K
+= 1) and selu (K = sa), and by u |y| for leaky_relu's and selu's products (their fp32 constants differ from the fp64
+ones by < u relative); RND_ACT = 2^-20 times (|y| + K e^pre [pre < 0]) covers each with a 4x margin (relu and relu6
+do not round). ey replaces band in dz and in the sm_w bound, |hv| replaces hv.
+f' as a function of y has slope S (0 for the piecewise constant relu, relu6 and leaky_relu; 1 for elu and selu on y <
+0 and for sigmoid's y (1 - y); 2 |y| for tanh's 1 - y y), so the kernel's f' errs by S ey + RND_ACT |f'|, and outside
+the ambiguity bands ddp = |f'| ddh + |dh| (S ey + RND_ACT |f'|). The ambiguity bands sit at the kinks of f', where
+the kernel may take either branch: 0 for relu, leaky_relu and selu (whose f' jumps from sa to s there), 0 and 6 for
+relu6; elu's f' is continuous at 0 and sigmoid and tanh have none. There ddp = jump |dh| + max|f'| ddh + |dh| (S ey +
+RND_ACT |f'|), with the jump of f' across the kink (relu: 1, giving the |dh| + ddh above). The builder moves biases so
+that every branch is taken: both signs for leaky_relu, elu and selu, pre above 6 for relu6, |pre| > 3 in saturated
+units for sigmoid and tanh (`_cover_activation`, asserted by `check_case`).
+
 The graph engine computes the same quantities with the same or tighter fp32 operations (IEEE division in the head, an
 fp32 dW GEMM on tf32 operands), so the same bound applies to it unchanged.
 
@@ -61,7 +79,9 @@ and every reported correct count lies in its range.
 
 `emulate` runs the kernel's arithmetic in fp32 on the CPU, with dpre converted to tf32 by truncation or by
 round-to-nearest; tests/test_fused_push_bound_cpu.py shows it inside the bound and each of a set of mutants (a dropped
-batch row, a zeroed k-chunk, ...) far outside it at every case whose coverage admits the mutant.
+batch row, a zeroed k-chunk, ...) far outside it at every case whose coverage admits the mutant, and
+tests/test_activations_cpu.py does the same for every activation with the activation's own mutants (f or f' not
+applied, f' of the pre-activation, relu6's f' without its upper kink).
 """
 from __future__ import annotations
 
@@ -83,6 +103,34 @@ U = 2.0 ** -24
 CLAMP = 1e-10            # the book loss's clip of p
 CHUNK = 32               # features per k-chunk of the fused kernel
 VARS = ("hid_w", "hid_b", "sm_w", "sm_b")
+RND_ACT = 2.0 ** -20     # relative rounding of f and f' (expf / tanhf 2 ulp + a few roundings, 4x margin)
+
+
+@dataclass(frozen=True)
+class ActBound:
+    """What the bound needs of an activation f: its Lipschitz constant, max |f'|, the jump of f' at its kinks (where
+    the kernel may take either branch), the slope of f' as a function of y (tanh: 2 |y|, `slope_y` True), whether f
+    and f' round at all, and the factor K of expf's absolute error term K e^x on the negative branch."""
+    lip: float
+    fmax: float
+    jump: float
+    kinks: Tuple[float, ...]
+    slope: float
+    slope_y: bool = False
+    rounds: bool = True
+    exp_k: float = 0.0
+
+
+ACT_BOUNDS = {
+    "relu": ActBound(1.0, 1.0, 1.0, (0.0,), 0.0, rounds=False),
+    "relu6": ActBound(1.0, 1.0, 1.0, (0.0, 6.0), 0.0, rounds=False),
+    "leaky_relu": ActBound(1.0, 1.0, 1.0 - mlp.LEAKY_RELU_ALPHA, (0.0,), 0.0),
+    "elu": ActBound(1.0, 1.0, 0.0, (), 1.0, exp_k=1.0),
+    "selu": ActBound(mlp.SELU_SCALE_ALPHA, mlp.SELU_SCALE_ALPHA, mlp.SELU_SCALE_ALPHA - mlp.SELU_SCALE, (0.0,), 1.0,
+                     exp_k=mlp.SELU_SCALE_ALPHA),
+    "sigmoid": ActBound(0.25, 0.25, 0.0, (), 1.0),
+    "tanh": ActBound(1.0, 1.0, 0.0, (), 2.0, slope_y=True),
+}
 
 
 @dataclass
@@ -105,8 +153,9 @@ class Case:
         return H, C, I, self.batch, self.spec.loss
 
 
-def spec_for(H: int, C: int, I: int, loss: str) -> mlp.MLPSpec:
-    return mlp.MLPSpec(name="book", in_features=I, hidden=(H,), num_classes=C, loss=loss, init="book")
+def spec_for(H: int, C: int, I: int, loss: str, activation: str = "relu") -> mlp.MLPSpec:
+    return mlp.MLPSpec(name="book", in_features=I, hidden=(H,), num_classes=C, loss=loss, init="book",
+                       activation=activation)
 
 
 def tf32_exact(t: torch.Tensor) -> torch.Tensor:
@@ -136,10 +185,12 @@ def _draw_batch(g: torch.Generator, protos: torch.Tensor, B: int) -> Tuple[torch
 
 
 def make_case(H: int, C: int, I: int, B: int, loss: str, seed: int, n_batches: int = 1, saturate: float = 0.0,
-              name: Optional[str] = None) -> Case:
+              name: Optional[str] = None, activation: str = "relu") -> Case:
     """A tf32-exact case at shape (H, C, I, B, loss), redrawn from `seed` until `check_case` passes (coverage, the
-    clamp margin). `saturate` scales W_last so that some rows' true-class p fall far below the clamp."""
-    spec = spec_for(H, C, I, loss)
+    clamp margin). `saturate` scales W_last so that some rows' true-class p fall far below the clamp. Under an
+    activation other than relu, biases are then moved so that every branch of it is taken (`_cover_activation`); relu
+    cases are drawn exactly as they were before activations existed."""
+    spec = spec_for(H, C, I, loss, activation)
     for attempt in range(64):
         sub = seed * 1000 + attempt
         g = torch.Generator().manual_seed(sub)
@@ -155,12 +206,41 @@ def make_case(H: int, C: int, I: int, B: int, loss: str, seed: int, n_batches: i
         # of every batch (small batches end up with every unit active, larger ones keep inactive pairs)
         top = torch.stack([(x.double() @ params["hid_w"].double().t()).amax(dim=0) for x, _ in batches]).amin(dim=0)
         params["hid_b"] = torch.maximum(params["hid_b"], (0.02 - top).float())
-        case = Case(name or f"H{H}-C{C}-I{I}-B{B}-{loss}" + ("-sat" if saturate else ""), spec, params, batches, sub,
+        if activation != "relu":
+            _cover_activation(activation, params, batches)
+        case = Case(name or f"H{H}-C{C}-I{I}-B{B}-{loss}" + ("-sat" if saturate else "") +
+                    ("" if activation == "relu" else f"-{activation}"), spec, params, batches, sub,
                     saturated=bool(saturate))
         if all(not check_case(case, x, y) for x, y in batches):
             assert exact_inputs(case) == [], exact_inputs(case)
             return case
     raise RuntimeError(f"no covered case at {(H, C, I, B, loss)} from seed {seed}")
+
+
+def _cover_activation(activation: str, params: Dict[str, torch.Tensor],
+                      batches: List[Tuple[torch.Tensor, torch.Tensor]]) -> None:
+    """Move hidden biases so that the batches reach every branch of `activation` (`check_case` asserts it): relu6's
+    upper kink (every third unit but the last tops out at 6.25 in some row; one unit alone is left below 6, where it
+    can show every other mutant), and saturated sigmoid / tanh units (every third unit
+    at least 3.5 in every row, the next one at most -3.5). The other units keep pre-activations of both signs, which
+    leaky_relu, elu and selu need."""
+    pre = [x.double() @ params["hid_w"].double().t() for x, _ in batches]
+    top = torch.stack([p.amax(dim=0) for p in pre]).amin(dim=0)
+    low = torch.stack([p.amin(dim=0) for p in pre]).amax(dim=0)
+    b = params["hid_b"].clone()
+    H, B = b.numel(), batches[0][0].shape[0]
+    if activation == "relu6" and H > 1:
+        up = torch.arange(0, H - 1, 3)   # the last unit stays below 6 (it shows a zeroed last hidden row)
+        b[up] = (6.25 - top[up]).float()
+    elif activation in ("sigmoid", "tanh"):
+        b[0::3] = (3.5 - low[0::3]).float()
+        b[1::3] = (-3.5 - top[1::3]).float()
+    elif activation in ("leaky_relu", "elu", "selu"):
+        if H > 1:
+            b[1::3] = (-0.5 - top[1::3]).float()                    # every row of these units negative
+        elif B > 1:
+            b[0] = (0.02 - top[0]).float()                          # one unit: its top row positive, the others not
+    params["hid_b"] = b
 
 
 def exact_inputs(case: Case) -> List[str]:
@@ -202,8 +282,9 @@ def shape_matrix() -> List[Tuple[str, Tuple[int, int, int, int, str], float]]:
     return out
 
 
-def case_for(shape: Tuple[int, int, int, int, str], saturate: float = 0.0, n_batches: int = 1, seed: int = 1) -> Case:
-    return make_case(*shape, seed=seed, n_batches=n_batches, saturate=saturate)
+def case_for(shape: Tuple[int, int, int, int, str], saturate: float = 0.0, n_batches: int = 1, seed: int = 1,
+             activation: str = "relu") -> Case:
+    return make_case(*shape, seed=seed, n_batches=n_batches, saturate=saturate, activation=activation)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -220,11 +301,13 @@ class Reference:
     # intermediates for coverage, mutants and localisation
     x: torch.Tensor = field(repr=False, default=None)
     pre: torch.Tensor = field(repr=False, default=None)
-    edge: torch.Tensor = field(repr=False, default=None)     # half-width of the ReLU's ambiguity band
+    edge: torch.Tensor = field(repr=False, default=None)     # half-width of the ambiguity band at f's kinks
     dh: torch.Tensor = field(repr=False, default=None)
     dpre: torch.Tensor = field(repr=False, default=None)
     dl: torch.Tensor = field(repr=False, default=None)
     p_true: torch.Tensor = field(repr=False, default=None)
+    active: torch.Tensor = field(repr=False, default=None)   # f' != 0, away from every kink
+    hv: torch.Tensor = field(repr=False, default=None)       # f(pre)
 
 
 def _k(spec: mlp.MLPSpec, B: int) -> float:
@@ -244,10 +327,19 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
     pre = x64 @ W.t() + b
     A = ax @ W.abs().t() + b.abs()
     band, edge = EPS_FWD * A, AMBIG * A
-    act, amb = pre > edge, pre.abs() <= edge
-    hv = pre.clamp_min(0.0)
+    ab = ACT_BOUNDS[spec.activation]
+    amb = torch.zeros_like(pre, dtype=torch.bool)
+    for kink in ab.kinks:
+        amb |= (pre - kink).abs() <= edge
+    hv = mlp.activate(spec.activation, pre)
+    fp = mlp.activation_grad(spec.activation, hv, torch.ones_like(hv))      # f'(pre), from y as the kernels do
+    act = ~amb & (fp != 0)
+    ahv = hv.abs()
+    ey = ab.lip * band                                                        # error of the kernel's hv
+    if ab.rounds:
+        ey = ey + RND_ACT * (ahv + ab.exp_k * torch.exp(pre.clamp(max=0.0)) * (pre < 0).to(d))
     z = logits
-    dzc = band @ aWl.t() + EPS_F * (hv @ aWl.t() + bl.abs())
+    dzc = ey @ aWl.t() + EPS_F * (ahv @ aWl.t() + bl.abs())
     dz = dzc.amax(dim=1, keepdim=True)
     p = torch.softmax(z, dim=1)
     zmax = z.amax(dim=1, keepdim=True)
@@ -263,13 +355,18 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
     else:
         dl = (p * y64.sum(dim=1, keepdim=True) - y64) * k
     dh = dl @ Wl
-    dpre = dh * (pre > 0).to(d)
+    dpre = mlp.activation_grad(spec.activation, hv, dh)
     ddh = E @ aWl + EPS_F * (dl.abs() @ aWl)
-    ddp = act.to(d) * ddh + amb.to(d) * (dh.abs() + ddh)
+    # f' of the kernel's y: off by slope * ey (tanh: 2 |y| ey), plus its own rounding
+    dfp = (ab.slope * ahv if ab.slope_y else torch.full_like(hv, ab.slope)) * ey
+    if ab.rounds:
+        dfp = dfp + RND_ACT * fp.abs()
+    ddp = ((~amb).to(d) * (fp.abs() * ddh + dh.abs() * dfp) +
+           amb.to(d) * (ab.jump * dh.abs() + ab.fmax * ddh + dh.abs() * dfp))
     bounds = {
         "hid_w": (TF32 * dpre.abs() + (1 + TF32) * ddp + EPS_F * dpre.abs()).t() @ ax,
         "hid_b": (ddp + EPS_F * dpre.abs()).sum(dim=0),
-        "sm_w": E.t() @ hv + dl.abs().t() @ band + EPS_F * (dl.abs().t() @ hv),
+        "sm_w": E.t() @ ahv + dl.abs().t() @ ey + EPS_F * (dl.abs().t() @ ahv),
         "sm_b": (E + EPS_F * dl.abs()).sum(dim=0),
     }
     esum = torch.exp(z - zmax).sum(dim=1)
@@ -288,7 +385,7 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
     right = z.argmax(dim=1) == y64.argmax(dim=1)
     lo = int((right & ~unsure).sum())
     return Reference({n: grads[n] for n in VARS}, bounds, float(loss), loss_bound, lo, lo + int(unsure.sum()),
-                     x64, pre, edge, dh, dpre, dl, p_true)
+                     x64, pre, edge, dh, dpre, dl, p_true, act, hv)
 
 
 def check_case(case: Case, x: torch.Tensor, y: torch.Tensor) -> List[str]:
@@ -296,11 +393,23 @@ def check_case(case: Case, x: torch.Tensor, y: torch.Tensor) -> List[str]:
     (beyond the ReLU's ambiguity band) in some row, every batch row has a nonzero x and a nonzero dlogits row (so it
     moves sm_b and the loss at least) unless it is a clamped row of the saturated case or there is one class, every
     k-chunk has a nonzero x under an active unit, and the book
-    loss keeps every true-class p outside [1e-10 / 2, 2e-10]; the saturated case has clamped and unclamped rows."""
+    loss keeps every true-class p outside [1e-10 / 2, 2e-10]; the saturated case has clamped and unclamped rows.
+    "Active" is f' != 0 outside the ambiguity bands (the ReLU: pre above the band). Each branch of the activation is
+    taken (beyond the band) where a single pre-activation does not rule it out: both signs for leaky_relu, elu and
+    selu, pre above 6 for relu6 (with H > 1), saturated |pre| > 3 for sigmoid and tanh."""
     spec = case.spec
     r = reference(spec, case.params, x, y)
-    act = r.pre > r.edge
+    act = r.pre > r.edge if spec.activation == "relu6" else r.active   # (units above 6 are not dead)
     bad = []
+    a = spec.activation
+    several = r.pre.numel() > 1
+    if a in ("leaky_relu", "elu", "selu") and several and not (bool((r.pre > r.edge).any()) and
+                                                               bool((r.pre < -r.edge).any())):
+        bad.append(f"{a}: pre-activations of one sign only")
+    if a == "relu6" and spec.hidden[0] > 1 and not bool((r.pre > 6 + r.edge).any()):
+        bad.append("relu6: no pre-activation above 6")
+    if a in ("sigmoid", "tanh") and not bool((r.pre.abs() > 3).any()):
+        bad.append(f"{a}: no saturated pre-activation")
     if not bool(act.any(dim=0).all()):
         bad.append(f"hidden units never active: {(~act.any(dim=0)).nonzero().flatten().tolist()}")
     live = torch.ones(x.shape[0], dtype=torch.bool) if spec.loss == "xent" else r.p_true >= CLAMP
@@ -335,8 +444,8 @@ class Step:
 
 def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor, y: torch.Tensor,
             tf32: str = "trunc", mutant: Optional[str] = None, arg: int = 0) -> Step:
-    """One fused step in fp32 with dpre converted to tf32 (`tf32` = "trunc" | "rne"). `mutant` (with `arg`) is one
-    of MUTANTS: a plausible kernel bug, applied where the kernel would make it."""
+    """One fused step in fp32 with dpre converted to tf32 (`tf32` = "trunc" | "rne"), under spec.activation. `mutant`
+    (with `arg`) is one of MUTANTS: a plausible kernel bug, applied where the kernel would make it."""
     f = torch.float32
     W, b, Wl, bl = (params[n].to(f) for n in VARS)
     x, y = x.to(f), y.to(f)
@@ -348,7 +457,8 @@ def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
         live[32 * arg:32 * (arg + 1)] = 0.0
     nb = 32 * ((B + 31) // 32) if mutant == "loss_32T" else B
     pre = x @ W.t() + b
-    hv = torch.relu(pre)
+    a = spec.activation
+    hv = pre if mutant == "act_forward_missing" else mlp.activate(a, pre)
     z = hv @ Wl.t() + bl
     p = torch.softmax(z, dim=1)
     if spec.loss == "book":
@@ -361,10 +471,19 @@ def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
         dl = k * (p * y.sum(dim=1, keepdim=True) - y)
         lc = -k * y * torch.log_softmax(z, dim=1)
     dl = dl * live
-    mask = (hv > 0).to(f)
-    if mutant == "relu_missing":
-        mask[:, arg] = 1.0
-    dpre = (dl @ Wl) * mask
+    if a == "relu":
+        mask = (hv > 0).to(f)
+        if mutant == "relu_missing":
+            mask[:, arg] = 1.0
+        dpre = (dl @ Wl) * mask
+    elif mutant == "act_grad_missing":
+        dpre = dl @ Wl
+    elif mutant == "act_grad_from_pre":
+        dpre = mlp.activation_grad(a, pre, dl @ Wl)
+    elif mutant == "relu6_upper_kink_missing":
+        dpre = mlp.activation_grad("relu", hv, dl @ Wl)
+    else:
+        dpre = mlp.activation_grad(a, hv, dl @ Wl)
     dW = to_tf32(dpre, tf32).t() @ x
     if mutant == "zero_chunk":
         dW[:, arg * CHUNK:(arg + 1) * CHUNK] = 0.0
@@ -381,14 +500,19 @@ def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
 
 
 MUTANTS = ("drop_row", "drop_tile", "zero_chunk", "zero_hidden_row", "relu_missing", "loss_32T", "sm_w_transposed",
-           "sm_w_class_shift")
+           "sm_w_class_shift", "act_forward_missing", "act_grad_missing", "act_grad_from_pre", "relu6_upper_kink_missing")
+ACT_MUTANTS = MUTANTS[-4:]   # the activation's own: f not applied, f' not applied, f' of pre, relu6's f' without its
+                             # upper kink
 
 
 def mutant_instances(case: Case, ref: Reference) -> List[Tuple[str, int]]:
     """(mutant, arg) pairs that this batch's coverage admits, i.e. that change the step beyond rounding: every
     mutant needs >= 2 classes (one class pushes exact zeros); a dropped tile and the last row of tile 0 need > 32
     rows; the 32 T normalisation needs B % 32 != 0; a transposed sm_w needs H >= 2; the missing ReLU mask needs an
-    inactive (b, j) under a nonzero dh and x (it takes the unit with the most such weight)."""
+    inactive (b, j) under a nonzero dh and x (it takes the unit with the most such weight). Under another activation
+    than relu, the missing mask is replaced by ACT_MUTANTS, each admitted where it changes the step: f not applied
+    where f(pre) differs from pre by more than 0.02, f' not applied or taken of pre where that changes some |dpre| |x|
+    by 5 % of the largest, relu6's upper kink likewise where a pre lies above 6."""
     H, C, I, B, _ = case.shape
     if C < 2:
         return []
@@ -400,10 +524,28 @@ def mutant_instances(case: Case, ref: Reference) -> List[Tuple[str, int]]:
         out.append(("loss_32T", 0))
     if H >= 2:
         out.append(("sm_w_transposed", 0))
-    off = (ref.pre < -ref.edge).to(torch.float64)
-    weight = ((off * ref.dh.abs()) * ref.x.abs().sum(dim=1, keepdim=True)).sum(dim=0)
-    if float(weight.max()) > 0:
-        out.append(("relu_missing", int(weight.argmax())))
+    a = case.spec.activation
+    rows = ref.x.abs().sum(dim=1, keepdim=True)
+
+    def moves(change: torch.Tensor) -> bool:   # f' changed by `change`, by 5 % of the largest |dpre| |x| somewhere
+        return float(((change.abs() * ref.dh.abs()) * rows).max()) > 0.05 * float((ref.dpre.abs() * rows).max())
+
+    if a == "relu":
+        off = (ref.pre < -ref.edge).to(torch.float64)
+        weight = ((off * ref.dh.abs()) * rows).sum(dim=0)
+        if float(weight.max()) > 0:
+            out.append(("relu_missing", int(weight.argmax())))
+        return out
+    one = torch.ones_like(ref.hv)
+    fp = mlp.activation_grad(a, ref.hv, one)
+    if float((ref.hv - ref.pre).abs().max()) > 0.02:
+        out.append(("act_forward_missing", 0))
+    if moves(fp - 1):
+        out.append(("act_grad_missing", 0))
+    if moves(mlp.activation_grad(a, ref.pre, one) - fp):
+        out.append(("act_grad_from_pre", 0))
+    if a == "relu6" and moves((ref.pre > 6 + ref.edge).to(torch.float64)):
+        out.append(("relu6_upper_kink_missing", 0))
     return out
 
 

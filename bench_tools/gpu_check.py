@@ -78,8 +78,11 @@ def random_shapes(n: int, seed: int, max_b: int = 256):
     return out
 
 
-def check_gemm_fwd() -> bool:
+def check_gemm_fwd(activation: str = "relu") -> bool:
+    """The forward epilogue without an activation and with `activation` (an mlp.ACTIVATIONS name): fp32 and bf16 out,
+    padding rows zero."""
     from dist_mnist_b200 import _native as N
+    from dist_mnist_b200.models import mlp
     from dist_mnist_b200.ops import gemm
     ok = True
     dev = "cuda"
@@ -94,23 +97,24 @@ def check_gemm_fwd() -> bool:
             wd, xd = padded(w, dt), padded(x, dt)
             outp = torch.zeros(B_pad, gemm.padded_ld(O), device=dev, dtype=tdtype(dt))
             out = outp[:, :O]
-            for relu in (False, True):
+            for act in (None, activation):
                 outp.zero_()
                 plan = gemm.forward_plan(w_ptr=wd.data_ptr(), x_ptr=xd.data_ptr(), out_ptr=outp.data_ptr(),
-                                         bias_ptr=bias.data_ptr(), O=O, I=I, B=B, B_pad=B_pad, dtype=dt, relu=relu,
+                                         bias_ptr=bias.data_ptr(), O=O, I=I, B=B, B_pad=B_pad, dtype=dt,
+                                         act=N.ACT_NONE if act is None else mlp.activation_code(act),
                                          ldw=wd.shape[1], ldx=xd.shape[1], ldo=outp.shape[1])
                 plan.launch()
                 torch.cuda.synchronize()
                 ref = round_operand(x[:B], dt) @ round_operand(w, dt).t() + bias
-                if relu:
-                    ref = torch.relu(ref)
+                if act is not None:
+                    ref = mlp.activate(act, ref)
                 e = rel_err(out[:B], ref)
                 ref_x = exact(x[:B], w.t()) + bias          # un-rounded operands
-                if relu:
-                    ref_x = torch.relu(ref_x)
+                if act is not None:
+                    ref_x = mlp.activate(act, ref_x)
                 ex = rel_err(out[:B], ref_x)
-                pad_zero = bool((out[B:] == 0).all())
-                ok &= report(f"fwd dt={dt} O={O} I={I} B={B} relu={relu}", e < tol and ex < TOL_EXACT[dt] and pad_zero,
+                pad_zero = bool((outp[B:] == 0).all() and (outp[:, O:] == 0).all())
+                ok &= report(f"fwd dt={dt} O={O} I={I} B={B} act={act}", e < tol and ex < TOL_EXACT[dt] and pad_zero,
                              f"rel_err={e:.2e} vs_unrounded_fp32={ex:.2e} pad_zero={pad_zero} stages={plan.params.stages}")
     return ok
 
@@ -155,8 +159,16 @@ def check_gemm_dw() -> bool:
     return ok
 
 
-def check_gemm_dx() -> bool:
+def _act_scale(activation: str) -> float:
+    """Spread of the pre-activations the dX and head checks draw: wide enough for saturated sigmoid / tanh units and
+    relu6's upper kink (ReLU keeps its standard normal inputs)."""
+    return 1.0 if activation == "relu" else 4.0
+
+
+def check_gemm_dx(activation: str = "relu") -> bool:
+    """The dX epilogue: dx = (dy . W) * f'(h) for `activation` f, with h = f(random), and its bias-gradient sums."""
     from dist_mnist_b200 import _native as N
+    from dist_mnist_b200.models import mlp
     from dist_mnist_b200.ops import gemm
     ok = True
     dev = "cuda"
@@ -168,25 +180,29 @@ def check_gemm_dx() -> bool:
             dy = torch.zeros(B_pad, O, device=dev)
             dy[:B] = torch.randn(B, O, device=dev) * 0.1
             h = torch.zeros(B_pad, I, device=dev)
-            h[:B] = torch.relu(torch.randn(B, I, device=dev))
+            h[:B] = mlp.activate(activation, _act_scale(activation) * torch.randn(B, I, device=dev))
             wd, dyd, hd = (padded(t, dt) for t in (w, dy, h))
             outp = torch.zeros(B_pad, gemm.padded_ld(I), device=dev, dtype=tdtype(dt))
             out = outp[:, :I]
             gb = torch.zeros(I + 32, device=dev)
             plan = gemm.dx_plan(w_ptr=wd.data_ptr(), dy_ptr=dyd.data_ptr(), out_ptr=outp.data_ptr(),
                                 mask_ptr=hd.data_ptr(), O=O, I=I, B=B, B_pad=B_pad, dtype=dt,
-                                ldw=wd.shape[1], lddy=dyd.shape[1], ldo=outp.shape[1],
+                                act=mlp.activation_code(activation), ldw=wd.shape[1], lddy=dyd.shape[1], ldo=outp.shape[1],
                                 colsum=gemm.local_push(gb.data_ptr()), colsum_offset=32)
             plan.launch()
             torch.cuda.synchronize()
-            ref = (round_operand(dy[:B], dt) @ round_operand(w, dt)) * (h[:B] > 0)
+            ref = mlp.activation_grad(activation, round_operand(h[:B], dt),
+                                      round_operand(dy[:B], dt) @ round_operand(w, dt))
             e = rel_err(out[:B], ref)
             eb = rel_err(gb[32:], ref.sum(dim=0))
-            ok &= report(f"dx dt={dt} O={O} I={I} B={B}", e < tol and eb < tol, f"rel_err={e:.2e} bias_grad_err={eb:.2e}")
+            pad_zero = bool((outp[B:] == 0).all())
+            ok &= report(f"dx dt={dt} O={O} I={I} B={B} act={activation}", e < tol and eb < tol and pad_zero,
+                         f"rel_err={e:.2e} bias_grad_err={eb:.2e} pad_zero={pad_zero}")
     return ok
 
 
-def check_head() -> bool:
+def check_head(activation: str = "relu") -> bool:
+    """The head kernel on h = f(random) of `activation` f: loss, correct count, small gradients and dpre = dh * f'(h)."""
     from dist_mnist_b200 import _native as N
     from dist_mnist_b200.models import mlp
     from dist_mnist_b200.ops import gemm, head
@@ -200,7 +216,7 @@ def check_head() -> bool:
                 torch.manual_seed(H + B)
                 adt = torch.bfloat16 if act_bf16 else torch.float32
                 h = torch.zeros(B_pad, H, device=dev)
-                h[:B] = torch.relu(torch.randn(B, H, device=dev))
+                h[:B] = mlp.activate(activation, _act_scale(activation) * torch.randn(B, H, device=dev))
                 hq = h.to(adt)
                 w = (torch.randn(Cn, H, device=dev) / H ** 0.5).contiguous()
                 b = torch.randn(Cn, device=dev) * 0.1
@@ -214,7 +230,7 @@ def check_head() -> bool:
                 plan = head.head_plan(h_ptr=hq.data_ptr(), labels_ptr=labels.data_ptr(), w_last_ptr=w.data_ptr(),
                                       b_last_ptr=b.data_ptr(), dpre_ptr=dpre.data_ptr(), result_ptr=res.data_ptr(),
                                       B=B, B_pad=B_pad, H=H, num_classes=Cn, loss_kind=loss_kind, act_bf16=act_bf16,
-                                      push=gemm.local_push(g.data_ptr()), off_w_last=off_w, off_b_last=off_b,
+                                      act=mlp.activation_code(activation), push=gemm.local_push(g.data_ptr()), off_w_last=off_w, off_b_last=off_b,
                                       off_b_hidden=off_bh)
                 plan.launch()
                 torch.cuda.synchronize()
@@ -226,7 +242,7 @@ def check_head() -> bool:
                 spec = mlp.MLPSpec(loss=loss_name)
                 loss = mlp.loss_from_logits(spec, logits, labels[:B])
                 gh, gw, gb_ = torch.autograd.grad(loss, [hf, wr, br])
-                dpre_ref = gh * (hf.detach() > 0)
+                dpre_ref = mlp.activation_grad(activation, hf.detach(), gh)
                 got_loss = res[:1].view(torch.float32).item()
                 got_correct = int(res[2].item())
                 e_loss = abs(got_loss - loss.item()) / (abs(loss.item()) + 1e-12)
@@ -239,7 +255,7 @@ def check_head() -> bool:
                 tol = 2e-2 if act_bf16 else 1e-4
                 good = (e_loss < 1e-4 and e_w < 1e-4 and e_b < 1e-4 and e_bh < tol and e_dp < tol and pad_ok
                         and got_correct == corr_ref)
-                ok &= report(f"head bf16={act_bf16} loss={loss_name} H={H} B={B}", good,
+                ok &= report(f"head bf16={act_bf16} loss={loss_name} H={H} B={B} act={activation}", good,
                              f"loss {got_loss:.6f}/{loss.item():.6f} e_w={e_w:.1e} e_b={e_b:.1e} e_bh={e_bh:.1e} "
                              f"e_dpre={e_dp:.1e} pad_ok={pad_ok} correct {got_correct}/{corr_ref}")
     return ok

@@ -90,7 +90,7 @@ def main() -> int:
         fin, fout = sizes[l]
         plans.append(gemm.forward_plan(w_ptr=wptr(wl), x_ptr=x.data_ptr() if l == 0 else act[l].data_ptr(),
                                        out_ptr=act[l + 1].data_ptr(), bias_ptr=params.data_ptr() + bl.offset * 4,
-                                       O=fout, I=fin, B=B, B_pad=B_pad, dtype=dt, relu=True, ldw=wl.ld,
+                                       O=fout, I=fin, B=B, B_pad=B_pad, dtype=dt, act=N.ACT_RELU, ldw=wl.ld,
                                        ldx=ld_in if l == 0 else act[l].shape[1], ldo=act[l + 1].shape[1],
                                        bump_seq_ptr=seq.data_ptr() if l == 0 else 0, splits=args.fwd_splits,
                                        name=f"fwd{l}"))
@@ -112,7 +112,7 @@ def main() -> int:
         if l > 0:   # dX before dW of the same layer (see Worker._build_cuda)
             pb = lay.by_name[names[l - 1][1]]
             plans.append(gemm.dx_plan(w_ptr=wptr(wl), dy_ptr=dact[l + 1].data_ptr(), out_ptr=dact[l].data_ptr(),
-                                      mask_ptr=act[l].data_ptr(), O=fout, I=fin, B=B, B_pad=B_pad, dtype=dt,
+                                      mask_ptr=act[l].data_ptr(), O=fout, I=fin, B=B, B_pad=B_pad, dtype=dt, act=N.ACT_RELU,
                                       ldw=wl.ld, lddy=dact[l + 1].shape[1], ldo=dact[l].shape[1], colsum=push,
                                       colsum_offset=pb.offset, colsum_item_base=pb.item_base, name=f"dx{l}"))
         plans.append(gemm.dw_plan(dy_ptr=dact[l + 1].data_ptr(), x_ptr=x.data_ptr() if l == 0 else act[l].data_ptr(),

@@ -30,6 +30,7 @@ DT_F32, DT_BF16 = 0, 1
 LR_CONSTANT, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_NATURAL_EXP, LR_POLYNOMIAL, LR_COSINE, LR_PIECEWISE = range(7)
 MAX_LR_BOUNDARIES = 8   # protocol.h kMaxLrBoundaries
 CLIP_OFF, CLIP_GLOBAL_NORM, CLIP_NORM, CLIP_VALUE = range(4)   # protocol.h GradClipKind
+ACT_NONE, ACT_RELU, ACT_RELU6, ACT_LEAKY_RELU, ACT_ELU, ACT_SELU, ACT_SIGMOID, ACT_TANH = range(8)   # protocol.h ActivationKind
 
 
 class PushTarget(C.Structure):
@@ -51,7 +52,7 @@ class GemmParams(C.Structure):
     _fields_ = [
         ("M", C.c_int), ("N", C.c_int), ("K", C.c_int),
         ("bn", C.c_int), ("stages", C.c_int), ("kc_per_split", C.c_int),
-        ("epi", C.c_int), ("out_bf16", C.c_int), ("relu", C.c_int),
+        ("epi", C.c_int), ("out_bf16", C.c_int), ("act", C.c_int),
         ("ldo", C.c_int), ("ldmask", C.c_int), ("mask_bf16", C.c_int),
         ("out", C.c_void_p), ("bias", C.c_void_p), ("mask", C.c_void_p),
         ("colsum", PushTarget),
@@ -87,6 +88,7 @@ class HeadParams(C.Structure):
         ("seq_ptr", C.c_void_p), ("inbox", C.c_void_p), ("ps_global_step", C.c_void_p),
         ("nslots", C.c_uint32), ("n_inbox", C.c_uint32),
         ("debug_ts", C.c_void_p),
+        ("act", C.c_int), ("act_pad_", C.c_int),
     ]
 
 
@@ -162,6 +164,7 @@ class FusedParams(C.Structure):
         ("clear_stop", C.c_uint32), ("wait_acks", C.c_uint32),
         ("clip_kind", C.c_int), ("clip_norm", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
         ("l2_scale", C.c_float), ("l2_biases", C.c_uint32),
+        ("act", C.c_int), ("act_pad_", C.c_uint32),
     ]
 
 
@@ -303,6 +306,7 @@ def _declare(l: C.CDLL) -> None:
         "dm_fused_max_lanes": (i, [i, i, C.POINTER(i)]),
         "dm_fused_max_lanes_clip": (i, [i, i, C.POINTER(i)]),
         "dm_fused_max_lanes_l2": (i, [i, i, i, C.POINTER(i)]),
+        "dm_fused_max_lanes_for": (i, [i, i, i, i, i, C.POINTER(i)]),
         "dm_launch_grad_clip": (i, [C.c_void_p, i, C.c_void_p]),
         "dm_fused_smem_bytes": (i, [i]),
         "dm_nvls_probe": (i, [i, sz, i, C.c_char_p, sz]),

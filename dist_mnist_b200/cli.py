@@ -227,6 +227,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--l2_variables", choices=list(L2_VARIABLES), default=None,
                    help="weights (default): every layer's weight matrix; all: the weights and the biases")
     p.add_argument("--model", choices=["book", "zhihu", "wide"], default="book")
+    p.add_argument("--activation", choices=list(mlp.ACTIVATIONS), default="relu",
+                   help="of every hidden layer (never the logits): TF1's tf.nn.relu, relu6, leaky_relu (alpha 0.2), "
+                        "elu, selu, sigmoid or tanh; worker-side only (a ps task ignores it, checkpoints do not store it)")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")
     p.add_argument("--push_mode", choices=["mailbox", "atomic"], default="mailbox")
@@ -300,7 +303,8 @@ def run(args: argparse.Namespace) -> int:
         raise ValueError(f"unknown job name {args.job_name!r} (expected 'ps' or 'worker')")
     cluster.task_endpoint(args.job_name, args.task_index)
     backend = resolve_backend(args.backend)
-    spec = mlp.get_model(args.model, args.hidden_units)
+    # the activation is the workers' alone: the ps stores and applies variables whatever computed their gradients
+    spec = mlp.get_model(args.model, args.hidden_units, args.activation if args.job_name == "worker" else "relu")
     opt = optimizer_config_from_args(args)
     cfg = engine_config_from_args(args, backend)
     cfg.validate(opt)

@@ -291,7 +291,14 @@ int dm_fused_max_lanes_clip(int dev, int batch, int* out) {
 // the same for the L2-regularizing instantiations, with (clip != 0) or without gradient clipping
 int dm_fused_max_lanes_l2(int dev, int batch, int clip, int* out) {
   DM_CUDA(cudaSetDevice(dev));
-  DM_CUDA(dm::fused_max_lanes_for(batch, clip != 0, true, out));
+  DM_CUDA(dm::fused_max_lanes_for(batch, clip != 0, true, dm::ACT_RELU, out));
+  return 0;
+}
+// the instantiation a fused step runs: with (clip != 0) or without gradient clipping, with (l2 != 0) or without L2
+// regularization, under activation `act` (ActivationKind)
+int dm_fused_max_lanes_for(int dev, int batch, int clip, int l2, int act, int* out) {
+  DM_CUDA(cudaSetDevice(dev));
+  DM_CUDA(dm::fused_max_lanes_for(batch, clip != 0, l2 != 0, act, out));
   return 0;
 }
 int dm_fused_smem_bytes(int batch) { return static_cast<int>(dm::fused_smem_bytes(batch)); }

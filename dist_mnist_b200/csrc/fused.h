@@ -22,6 +22,7 @@ size_t fused_smem_bytes(int B);
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream);
 cudaError_t fused_max_lanes(int B, int* out);
 cudaError_t fused_max_lanes_clip(int B, int* out);   // the same for the gradient-clipping instantiations
-cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int* out);   // ... with or without clip / L2
+// ... with or without clip / L2, under activation `act` (ActivationKind)
+cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int act, int* out);
 
 }  // namespace dm

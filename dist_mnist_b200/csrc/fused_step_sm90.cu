@@ -45,6 +45,7 @@
 // SURVEY K1-K6, K12, X3-X5 for the flagship model; deeper / wider / bf16 models use the per-layer kernels
 // (gemm_sm90.cu, head_sm90.cu) chained in a CUDA graph.
 #include "common.cuh"
+#include "activation.cuh"
 #include "fused.h"
 #include "grad_clip.cuh"
 
@@ -197,7 +198,10 @@ __device__ __forceinline__ void fs_wait_acks(const FusedParams& p, uint32_t need
 // handed the staging tile over (named barrier 2) instead of after its barrier #1. Every CTA sums w*w over what it
 // owns (its W k-slice, W_last / b of its 16 hidden units, b_last on CTA 0) into one partial on CTA 0, whose publisher
 // adds the 8 partials in a fixed order and reports loss + S * sum / 2.
-template <int kMaxTiles, bool kClip, bool kL2>
+// kAct: the hidden layer's activation is FusedParams::act (activation.cuh) instead of the ReLU: f where the hidden
+// values hv are formed, f'(hv) where dpre is. Units >= H stay 0; padding rows (>= B) hold f(bias), which nothing
+// reads: their dlogits are 0, so they add 0 to dpre and to every sum, and the loss and correct count mask them.
+template <int kMaxTiles, bool kClip, bool kL2, bool kAct>
 __global__ void __launch_bounds__(kFsThreads, 1)
 fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant__ FusedParams p) {
   constexpr bool kMulti = kMaxTiles > 1;
@@ -651,10 +655,17 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             const float4 t = *reinterpret_cast<const float4*>(red + (s * 128 + et) * 4);
             acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
           }
-          hv[0] = unit_ok ? fmaxf(acc.x + bias, 0.f) : 0.f;
-          hv[1] = unit_ok ? fmaxf(acc.y + bias, 0.f) : 0.f;
-          hv[2] = unit_ok ? fmaxf(acc.z + bias, 0.f) : 0.f;
-          hv[3] = unit_ok ? fmaxf(acc.w + bias, 0.f) : 0.f;
+          if constexpr (kAct) {
+            hv[0] = unit_ok ? act_forward(p.act, acc.x + bias) : 0.f;
+            hv[1] = unit_ok ? act_forward(p.act, acc.y + bias) : 0.f;
+            hv[2] = unit_ok ? act_forward(p.act, acc.z + bias) : 0.f;
+            hv[3] = unit_ok ? act_forward(p.act, acc.w + bias) : 0.f;
+          } else {
+            hv[0] = unit_ok ? fmaxf(acc.x + bias, 0.f) : 0.f;
+            hv[1] = unit_ok ? fmaxf(acc.y + bias, 0.f) : 0.f;
+            hv[2] = unit_ok ? fmaxf(acc.z + bias, 0.f) : 0.f;
+            hv[3] = unit_ok ? fmaxf(acc.w + bias, 0.f) : 0.f;
+          }
         }
         // ---- head on my 4 batch rows ----
 #pragma unroll
@@ -742,7 +753,8 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             if (4 * c4 + 2 < kFsPart - 1) dw[4 * c4 + 2] = fmaf(d.z, hv[i], dw[4 * c4 + 2]);
             if (4 * c4 + 3 < kFsPart - 1) dw[4 * c4 + 3] = fmaf(d.w, hv[i], dw[4 * c4 + 3]);
           }
-          dp[i] = hv[i] > 0.f ? dh : 0.f;       // rows >= B carry dlogits == 0 -> dp == 0
+          if constexpr (kAct) dp[i] = act_backward(p.act, hv[i], dh);   // (finite f': 0 for rows >= B as well)
+          else dp[i] = hv[i] > 0.f ? dh : 0.f;       // rows >= B carry dlogits == 0 -> dp == 0
           dbh += dp[i];
         }
         dw[kFsPart - 1] = dbh;
@@ -1050,27 +1062,33 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-template <int kMaxTiles, bool kClip, bool kL2>
+template <int kMaxTiles, bool kClip, bool kL2, bool kAct>
 static cudaError_t prepare_fused_instance() {
-  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip, kL2>,
+  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip, kL2, kAct>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(fs_smem_bytes<kMaxTiles>()));
   if (e != cudaSuccess) return e;
   cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip, kL2>);   // force-load (see preload_ps_kernels)
+  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip, kL2, kAct>);   // force-load (see preload_ps_kernels)
 }
 
-template <bool kClip, bool kL2>
+template <bool kClip, bool kL2, bool kAct>
 static cudaError_t prepare_fused_pair() {
-  cudaError_t e = prepare_fused_instance<1, kClip, kL2>();
-  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, kClip, kL2>();
+  cudaError_t e = prepare_fused_instance<1, kClip, kL2, kAct>();
+  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, kClip, kL2, kAct>();
+}
+
+template <bool kAct>
+static cudaError_t prepare_fused_act() {
+  cudaError_t e = prepare_fused_pair<false, false, kAct>();
+  if (e == cudaSuccess) e = prepare_fused_pair<true, false, kAct>();
+  if (e == cudaSuccess) e = prepare_fused_pair<false, true, kAct>();
+  return e != cudaSuccess ? e : prepare_fused_pair<true, true, kAct>();
 }
 
 cudaError_t prepare_fused_kernel() {
-  cudaError_t e = prepare_fused_pair<false, false>();
-  if (e == cudaSuccess) e = prepare_fused_pair<true, false>();
-  if (e == cudaSuccess) e = prepare_fused_pair<false, true>();
-  return e != cudaSuccess ? e : prepare_fused_pair<true, true>();
+  cudaError_t e = prepare_fused_act<false>();
+  return e != cudaSuccess ? e : prepare_fused_act<true>();
 }
 
 static bool fused_multi_tile(int B) { return B > 32; }
@@ -1095,39 +1113,46 @@ static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t str
 
 using FusedKernel = void (*)(const FusedMaps, const FusedParams);
 
-// The instantiation batch B runs with or without the clip and the L2 term.
-static FusedKernel fused_kernel_for(int B, bool clip, bool l2) {
-  const bool multi = fused_multi_tile(B);
+template <bool kAct>
+static FusedKernel fused_kernel_act(bool multi, bool clip, bool l2) {
   if (l2) {
-    if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, true> : fused_step_kernel<1, true, true>;
-    return multi ? fused_step_kernel<kFsMaxTiles, false, true> : fused_step_kernel<1, false, true>;
+    if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, true, kAct> : fused_step_kernel<1, true, true, kAct>;
+    return multi ? fused_step_kernel<kFsMaxTiles, false, true, kAct> : fused_step_kernel<1, false, true, kAct>;
   }
-  if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, false> : fused_step_kernel<1, true, false>;
-  return multi ? fused_step_kernel<kFsMaxTiles, false, false> : fused_step_kernel<1, false, false>;
+  if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, false, kAct> : fused_step_kernel<1, true, false, kAct>;
+  return multi ? fused_step_kernel<kFsMaxTiles, false, false, kAct> : fused_step_kernel<1, false, false, kAct>;
+}
+
+// The instantiation batch B runs with or without the clip and the L2 term, under activation `act` (ACT_NONE, the
+// value of a zero-initialised FusedParams, and ACT_RELU run the ReLU instantiations).
+static FusedKernel fused_kernel_for(int B, bool clip, bool l2, int act) {
+  const bool multi = fused_multi_tile(B);
+  return act > ACT_RELU ? fused_kernel_act<true>(multi, clip, l2) : fused_kernel_act<false>(multi, clip, l2);
 }
 
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
   if (lanes < 1 || p.B < 1 || p.B > 32 * kFsMaxTiles || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 ||
       (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1 || p.clip_kind < CLIP_OFF ||
       p.clip_kind > CLIP_VALUE || !(p.l2_scale >= 0.f && p.l2_scale < INFINITY) ||
-      (p.l2_scale != 0.f && p.shard[0].push.mode == PUSH_ATOMIC))
+      (p.l2_scale != 0.f && p.shard[0].push.mode == PUSH_ATOMIC) || !act_valid(p.act))
     return cudaErrorInvalidValue;
   for (int r = 0; r < kFusedCluster; ++r)
     if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
-  return cudaLaunchKernelEx(&cfg, fused_kernel_for(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f), maps, p);
+  return cudaLaunchKernelEx(&cfg, fused_kernel_for(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f, p.act), maps, p);
 }
 
 // How many clusters of the fused kernel that runs batch B can be co-resident on the device (upper bound for `lanes`).
-cudaError_t fused_max_lanes(int B, int* out) { return fused_max_lanes_for(B, false, false, out); }
+cudaError_t fused_max_lanes(int B, int* out) { return fused_max_lanes_for(B, false, false, ACT_RELU, out); }
 
-cudaError_t fused_max_lanes_clip(int B, int* out) { return fused_max_lanes_for(B, true, false, out); }
+cudaError_t fused_max_lanes_clip(int B, int* out) { return fused_max_lanes_for(B, true, false, ACT_RELU, out); }
 
-cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int* out) {
+cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int act, int* out) {
+  if (!act_valid(act)) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  return cudaOccupancyMaxActiveClusters(out, fused_kernel_for(B, clip, l2), &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_kernel_for(B, clip, l2, act), &cfg);
 }
 
 }  // namespace dm

@@ -4,12 +4,12 @@
 //
 // Operand roles in the MLP (all tensors keep their natural row-major layout; no transposes in global memory):
 //   forward   : A = W[out][in]   (K-major, *pulled straight from the PS shard over NVLink by TMA*)
-//               B = x[batch][in] (K-major)          D = pre-activation^T      -> EPI_TRANSPOSED (+bias, relu)
+//               B = x[batch][in] (K-major)          D = pre-activation^T      -> EPI_TRANSPOSED (+bias, act)
 //   dW        : A = dy[batch][out] (MN-major)  B = x[batch][in] (MN-major)   reduction over batch
 //               D = dW[out][in]                     -> EPI_ROWMAJOR_PUSH: the epilogue *is* the gradient
 //               push (P2P stores into the PS mailbox + release flag, or red.add for async SGD)
 //   dX        : A = W[out][in] (MN-major, pulled from the PS)  B = dy[batch][out] (K-major)
-//               D = dx^T                            -> EPI_TRANSPOSED (* relu' mask, bias-grad sums)
+//               D = dx^T                            -> EPI_TRANSPOSED (* act'(mask), bias-grad sums)
 //
 // These replace the MatMul/BiasAdd/Relu (+grads) ops of the reference training script and the implicit gRPC
 // variable fetch / gradient send around them (SURVEY.md K1,K2,K6,X3,X4).
@@ -24,6 +24,7 @@
 // cluster and reduce-scatter their partial accumulators through distributed shared memory (global-scratch
 // variants remain for tiles wider than 64 columns). Kernels of one training step are chained with programmatic
 // dependent launch (griddepcontrol). (The 784-H-10 models run the whole step in fused_step_sm90.cu instead.)
+#include "activation.cuh"
 #include "common.cuh"
 #include "protocol.h"
 
@@ -376,13 +377,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const int n = n0 + c;
             if (n < p.N && m_ok) {
               float val = acc + bias_pref;
-              if (p.relu) val = fmaxf(val, 0.f);
               if (p.mask != nullptr) {
                 const float a = p.mask_bf16
                                     ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(
                                           p.mask)[static_cast<size_t>(n) * p.ldmask + m])
                                     : reinterpret_cast<const float*>(p.mask)[static_cast<size_t>(n) * p.ldmask + m];
-                val = a > 0.f ? val : 0.f;
+                val = act_backward(p.act, a, val);   // dX: act'(y) from the layer's output
+              } else {
+                val = act_forward(p.act, val);
               }
               const size_t o = static_cast<size_t>(n) * p.ldo + m;
               if (p.out_bf16) reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16(val);
@@ -436,13 +438,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const int n = n0 + c0 + j;
             if (n < p.N && m_ok) {
               float val = v[j] + bias;
-              if (p.relu) val = fmaxf(val, 0.f);
               if (p.mask != nullptr) {
                 const float a = p.mask_bf16
                                     ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(
                                           p.mask)[static_cast<size_t>(n) * p.ldmask + m])
                                     : reinterpret_cast<const float*>(p.mask)[static_cast<size_t>(n) * p.ldmask + m];
-                val = a > 0.f ? val : 0.f;
+                val = act_backward(p.act, a, val);   // dX: act'(y) from the layer's output
+              } else {
+                val = act_forward(p.act, val);
               }
               colsum += val;
               const size_t o = static_cast<size_t>(n) * p.ldo + m;
@@ -554,13 +557,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int n = n0 + c;
         if (n < p.N && m_ok) {
           float val = acc + bias;
-          if (p.relu) val = fmaxf(val, 0.f);
           if (p.mask != nullptr) {
             const float a = p.mask_bf16
                                 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(
                                       p.mask)[static_cast<size_t>(n) * p.ldmask + m])
                                 : reinterpret_cast<const float*>(p.mask)[static_cast<size_t>(n) * p.ldmask + m];
-            val = a > 0.f ? val : 0.f;
+            val = act_backward(p.act, a, val);   // dX: act'(y) from the layer's output
+          } else {
+            val = act_forward(p.act, val);
           }
           colsum += val;
           const size_t o = static_cast<size_t>(n) * p.ldo + m;
@@ -669,6 +673,7 @@ static cudaError_t launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, co
 // dtype: 0 = fp32 (tf32 MMA), 1 = bf16
 cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int dtype, bool a_mn,
                         bool b_mn, int splits, cudaStream_t stream) {
+  if (!act_valid(p.act)) return cudaErrorInvalidValue;
   dim3 grid((p.M + kTileM - 1) / kTileM, (p.N + p.bn - 1) / p.bn, splits);
 #define DM_DISPATCH(T)                                                                  \
   if (!a_mn && !b_mn) return launch_one<T, false, false>(tmA, tmB, p, grid, stream);   \

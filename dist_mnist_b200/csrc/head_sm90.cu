@@ -8,7 +8,7 @@
 //            LOSS_XENT: mean_B(softmax_cross_entropy_with_logits)           reference DS:35
 //   correct= #(argmax logits == argmax labels)                              (accuracy numerator, SURVEY K12)
 //   dlogits, dW_last = dlogits^T . h, db_last = sum_B dlogits
-//   dpre   = (dlogits . W_last) * relu'(h)      -> [B][H] buffer consumed by the wgmma dW / dX GEMMs
+//   dpre   = (dlogits . W_last) * act'(h)       -> [B][H] buffer consumed by the wgmma dW / dX GEMMs
 //   db_hid = sum_B dpre
 // and pushes dW_last / db_last / db_hid to the parameter server (mailbox + flags, or red.add for SGD).
 //
@@ -18,6 +18,7 @@
 // of dependent instructions deep: operands are staged in shared memory once, all global loads of a phase are
 // independent, 16 warps hide the shared-memory latency.
 // Replaces reference ops DS:52-53 + their gradients from DS:103 (SURVEY K3, K4, K5, part of K6, K12).
+#include "activation.cuh"
 #include "common.cuh"
 #include "protocol.h"
 
@@ -268,6 +269,7 @@ __global__ void __launch_bounds__(kHeadThreads, 1) head_kernel(const __grid_cons
 #pragma unroll
   for (int c = 0; c < kMaxC; ++c) dw[c] = 0.f;
   float dbh = 0.f;
+  const int act = p.act == ACT_NONE ? ACT_RELU : p.act;   // (a zero-initialised HeadParams keeps the ReLU)
   for (int b = grp; b < B; b += kHeadGroups) {
     const float hv = sHs[b * kHeadSlice + hh];
     const float4* dl4 = reinterpret_cast<const float4*>(sLogit + b * kMaxC);  // broadcast reads
@@ -280,7 +282,7 @@ __global__ void __launch_bounds__(kHeadThreads, 1) head_kernel(const __grid_cons
       dw[4 * c4 + 2] = fmaf(d.z, hv, dw[4 * c4 + 2]); dh = fmaf(d.z, wcol[4 * c4 + 2], dh);
       dw[4 * c4 + 3] = fmaf(d.w, hv, dw[4 * c4 + 3]); dh = fmaf(d.w, wcol[4 * c4 + 3], dh);
     }
-    const float dp = hv > 0.f ? dh : 0.f;
+    const float dp = act_backward(act, hv, dh);
     dbh += dp;
     if (h_ok) st_act(p.dpre, static_cast<size_t>(b) * p.ldh + h, p.act_bf16, dp);
   }
@@ -349,7 +351,7 @@ cudaError_t prepare_head_kernel() {
 }
 
 cudaError_t launch_head(const HeadParams& p, cudaStream_t stream) {
-  if (p.C > kMaxC || p.B > kMaxB || p.B_pad > kMaxB) return cudaErrorInvalidValue;
+  if (p.C > kMaxC || p.B > kMaxB || p.B_pad > kMaxB || !act_valid(p.act)) return cudaErrorInvalidValue;
   const size_t smem = head_smem_bytes(p.B_pad, p.H, p.C);
   if (smem > static_cast<size_t>(kHeadMaxSmem)) return cudaErrorInvalidValue;
   const int grid = (p.H + kHeadSlice - 1) / kHeadSlice;

@@ -43,7 +43,8 @@ struct PushTarget {
 // Epilogue selection for the wgmma GEMM  D[M,N] = A[M,K] * B[N,K]^T  (fp32 accumulators)
 enum GemmEpilogue : int {
   // out[n * ldo + m] = f(acc[m][n]) — lanes write consecutive m (coalesced). Forward and dX GEMMs.
-  //   f = (+bias[m]) -> (relu) -> (* (mask[n*ldmask+m] > 0)), optional sums over n (bias grads).
+  //   forward (mask null): f = (+bias[m]) -> act;  dX (mask set): f = act'(mask[n*ldmask+m]) * acc, the derivative
+  //   computed from the layer's output as TF's *Grad ops do; optional sums over n (bias grads).
   EPI_TRANSPOSED = 0,
   // out[m * ldo + n] = acc[m][n] — each lane owns a row run. dW GEMMs, fused with the gradient push.
   EPI_ROWMAJOR_PUSH = 1,
@@ -56,13 +57,13 @@ struct GemmParams {
   int kc_per_split;     // k-chunks handled per blockIdx.z
   int epi;              // GemmEpilogue
   int out_bf16;         // EPI_TRANSPOSED: output element type (0 = fp32, 1 = bf16)
-  int relu;
+  int act;             // ActivationKind of the layer (0 = none, 1 = relu: the values of the former `relu` flag)
   int ldo;
   int ldmask;
   int mask_bf16;
   void* out;            // EPI_TRANSPOSED destination
   const float* bias;    // [M] or null (may be a peer pointer into the PS arena)
-  const void* mask;     // [N][ldmask] activations (relu' = mask > 0) or null
+  const void* mask;     // [N][ldmask] activations y of the layer whose act' the dX epilogue applies, or null
   PushTarget colsum;    // EPI_TRANSPOSED: optional sum over n of the stored value -> vector[m] (bias grads)
   uint64_t colsum_offset;  // element offset of the vector inside colsum.base
   int colsum_item_base; // flag item index of mtile 0 of the vector
@@ -82,6 +83,18 @@ struct GemmParams {
                              // pdl = 1: launch with programmatic stream serialization (prologue overlaps the
                              //    previous kernel of the step; data reads wait on griddepcontrol.wait)
   int pad2_, pad3_;
+};
+
+// Activation of a hidden layer (TF 1.15 tf.nn functors; activation.cuh has f and f', models/mlp.py the reference).
+enum ActivationKind : int {
+  ACT_NONE = 0,
+  ACT_RELU = 1,
+  ACT_RELU6 = 2,
+  ACT_LEAKY_RELU = 3,   // alpha 0.2
+  ACT_ELU = 4,
+  ACT_SELU = 5,
+  ACT_SIGMOID = 6,
+  ACT_TANH = 7,
 };
 
 // Softmax-cross-entropy head (last dense layer + loss + its gradients), see head_sm90.cu
@@ -110,7 +123,7 @@ struct HeadParams {
   const float* labels;  // [B_pad][C] one-hot (or soft) labels
   const float* w_last;  // [C][H] fp32 master on the PS (peer pointer)
   const float* b_last;  // [C]
-  void* dpre;           // [B_pad][ldh] gradient wrt last hidden pre-activation (relu' applied)
+  void* dpre;           // [B_pad][ldh] gradient wrt last hidden pre-activation (act' applied)
   PushTarget push;      // dW_last   — each small gradient goes to the shard that owns its variable
   PushTarget push_bl;   // db_last     (round-robin placement puts sm_w and sm_b on different ps tasks)
   PushTarget push_bh;   // db of the last hidden layer
@@ -127,6 +140,9 @@ struct HeadParams {
   uint32_t nslots;
   uint32_t n_inbox;          // number of PS shards this worker pushes to
   long long* debug_ts;       // optional clock64() phase stamps of CTA 0; null in production
+  int act;                   // ActivationKind of the last hidden layer, whose act'(h) gives dpre (appended; ACT_NONE,
+                             // the value of a zero-initialised block, is read as ACT_RELU)
+  int act_pad_;
 };
 
 // One unit of PS apply work.
@@ -328,6 +344,10 @@ struct FusedParams {
   // weights (and, with l2_biases, the biases) before the clip. 0 runs the unregularized instantiations.
   float l2_scale;          // finite, >= 0
   uint32_t l2_biases;      // 1: the biases are regularized too
+  // activation of the hidden layer (ActivationKind, appended): ACT_NONE (a zero-initialised block) and ACT_RELU run
+  // the ReLU instantiations, any other the ones that read this field
+  int act;
+  uint32_t act_pad_;
 };
 enum GradClipKind : int {
   CLIP_OFF = 0,

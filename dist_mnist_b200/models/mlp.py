@@ -19,7 +19,7 @@ path of the CPU plumbing backend; it is *not* the GPU hot path (that is `ops/` +
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Dict, List, Tuple
 
 import torch
@@ -42,6 +42,19 @@ class VarSpec:
         return n
 
 
+# Activations of the hidden layers (`--activation`), TF 1.15's tf.nn functors and registered gradients. The index of a
+# name is its protocol.h ActivationKind code minus one (code 0 is "none").
+ACTIVATIONS = ("relu", "relu6", "leaky_relu", "elu", "selu", "sigmoid", "tanh")
+LEAKY_RELU_ALPHA = 0.2                                 # tf.nn.leaky_relu's default
+SELU_SCALE = 1.0507009873554804934193349852946         # TF's selu constants: scale
+SELU_SCALE_ALPHA = 1.7580993408473768599402175208123   # and scale * alpha
+
+
+def activation_code(name: str) -> int:
+    """protocol.h ActivationKind of a hidden-layer activation (ACT_RELU = 1, ...)."""
+    return ACTIVATIONS.index(name) + 1
+
+
 @dataclass(frozen=True)
 class MLPSpec:
     name: str = "book"
@@ -50,6 +63,11 @@ class MLPSpec:
     num_classes: int = 10
     loss: str = "book"   # "book" | "xent"
     init: str = "book"   # "book" (truncated normal, DS:41-47) | "glorot" (tf.layers.dense default)
+    activation: str = "relu"   # of every hidden layer, one of ACTIVATIONS (the logits layer has none)
+
+    def __post_init__(self):
+        if self.activation not in ACTIVATIONS:
+            raise ValueError(f"unknown activation {self.activation!r} (expected {' | '.join(ACTIVATIONS)})")
 
     @property
     def layer_sizes(self) -> List[Tuple[int, int]]:
@@ -105,14 +123,16 @@ def wide_model() -> MLPSpec:
     return MLPSpec(name="wide", hidden=(1024, 1024), loss="xent", init="glorot")
 
 
-def get_model(name: str, hidden_units: int = 100) -> MLPSpec:
+def get_model(name: str, hidden_units: int = 100, activation: str = "relu") -> MLPSpec:
     if name == "book":
-        return book_model(hidden_units)
-    if name == "zhihu":
-        return zhihu_model()
-    if name == "wide":
-        return wide_model()
-    raise ValueError(f"unknown model {name!r} (expected book | zhihu | wide)")
+        spec = book_model(hidden_units)
+    elif name == "zhihu":
+        spec = zhihu_model()
+    elif name == "wide":
+        spec = wide_model()
+    else:
+        raise ValueError(f"unknown model {name!r} (expected book | zhihu | wide)")
+    return spec if activation == "relu" else replace(spec, activation=activation)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -162,14 +182,63 @@ def to_reference_layout(params: Dict[str, torch.Tensor]) -> Dict[str, torch.Tens
 # ----------------------------------------------------------------------------------------------
 # plain-PyTorch model (numerical reference + CPU backend compute)
 # ----------------------------------------------------------------------------------------------
-def forward_logits(spec: MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+def activate(name: str, x: torch.Tensor) -> torch.Tensor:
+    """y = f(x), TF 1.15's functor of `name`, each operation rounded in x's dtype (no fused multiply-add, exp - 1 rather
+    than expm1): what every engine computes."""
+    if name == "relu":
+        return torch.relu(x)
+    if name == "relu6":
+        return torch.clamp(torch.clamp(x, min=0.0), max=6.0)
+    if name == "leaky_relu":
+        return torch.where(x > 0, x, LEAKY_RELU_ALPHA * x)
+    if name == "elu":
+        return torch.where(x < 0, torch.exp(x) - 1, x)
+    if name == "selu":
+        return torch.where(x < 0, SELU_SCALE_ALPHA * (torch.exp(x) - 1), SELU_SCALE * x)
+    if name == "sigmoid":
+        return 1 / (1 + torch.exp(-x))
+    if name == "tanh":
+        return torch.tanh(x)
+    raise ValueError(f"unknown activation {name!r}")
+
+
+def activation_grad(name: str, y: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
+    """dx = dy * f'(x), computed from the layer's output y as TF's *Grad ops compute it."""
+    if name == "relu":
+        return dy * (y > 0).to(dy.dtype)
+    if name == "relu6":
+        return dy * ((y > 0) & (y < 6)).to(dy.dtype)
+    if name == "leaky_relu":
+        return torch.where(y > 0, dy, LEAKY_RELU_ALPHA * dy)
+    if name == "elu":
+        return torch.where(y < 0, dy * (y + 1), dy)
+    if name == "selu":
+        return torch.where(y < 0, dy * (y + SELU_SCALE_ALPHA), dy * SELU_SCALE)
+    if name == "sigmoid":
+        return dy * y * (1 - y)
+    if name == "tanh":
+        return dy * (1 - y * y)
+    raise ValueError(f"unknown activation {name!r}")
+
+
+def _activate_autograd(name: str, x: torch.Tensor) -> torch.Tensor:
+    """torch's own activations (their autograd derivatives are independent of `activation_grad`)."""
+    F = torch.nn.functional
+    fns = {"relu": torch.relu, "relu6": F.relu6, "leaky_relu": lambda t: F.leaky_relu(t, LEAKY_RELU_ALPHA),
+           "elu": F.elu, "selu": F.selu, "sigmoid": torch.sigmoid, "tanh": torch.tanh}
+    return fns[name](x)
+
+
+def forward_logits(spec: MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
+                   act_fn=activate) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+    """(logits, [x, hidden activations...]); `act_fn(name, z)` applies the hidden layers' activation."""
     acts = [x]
     h = x
     names = spec.variable_names()
     for i, (wn, bn) in enumerate(names):
         z = h @ params[wn].t() + params[bn]
         if i < len(names) - 1:
-            h = torch.relu(z)
+            h = act_fn(spec.activation, z)
             acts.append(h)
         else:
             return z, acts
@@ -192,7 +261,7 @@ def accuracy_count(logits: torch.Tensor, labels: torch.Tensor) -> int:
 def loss_and_grads(spec: MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor, labels: torch.Tensor):
     """Autograd reference: returns (loss, grads by name, logits)."""
     leaves = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
-    logits, _ = forward_logits(spec, leaves, x)
+    logits, _ = forward_logits(spec, leaves, x, act_fn=_activate_autograd)
     loss = loss_from_logits(spec, logits, labels)
     grads = torch.autograd.grad(loss, list(leaves.values()))
     return loss.detach(), {k: g for k, g in zip(leaves.keys(), grads)}, logits.detach()
@@ -220,7 +289,7 @@ def manual_loss_and_grads(spec: MLPSpec, params: Dict[str, torch.Tensor], x: tor
         grads[wn] = d.t() @ acts[i]
         grads[bn] = d.sum(dim=0)
         if i > 0:
-            d = (d @ params[wn]) * (acts[i] > 0).to(d.dtype)
+            d = activation_grad(spec.activation, acts[i], d @ params[wn])
     return loss, grads, logits
 
 

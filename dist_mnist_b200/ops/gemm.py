@@ -149,10 +149,11 @@ def _base_params(M, N_, K, bn, dtype, splits) -> N.GemmParams:
 
 
 def forward_plan(*, w_ptr: int, x_ptr: int, out_ptr: int, bias_ptr: int, O: int, I: int, B: int, B_pad: int,
-                 dtype: int, relu: bool, ldw: Optional[int] = None, ldx: Optional[int] = None,
+                 dtype: int, act: int, ldw: Optional[int] = None, ldx: Optional[int] = None,
                  ldo: Optional[int] = None, bump_seq_ptr: int = 0, seq_counter_ptr: int = 0, splits: Optional[int] = None,
                  name: str = "fwd") -> GemmPlan:
-    """out[b, o] = act(x[b, :] . W[o, :] + bias[o]); A = W (K-major, may be peer), B = x (K-major)."""
+    """out[b, o] = act(x[b, :] . W[o, :] + bias[o]) (`act` an ActivationKind, N.ACT_NONE for none); A = W (K-major, may
+    be peer), B = x (K-major)."""
     assert B_pad % 16 == 0 and B_pad <= 256 and B <= B_pad
     es = elem_size(dtype)
     ldw = I if ldw is None else ldw
@@ -175,7 +176,7 @@ def forward_plan(*, w_ptr: int, x_ptr: int, out_ptr: int, bias_ptr: int, O: int,
     p.out_bf16 = int(dtype == N.DT_BF16)
     p.ldo = ldo
     p.bias = bias_ptr
-    p.relu = int(relu)
+    p.act = act
     p.bump_seq = bump_seq_ptr
     p.seq_counter = seq_counter_ptr or bump_seq_ptr
     grid = (mtiles, 1, splits)
@@ -218,10 +219,11 @@ def dw_tiles(O: int, I: int, bn: int = 64):
 
 
 def dx_plan(*, w_ptr: int, dy_ptr: int, out_ptr: int, mask_ptr: int, O: int, I: int, B: int, B_pad: int,
-            dtype: int, ldw: Optional[int] = None, lddy: Optional[int] = None, ldo: Optional[int] = None,
+            dtype: int, act: int, ldw: Optional[int] = None, lddy: Optional[int] = None, ldo: Optional[int] = None,
             colsum: Optional[N.PushTarget] = None, colsum_offset: int = 0, colsum_item_base: int = 0,
             splits: Optional[int] = None, name: str = "dx") -> GemmPlan:
-    """dx[b, i] = (dy[b, :] . W[:, i]) * (mask[b, i] > 0); A = W (MN-major, may be peer), B = dy (K-major)."""
+    """dx[b, i] = (dy[b, :] . W[:, i]) * act'(mask[b, i]), the derivative of ActivationKind `act` from the layer's
+    output `mask`; A = W (MN-major, may be peer), B = dy (K-major)."""
     assert B_pad % 16 == 0 and B_pad <= 256
     es = elem_size(dtype)
     k = bke(dtype)
@@ -246,6 +248,7 @@ def dx_plan(*, w_ptr: int, dy_ptr: int, out_ptr: int, mask_ptr: int, O: int, I: 
     p.mask = mask_ptr
     p.ldmask = ldo
     p.mask_bf16 = int(dtype == N.DT_BF16)
+    p.act = act
     if colsum is not None:
         p.colsum = colsum
         p.colsum_offset = colsum_offset

@@ -32,7 +32,7 @@ class HeadPlan:
 
 
 def head_plan(*, h_ptr: int, labels_ptr: int, w_last_ptr: int, b_last_ptr: int, dpre_ptr: int, result_ptr: int,
-              B: int, B_pad: int, H: int, num_classes: int, loss_kind: int, act_bf16: bool,
+              B: int, B_pad: int, H: int, num_classes: int, loss_kind: int, act_bf16: bool, act: int = N.ACT_RELU,
               push: Optional[N.PushTarget] = None, push_bh: Optional[N.PushTarget] = None,
               push_bl: Optional[N.PushTarget] = None,
               off_w_last: int = 0, off_b_last: int = 0, off_b_hidden: int = 0,
@@ -44,6 +44,7 @@ def head_plan(*, h_ptr: int, labels_ptr: int, w_last_ptr: int, b_last_ptr: int, 
     p.B, p.B_pad, p.H, p.C = B, B_pad, H, num_classes
     p.loss_kind = loss_kind
     p.act_bf16 = int(act_bf16)
+    p.act = act   # ActivationKind of the last hidden layer: dpre = (dlogits . W_last) * act'(h)
     p.ldh = H if ldh is None else ldh
     p.compute_grads = int(compute_grads)
     p.h, p.labels, p.w_last, p.b_last, p.dpre = h_ptr, labels_ptr, w_last_ptr, b_last_ptr, dpre_ptr

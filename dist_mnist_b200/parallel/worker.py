@@ -581,6 +581,7 @@ class Worker:
         names = spec.variable_names()
         sizes = spec.layer_sizes
         L = len(sizes)
+        act_code = mlp.activation_code(spec.activation)
         # activations / pre-activation gradients of the hidden layers (row padded, zero initialised)
         # (one set per executor slot: steps of different slots may run concurrently)
         self._slot_act = [[None] + [torch.zeros(self.B_pad, gemm_ops.padded_ld(sizes[l][1]), dtype=self.tdtype,
@@ -601,7 +602,7 @@ class Worker:
             self._eval_plans.append(gemm_ops.forward_plan(
                 w_ptr=self._weight_ptr(wl), x_ptr=self._eval_x.data_ptr() if l == 0 else self.act[l].data_ptr(),
                 out_ptr=self.act[l + 1].data_ptr(), bias_ptr=self.ps_segs[bl.ps].addr("params", bl.offset * 4),
-                O=fout, I=fin, B=self.batch, B_pad=self.B_pad, dtype=self.dt, relu=True, ldw=wl.ld,
+                O=fout, I=fin, B=self.batch, B_pad=self.B_pad, dtype=self.dt, act=act_code, ldw=wl.ld,
                 ldx=self.ld_in if l == 0 else self.act[l].shape[1], ldo=self.act[l + 1].shape[1], name=f"eval_fwd{l}"))
         wl, bl = lay.by_name[names[L - 1][0]], lay.by_name[names[L - 1][1]]
         self._eval_plans.append(head_ops.head_plan(
@@ -610,7 +611,7 @@ class Worker:
             b_last_ptr=self.ps_segs[bl.ps].addr("params", bl.offset * 4), dpre_ptr=self.dact[L - 1].data_ptr(),
             result_ptr=self._eval_res.data_ptr(), B=self.batch, B_pad=self.B_pad, H=sizes[L - 1][0],
             num_classes=spec.num_classes, loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT,
-            act_bf16=cfg.dtype == "bf16", compute_grads=False, ldh=self.act[L - 1].shape[1]))
+            act_bf16=cfg.dtype == "bf16", act=act_code, compute_grads=False, ldh=self.act[L - 1].shape[1]))
         torch.cuda.synchronize(self.device)
         clip = self.opt.clip.enabled or self.opt.l2.enabled
         # gradient clipping / L2 regularization: per ring slot, a local gradient buffer per shard (the epilogues' push
@@ -650,7 +651,7 @@ class Worker:
                 plans.append(gemm_ops.forward_plan(
                     w_ptr=self._weight_ptr(wl), x_ptr=in_ptr, out_ptr=act[l + 1].data_ptr(),
                     bias_ptr=self.ps_segs[bl.ps].addr("params", bl.offset * 4), O=fout, I=fin, B=self.batch,
-                    B_pad=self.B_pad, dtype=self.dt, relu=True, ldw=wl.ld, ldx=ld_in, ldo=act[l + 1].shape[1],
+                    B_pad=self.B_pad, dtype=self.dt, act=act_code, ldw=wl.ld, ldx=ld_in, ldo=act[l + 1].shape[1],
                     bump_seq_ptr=seq_ptr if l == 0 else 0, seq_counter_ptr=seq_counter, name=f"fwd{l}"))
             # ---- classifier head ----
             wn, bn = names[L - 1]
@@ -665,7 +666,7 @@ class Worker:
                 dpre_ptr=dact[L - 1].data_ptr(), result_ptr=rd.value, B=self.batch, B_pad=self.B_pad,
                 H=sizes[L - 1][0], num_classes=spec.num_classes,
                 loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT, act_bf16=cfg.dtype == "bf16",
-                push=push(wl.ps), push_bh=push(hb.ps), push_bl=push(bl.ps),
+                act=act_code, push=push(wl.ps), push_bh=push(hb.ps), push_bl=push(bl.ps),
                 off_w_last=wl.offset, off_b_last=bl.offset, off_b_hidden=hb.offset,
                 item_w_last_base=wl.item_base, item_b_last=bl.item_base, item_b_hidden_base=hb.item_base,
                 seq_ptr=seq_ptr, inbox_ptr=inbox_ptr, n_inbox=len(self.inbox_order), ps_global_step_ptr=gs_ptr,
@@ -686,6 +687,7 @@ class Worker:
                     plans.append(gemm_ops.dx_plan(
                         w_ptr=self._weight_ptr(wl), dy_ptr=dact[l + 1].data_ptr(), out_ptr=dact[l].data_ptr(),
                         mask_ptr=act[l].data_ptr(), O=fout, I=fin, B=self.batch, B_pad=self.B_pad, dtype=self.dt,
+                        act=act_code,
                         ldw=wl.ld, lddy=dact[l + 1].shape[1], ldo=dact[l].shape[1],
                         colsum=push(pb.ps), colsum_offset=pb.offset, colsum_item_base=pb.item_base,
                         name=f"dx{l}"))
@@ -778,12 +780,9 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
-        if self.opt.l2.enabled:
-            N.check(self.lib.dm_fused_max_lanes_l2(self.device, self.batch, int(self.opt.clip.enabled),
-                                                   C.byref(max_lanes)), "fused occupancy")
-        else:
-            occupancy = self.lib.dm_fused_max_lanes_clip if self.opt.clip.enabled else self.lib.dm_fused_max_lanes
-            N.check(occupancy(self.device, self.batch, C.byref(max_lanes)), "fused occupancy")
+        N.check(self.lib.dm_fused_max_lanes_for(self.device, self.batch, int(self.opt.clip.enabled),
+                                                int(self.opt.l2.enabled), mlp.activation_code(spec.activation),
+                                                C.byref(max_lanes)), "fused occupancy")
         free = max_lanes.value
         if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
             # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots
@@ -852,6 +851,7 @@ class Worker:
                             if cfg.push_mode == "atomic" else None)
         self.opt.clip.fill_native(p)   # CLIP_OFF: the unclipped kernels
         self.opt.l2.fill_native(p)     # l2_scale 0: the unregularized kernels
+        p.act = mlp.activation_code(spec.activation)   # ACT_RELU: the ReLU kernels
         if os.environ.get("DM_FUSED_DEBUG_TS") == "1":
             self._fx_dbg = torch.zeros(64, dtype=torch.int64, device=f"cuda:{self.device}")
             p.debug_ts = self._fx_dbg.data_ptr()
