@@ -402,8 +402,9 @@ def check_ps_serve(ieee: bool = False, schedule=None, sched_step: int = 0, movin
     return ok
 
 
-def _ref_apply(opt, p, m, v, g, lr, t):
-    """One optimizer step of any kind at rate `lr` (Adam: its t-th step), on tensors in their own dtype."""
+def _ref_apply(opt, p, m, v, g, lr, t, mg=None, global_step=None):
+    """One optimizer step of any kind at rate `lr` (Adam: its t-th step), on tensors in their own dtype. `mg`: centered
+    RMSProp's third slot (the result is then (p, m, v, mg)); `global_step`: AdagradDA's T."""
     if opt.kind == "sgd":
         return p - lr * g, m, v
     if opt.kind == "adam":
@@ -414,19 +415,21 @@ def _ref_apply(opt, p, m, v, g, lr, t):
         lr_t = lr * (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
         return p - lr_t * m / (v.sqrt() + eps), m, v
     from bench_tools.gpu_e2e import tf1_apply
-    return tf1_apply(dataclasses.replace(opt, lr=lr), p, m, v, g)
+    return tf1_apply(dataclasses.replace(opt, lr=lr), p, m, v, g, mg=mg, global_step=global_step)
 
 
 def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step: int = 0) -> bool:
-    """The serve kernel's Momentum / Adagrad / RMSProp / Adadelta / FTRL / ProximalAdagrad / ProximalGradientDescent
-    instantiations (`opt`: an OptimizerConfig; `opt.math` picks the fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
+    """The serve kernel's Momentum / Adagrad / RMSProp (centered too) / Adadelta / FTRL / ProximalAdagrad /
+    ProximalGradientDescent / AdagradDA instantiations (`opt`: an OptimizerConfig; `opt.math` picks the fast or the ieee one) alone, set up as `check_ps_serve`: 3 workers with 3 pushes each, staged before the launch,
     against the TF1 formulas in fp64 (parameters and both slot buffers within 1e-5 relative error; the bf16 shadow,
     global_step and the acks exact). `resident`: one pushed push per worker and pass (lookahead 1) and one vectorisable
     item of <= 4096 elements per CTA, the geometry that keeps the item's state in registers from pass to pass.
     A non-constant `opt.schedule` runs the scheduled instantiation (Adam and SGD too), every item starting at schedule
     step `sched_step`; the check then includes every item's final sched_step. `opt.moving_average_decay` runs the
     averaging instantiation (any rule, any schedule): the shadows start at the initial parameters and are checked
-    against fp64 within the same bound."""
+    against fp64 within the same bound. Centered RMSProp's third slot mg is checked like the other two. AdagradDA
+    runs in the scheduled instantiation whatever the schedule: the step whose last push sits at position q has
+    T = sched_step + q + 1, and the final sched_step is checked."""
     from dist_mnist_b200 import _native as N
     dev = "cuda"
     torch.manual_seed(6)
@@ -447,6 +450,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     p0 = params.clone()
     m = torch.full((arena,), m0, device=dev)
     v = torch.full((arena,), v0, device=dev)
+    mg = torch.zeros(arena, device=dev) if opt.uses_mg else None
     shadow = torch.zeros(arena, dtype=torch.bfloat16, device=dev)
     mailbox = torch.zeros(n_workers, nslots, arena, device=dev)
     flags = torch.zeros(n_workers, nslots, n_items, dtype=torch.int32, device=dev)
@@ -480,6 +484,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     P.n_flags = n_items
     P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
     opt.fill_native_rule(P)
+    P.mg = mg.data_ptr() if mg is not None else None
     P.ieee_math = 1 if opt.math == "ieee" else 0
     opt.schedule.fill_native(P)
     ema = params.clone() if opt.moving_averages else None
@@ -508,6 +513,7 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
     # moving averages: the step whose last push sits at position q moves the shadows by 1 - ema_decay_at(sched_step +
     # q + 1) (fp32 decay as the kernel computes it, the update in fp64)
     er = p0.double()
+    gr = torch.zeros(arena, dtype=torch.float64, device=dev) if mg is not None else None
     t = 0
     for s in range(n_push):
         group = [grads[w, s].double() for w in range(n_workers)]
@@ -515,30 +521,37 @@ def check_ps_serve_tf1(opt, apply_mode: int, resident: bool = False, sched_step:
                  else [(g, s * n_workers + w) for w, g in enumerate(group)])
         for gg, pos in steps:
             t += 1
-            pr, mr, vr = _ref_apply(opt, pr, mr, vr, gg, opt.lr_at(sched_step + pos), t)
+            last = s * n_workers + n_workers - 1 if apply_mode == N.APPLY_MERGED else pos
+            # AdagradDA's T: the item's applied pushes after this step, as a uint32 like PsItemState::sched_step
+            da_t = (sched_step + last + 1) & 0xFFFFFFFF if opt.kind == "adagrad_da" else None
+            out = _ref_apply(opt, pr, mr, vr, gg, opt.lr_at(sched_step + pos), t, mg=gr, global_step=da_t)
+            if gr is not None:
+                pr, mr, vr, gr = out
+            else:
+                pr, mr, vr = out
             if ema is not None:
-                last = s * n_workers + n_workers - 1 if apply_mode == N.APPLY_MERGED else pos
                 er = er - (er - pr) * (1.0 - opt.ema_decay_at(sched_step + last + 1))
     pr, mr, vr = torch.where(mask, pr, p0.double()), torch.where(mask, mr, m0), torch.where(mask, vr, v0)
     e_p, e_m, e_v = rel_err(params, pr), rel_err(m, mr), rel_err(v, vr)
+    e_g = rel_err(mg, torch.where(mask, gr, 0.0)) if mg is not None else 0.0
     e_e = rel_err(ema, torch.where(mask, er, p0.double())) if ema is not None else 0.0
     shadow_exact = bool(torch.equal(shadow[mask], params[mask].to(torch.bfloat16)))
     gs = int(gstep.item())
     acks = inbox[:, 0].tolist()
-    good = (max(e_p, e_m, e_v, e_e) < 1e-5 and shadow_exact and gs == n_workers * n_push
+    good = (max(e_p, e_m, e_v, e_e, e_g) < 1e-5 and shadow_exact and gs == n_workers * n_push
             and acks == [n_push] * n_workers and int(exitc.item()) == n_ctas)
-    name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''} momentum={opt.momentum} math={opt.math} "
-            f"mode={apply_mode} resident={resident}")
-    if opt.kind in ("adadelta", "ftrl", "proximal_adagrad", "proximal_sgd"):
+    name = (f"ps_serve {opt.kind}{' nesterov' if opt.use_nesterov else ''}{' centered' if opt.centered else ''} "
+            f"momentum={opt.momentum} math={opt.math} mode={apply_mode} resident={resident}")
+    if opt.kind in ("adadelta", "ftrl", "proximal_adagrad", "proximal_sgd", "adagrad_da"):
         name += (f" rho={opt.rho} l1={opt.l1_regularization_strength} l2={opt.l2_regularization_strength} "
                  f"shrinkage={opt.l2_shrinkage_regularization_strength} lr_power={opt.learning_rate_power} "
                  f"accum0={opt.initial_accumulator_value}")
-    extra = ""
-    if not opt.schedule.constant or ema is not None:
+    extra = f" mg={e_g:.1e}" if mg is not None else ""
+    if not opt.schedule.constant or ema is not None or opt.kind == "adagrad_da":
         steps_now = sorted({int(x) & 0xFFFFFFFF for x in state.view(torch.int32).view(n_items, 4)[:, 3].tolist()})
         good &= steps_now == [(sched_step + n_workers * n_push) & 0xFFFFFFFF]
         name += f" schedule={opt.schedule.kind} from={sched_step}"
-        extra = f" sched_step={steps_now}"
+        extra += f" sched_step={steps_now}"
     if ema is not None:
         name += f" ema={opt.moving_average_decay} num_updates={opt.moving_average_num_updates}"
         extra += f" err ema={e_e:.1e}"

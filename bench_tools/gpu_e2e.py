@@ -7,6 +7,7 @@
 from __future__ import annotations
 
 import dataclasses
+import struct
 import subprocess
 import sys
 import os
@@ -28,12 +29,39 @@ def _prox_shrink(prox, a, l1, l2):
     return prox / (1 + l2 * a)
 
 
-def tf1_apply(opt, p, m, v, g):
-    """One TF1 `training_ops` step of Momentum / Adagrad / RMSProp (not centered) / Adadelta / FTRL (V2 with
-    l2_shrinkage) / ProximalAdagrad / ProximalGradientDescent on tensors, in their own dtype: `m` is the slot kept in
-    adam_m (momentum accumulator, RMSProp mom, Adadelta accum_update, FTRL linear), `v` the one in adam_v (Adagrad,
-    FTRL and ProximalAdagrad accumulator, RMSProp ms, Adadelta accum). Returns the new (p, m, v)."""
-    if opt.kind == "momentum":
+def _f32(x: float) -> float:
+    return struct.unpack("f", struct.pack("f", float(x)))[0]
+
+
+def tf1_apply(opt, p, m, v, g, mg=None, global_step=None):
+    """One TF1 `training_ops` step of Momentum / Adagrad / RMSProp / Adadelta / FTRL (V2 with l2_shrinkage) /
+    ProximalAdagrad / ProximalGradientDescent / AdagradDA on tensors, in their own dtype: `m` is the slot kept in
+    adam_m (momentum accumulator, RMSProp mom, Adadelta accum_update, FTRL linear, AdagradDA gradient_accumulator), `v`
+    the one in adam_v (Adagrad, FTRL and ProximalAdagrad accumulator, RMSProp ms, Adadelta accum, AdagradDA
+    gradient_squared_accumulator). Returns the new (p, m, v).
+
+    `mg`: centered RMSProp's third slot (needed when opt.centered); the result is then (p, m, v, mg).
+    `global_step`: AdagradDA's T, the applied steps including this one (an integer; converted to fp32 once, as TF's
+    static_cast<float> and the ps do)."""
+    if opt.kind == "rmsprop" and opt.centered:
+        if mg is None:
+            raise ValueError("centered rmsprop needs its mg slot")
+        v = v + (g * g - v) * (1 - opt.decay)
+        mg = mg + (g - mg) * (1 - opt.decay)
+        m = m * opt.momentum + (g * opt.lr) / ((v - mg * mg) + opt.eps).sqrt()
+        return p - m, m, v, mg
+    if opt.kind == "adagrad_da":
+        if global_step is None:
+            raise ValueError("adagrad_da needs the global step T")
+        T = _f32(int(global_step))
+        l1, l2, lr = opt.l1_regularization_strength, opt.l2_regularization_strength, opt.lr
+        m = m + g
+        v = v + g * g
+        if l1 > 0:
+            p = -lr * m.sign() * (m.abs() - T * l1).clamp_min(0) / (l2 * (T * lr) + v.sqrt())
+        else:
+            p = -lr * m / ((T * lr) * l2 + v.sqrt())
+    elif opt.kind == "momentum":
         m = opt.momentum * m + g
         p = p - (g * opt.lr + m * opt.momentum * opt.lr) if opt.use_nesterov else p - opt.lr * m
     elif opt.kind == "adagrad":
@@ -67,17 +95,21 @@ def tf1_apply(opt, p, m, v, g):
         v = n
     else:
         raise ValueError(opt.kind)
-    return p, m, v
+    return (p, m, v) if mg is None else (p, m, v, mg)
 
 
-def ref_slots(opt, params):
-    """Initial (m, v) slot dicts of `opt` for `params` (Worker.initialize_variables writes the same values)."""
+def ref_slots(opt, params, with_mg=False):
+    """Initial (m, v) slot dicts of `opt` for `params` (Worker.initialize_variables writes the same values).
+    `with_mg`: (m, v, mg), with centered RMSProp's third slot (zeros)."""
     m0, v0 = opt.slot_init()
-    return ({k: torch.full_like(t, m0) for k, t in params.items()}, {k: torch.full_like(t, v0) for k, t in params.items()})
+    m, v = {k: torch.full_like(t, m0) for k, t in params.items()}, {k: torch.full_like(t, v0) for k, t in params.items()}
+    return (m, v, {k: torch.zeros_like(t) for k, t in params.items()}) if with_mg else (m, v)
 
 
-def ref_step(spec, params, m, v, t, x, y, opt, lr=None):
-    """One reference training step in place; `lr`: this step's rate (a learning-rate schedule's), else opt.lr."""
+def ref_step(spec, params, m, v, t, x, y, opt, lr=None, mg=None, global_step=None):
+    """One reference training step in place; `lr`: this step's rate (a learning-rate schedule's), else opt.lr.
+    `mg`: centered RMSProp's third slot dict (updated in place). `global_step`: AdagradDA's T for this step, by default
+    the returned step count (one worker, starting from step 0)."""
     if lr is not None:
         opt = dataclasses.replace(opt, lr=lr)
     loss, grads, _ = mlp.manual_loss_and_grads(spec, params, x, y)
@@ -86,8 +118,11 @@ def ref_step(spec, params, m, v, t, x, y, opt, lr=None):
         g = grads[k]
         if opt.kind == "sgd":
             params[k] = params[k] - opt.lr * g
+        elif opt.kind == "rmsprop" and opt.centered:
+            params[k], m[k], v[k], mg[k] = tf1_apply(opt, params[k], m[k], v[k], g, mg=mg[k])
         elif opt.kind != "adam":
-            params[k], m[k], v[k] = tf1_apply(opt, params[k], m[k], v[k], g)
+            params[k], m[k], v[k] = tf1_apply(opt, params[k], m[k], v[k], g,
+                                              global_step=t if global_step is None else global_step)
         else:
             m[k] = opt.beta1 * m[k] + (1 - opt.beta1) * g
             v[k] = opt.beta2 * v[k] + (1 - opt.beta2) * g * g

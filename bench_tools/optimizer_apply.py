@@ -1,6 +1,7 @@
 """What each ps optimizer costs in the flagship configuration: Adam, SGD, Momentum, Nesterov momentum, Adagrad,
 RMSProp, Adadelta, FTRL (at lr_power -0.5, the square-root path, and as `ftrl_pow` at -0.25, the general power),
-ProximalAdagrad and ProximalGradientDescent, one after the other, in bench.py's single-GPU setup (ps and worker sharing the GPU, fused engine, default
+ProximalAdagrad, ProximalGradientDescent, centered RMSProp (`rmsprop_centered`) and AdagradDA (which always runs the
+Adagrad family's scheduled serve kernel), one after the other, in bench.py's single-GPU setup (ps and worker sharing the GPU, fused engine, default
 lanes, device-resident data).
 
 Per optimizer, two in-process clusters: one for the device-timed steps/s of `Worker.run_resident` (the serve kernel's
@@ -30,7 +31,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 RULES = ["adam", "sgd", "momentum", "nesterov", "adagrad", "rmsprop", "adadelta", "ftrl", "ftrl_pow", "proximal_adagrad",
-         "proximal_sgd"]
+         "proximal_sgd", "rmsprop_centered", "adagrad_da"]
 
 
 def schedule(kind: str, lr: float):
@@ -52,6 +53,8 @@ def optimizer(rule: str, lr: float, sched: str = "constant", ema=None):
     if rule == "nesterov":
         return OptimizerConfig("momentum", lr, use_nesterov=True, schedule=schedule(sched, lr),
                                moving_average_decay=ema)
+    if rule == "rmsprop_centered":
+        return OptimizerConfig("rmsprop", lr, centered=True, schedule=schedule(sched, lr), moving_average_decay=ema)
     if rule == "ftrl_pow":
         return OptimizerConfig("ftrl", lr, learning_rate_power=-0.25, schedule=schedule(sched, lr),
                                moving_average_decay=ema)

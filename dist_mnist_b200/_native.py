@@ -25,6 +25,7 @@ EPI_TRANSPOSED, EPI_ROWMAJOR_PUSH = 0, 1
 LOSS_BOOK, LOSS_XENT = 0, 1
 OPT_SGD, OPT_ADAM, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3, 4
 OPT_ADADELTA, OPT_FTRL, OPT_PROXIMAL_ADAGRAD, OPT_PROXIMAL_SGD = 5, 6, 7, 8
+OPT_ADAGRAD_DA = 9
 APPLY_PER_PUSH, APPLY_MERGED = 0, 1
 DT_F32, DT_BF16 = 0, 1
 LR_CONSTANT, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_NATURAL_EXP, LR_POLYNOMIAL, LR_COSINE, LR_PIECEWISE = range(7)
@@ -123,6 +124,7 @@ class PsServeParams(C.Structure):
         ("values", C.c_float * (MAX_LR_BOUNDARIES + 1)),
         ("ema", C.c_void_p), ("ema_decay", C.c_float), ("ema_num_updates", C.c_uint32),
         ("l1", C.c_float), ("l2", C.c_float), ("l2_shrinkage", C.c_float), ("lr_power", C.c_float),
+        ("mg", C.c_void_p), ("centered", C.c_uint32), ("pad2_", C.c_uint32),
     ]
 
 

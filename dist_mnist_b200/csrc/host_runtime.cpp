@@ -54,9 +54,10 @@ float prox_shrink_cpu(float prox, float a, float l1, float l2) {
   return num / (1.f + l2 * a);
 }
 
-// TF1 Apply{Momentum,Adagrad,RMSProp,Adadelta,FtrlV2,ProximalAdagrad,ProximalGradientDescent} with IEEE arithmetic and
-// the C library's float functions (ps_apply_sm90.cu tf1_step)
-void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, float& v, float g) {
+// TF1 Apply{Momentum,Adagrad,RMSProp,CenteredRMSProp,Adadelta,FtrlV2,ProximalAdagrad,ProximalGradientDescent,AdagradDA}
+// with IEEE arithmetic and the C library's float functions (ps_apply_sm90.cu tf1_step). `mg`: centered RMSProp's third
+// slot; `da_t`: AdagradDA's global step T in fp32.
+void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, float& v, float& mg, float g, float da_t) {
   if (P.opt == dm::OPT_MOMENTUM) {
     m = P.momentum * m + g;
     if (P.nesterov) p -= g * lr + m * P.momentum * lr;
@@ -64,10 +65,22 @@ void tf1_step_cpu(const dm::PsServeParams& P, float lr, float& p, float& m, floa
   } else if (P.opt == dm::OPT_ADAGRAD) {
     v += g * g;
     p -= lr * g / std::sqrt(v);
+  } else if (P.opt == dm::OPT_RMSPROP && P.centered) {
+    v += (g * g - v) * (1.f - P.decay);
+    mg += (g - mg) * (1.f - P.decay);
+    m = m * P.momentum + (g * lr) / std::sqrt((v - mg * mg) + P.eps);
+    p -= m;
   } else if (P.opt == dm::OPT_RMSPROP) {
     v += (g * g - v) * (1.f - P.decay);
     m = P.momentum * m + lr * g / std::sqrt(v + P.eps);
     p -= m;
+  } else if (P.opt == dm::OPT_ADAGRAD_DA) {   // m = gradient_accumulator, v = gradient_squared_accumulator
+    m += g;
+    v += g * g;
+    if (P.l1 > 0.f)
+      p = -lr * std::copysign(std::fmax(std::fabs(m) - da_t * P.l1, 0.f), m) / (P.l2 * (da_t * lr) + std::sqrt(v));
+    else
+      p = -lr * m / ((da_t * lr) * P.l2 + std::sqrt(v));
   } else if (P.opt == dm::OPT_ADADELTA) {   // v = accum, m = accum_update, rho = P.decay
     v = v * P.decay + g * g * (1.f - P.decay);
     const float upd = std::sqrt(m + P.eps) * (1.f / std::sqrt(v + P.eps)) * g;
@@ -98,6 +111,7 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
   const bool tf1 = P.opt != dm::OPT_ADAM && P.opt != dm::OPT_SGD;
   const bool use_m = dm::opt_uses_m(P.opt);
   const bool use_v = dm::opt_uses_v(P.opt);
+  const bool use_mg = P.opt == dm::OPT_RMSPROP && P.centered;
   // rate of the k-th push of the pass (workers in order), lr(sched_step + k); a merged step uses lr(sched_step)
   float lrs[dm::kMaxWorkers];
   for (int k = 0; k < __builtin_popcount(mask); ++k)
@@ -112,15 +126,17 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
     for (int c = 0; c < it.cols; ++c) {
       const uint64_t a = it.offset + static_cast<uint64_t>(r) * it.ld + c;
       float p = P.params[a];
-      float m = 0.f, v = 0.f, e = 0.f;
+      float m = 0.f, v = 0.f, e = 0.f, mg = 0.f;
       if (use_m) m = P.adam_m[a];
       if (use_v) v = P.adam_v[a];
+      if (use_mg) mg = P.mg[a];
       if (ema) e = P.ema[a];
       float b1p = st.beta1_pow, b2p = st.beta2_pow;
-      // one optimizer step with gradient g at rate lr, then the moving average with 1 - d = omd
-      const auto apply_step = [&](float g, float lr, float omd) {
+      // one optimizer step with gradient g at rate lr whose last push is the k-th of the pass, then the moving average
+      // with 1 - d = omd; AdagradDA's T is sched_step + k + 1
+      const auto apply_step = [&](float g, float lr, float omd, int k) {
         if (tf1) {
-          tf1_step_cpu(P, lr, p, m, v, g);
+          tf1_step_cpu(P, lr, p, m, v, mg, g, static_cast<float>(st.sched_step + static_cast<uint32_t>(k) + 1u));
         } else if (P.opt == dm::OPT_ADAM) {
           b1p *= P.beta1; b2p *= P.beta2;
           const float lr_t = lr * std::sqrt(1.f - b2p) / (1.f - b1p);
@@ -142,12 +158,14 @@ void apply_item_cpu(const dm::PsServeParams& P, const dm::PsItem& it, dm::PsItem
         const float g = P.mailbox[static_cast<uint64_t>(w) * wstride + static_cast<uint64_t>(slot) * P.arena_elems + a];
         if (P.apply_mode == dm::APPLY_MERGED) { gsum += g; continue; }
         const float omd = ema ? ema_omd[k] : 0.f;
-        apply_step(g, lrs[k++], omd);
+        apply_step(g, lrs[k], omd, k);
+        ++k;
       }
-      if (P.apply_mode == dm::APPLY_MERGED) apply_step(gsum, lrs[0], ema ? ema_omd[npush - 1] : 0.f);
+      if (P.apply_mode == dm::APPLY_MERGED) apply_step(gsum, lrs[0], ema ? ema_omd[npush - 1] : 0.f, npush - 1);
       P.params[a] = p;
       if (use_m) P.adam_m[a] = m;
       if (use_v) P.adam_v[a] = v;
+      if (use_mg) P.mg[a] = mg;
       if (ema) P.ema[a] = e;
       if (P.shadow_bf16 != nullptr && (it.flags & 1)) P.shadow_bf16[a] = f32_to_bf16(p);
     }
@@ -179,8 +197,8 @@ void serve_loop(CpuPs* ps) {
       dm::PsItemState ns = st;
       ns.t += nsteps;
       for (int k = 0; k < nsteps; ++k) { ns.beta1_pow *= P.beta1; ns.beta2_pow *= P.beta2; }
-      // one schedule step per push, both apply modes (also the moving averages' num_updates)
-      if (P.lr_schedule != dm::LR_CONSTANT || P.ema != nullptr) ns.sched_step += npush;
+      // one schedule step per push, both apply modes (also the moving averages' num_updates and AdagradDA's T)
+      if (P.lr_schedule != dm::LR_CONSTANT || P.ema != nullptr || P.opt == dm::OPT_ADAGRAD_DA) ns.sched_step += npush;
       P.item_state[item] = ns;
       uint32_t mm = mask;
       while (mm) {

@@ -165,8 +165,10 @@ struct PsItemState {  // persisted across serve-kernel launches and checkpointed
 };
 
 // TF1 `training_ops` rules applied per push (or per round, APPLY_MERGED). Slot buffers: adam_m = Adam m / momentum
-// accumulator / RMSProp mom / Adadelta accum_update / FTRL linear; adam_v = Adam v / Adagrad accumulator / RMSProp ms /
-// Adadelta accum / FTRL accum / ProximalAdagrad accumulator. ProximalGradientDescent has no slot.
+// accumulator / RMSProp mom / Adadelta accum_update / FTRL linear / AdagradDA gradient_accumulator; adam_v = Adam v /
+// Adagrad accumulator / RMSProp ms / Adadelta accum / FTRL accum / ProximalAdagrad accumulator / AdagradDA
+// gradient_squared_accumulator; mg = centered RMSProp's mean gradient (PsServeParams::centered only).
+// ProximalGradientDescent has no slot.
 enum OptimizerKind : int {
   OPT_SGD = 0,
   OPT_ADAM = 1,
@@ -177,14 +179,16 @@ enum OptimizerKind : int {
   OPT_FTRL = 6,
   OPT_PROXIMAL_ADAGRAD = 7,
   OPT_PROXIMAL_SGD = 8,
+  OPT_ADAGRAD_DA = 9,   // runs in the Adagrad family's scheduled / averaging instantiations (T = the item's sched_step)
 };
 // The slot buffers rule `opt` reads and writes (the serve kernel and the CPU serve loop load and store only these).
 constexpr bool opt_uses_m(int opt) {
-  return opt == OPT_ADAM || opt == OPT_MOMENTUM || opt == OPT_RMSPROP || opt == OPT_ADADELTA || opt == OPT_FTRL;
+  return opt == OPT_ADAM || opt == OPT_MOMENTUM || opt == OPT_RMSPROP || opt == OPT_ADADELTA || opt == OPT_FTRL ||
+         opt == OPT_ADAGRAD_DA;
 }
 constexpr bool opt_uses_v(int opt) {
   return opt == OPT_ADAM || opt == OPT_ADAGRAD || opt == OPT_RMSPROP || opt == OPT_ADADELTA || opt == OPT_FTRL ||
-         opt == OPT_PROXIMAL_ADAGRAD;
+         opt == OPT_PROXIMAL_ADAGRAD || opt == OPT_ADAGRAD_DA;
 }
 enum ApplyMode : int {
   APPLY_PER_PUSH = 0,  // reference semantics: every worker push is its own optimizer step
@@ -262,6 +266,12 @@ struct PsServeParams {
   float l2;                    //   the same three: l2_regularization_strength (>= 0)
   float l2_shrinkage;          // OPT_FTRL: l2_shrinkage_regularization_strength (>= 0; 0 = ApplyFtrl, else ApplyFtrlV2)
   float lr_power;              // OPT_FTRL: learning_rate_power (<= 0; -0.5 takes the square-root path)
+  // centered RMSProp (appended, so that no earlier field moves): its third slot, the mean gradient
+  //   mg += (g - mg)(1 - decay) ; mom <- momentum mom + g lr / sqrt((ms - mg^2) + eps)
+  // l1 / l2 above are also OPT_ADAGRAD_DA's strengths
+  float* mg;                   // [arena], null unless centered
+  uint32_t centered;           // OPT_RMSPROP: 1 = centered (TF1 RMSPropOptimizer(centered=True))
+  uint32_t pad2_;
 };
 enum LrScheduleKind : int {
   LR_CONSTANT = 0,

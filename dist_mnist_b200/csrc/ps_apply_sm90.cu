@@ -95,10 +95,12 @@ __device__ __forceinline__ float prox_shrink(float prox, float a, float l1, floa
   const float num = l1 > 0.f ? copysignf(fmaxf(fabsf(prox) - a * l1, 0.f), prox) : prox;
   return div_m<kIeee>(num, fmaf(l2, a, 1.f));
 }
-// kSched: the step's rate is `lr_sched`; else P.lr (read from the parameter block as the measured instantiations do)
+// kSched: the step's rate is `lr_sched`; else P.lr (read from the parameter block as the measured instantiations do).
+// `mg`: centered RMSProp's third slot. `da_t` (kSched): AdagradDA's global step T, the item's applied pushes with this
+// step's included, converted to fp32 once.
 template <int kOpt, bool kIeee, bool kSched>
-__device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, const PsServeParams& P,
-                                         const float& lr_sched) {
+__device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float& mg, float g, const PsServeParams& P,
+                                         const float& lr_sched, float da_t) {
   const float& lr = kSched ? lr_sched : P.lr;
   if constexpr (kOpt == OPT_MOMENTUM) {
     // accum <- momentum accum + g ; p <- p - lr accum  (Nesterov: p <- p - lr g - lr momentum accum)
@@ -106,13 +108,35 @@ __device__ __forceinline__ void tf1_step(float& p, float& m, float& v, float g, 
     if (P.nesterov) p = p - fmaf(g, lr, m * P.momentum * lr);
     else p = fmaf(-lr, m, p);
   } else if constexpr (kOpt == OPT_ADAGRAD) {
-    // accum <- accum + g^2 ; p <- p - lr g / sqrt(accum)   (no epsilon)
-    v = fmaf(g, g, v);
-    p = p - div_sqrt<kIeee>(lr * g, v);
+    bool da = false;
+    if constexpr (kSched) da = P.opt == OPT_ADAGRAD_DA;
+    if (da) {
+      // ApplyAdagradDA (m = gradient_accumulator, v = gradient_squared_accumulator): g_acc <- g_acc + g ;
+      // gg_acc <- gg_acc + g^2 ; p <- -lr sign(g_acc) max(|g_acc| - T l1, 0) / (l2 (T lr) + sqrt(gg_acc))
+      //                              (l1 = 0: -lr g_acc / ((T lr) l2 + sqrt(gg_acc)))
+      m = m + g;
+      v = fmaf(g, g, v);
+      const float tl = da_t * lr;
+      if (P.l1 > 0.f)
+        p = div_m<kIeee>(-lr * copysignf(fmaxf(fabsf(m) - da_t * P.l1, 0.f), m), fmaf(P.l2, tl, sqrt_m<kIeee>(v)));
+      else
+        p = div_m<kIeee>(-lr * m, fmaf(tl, P.l2, sqrt_m<kIeee>(v)));
+    } else {
+      // accum <- accum + g^2 ; p <- p - lr g / sqrt(accum)   (no epsilon)
+      v = fmaf(g, g, v);
+      p = p - div_sqrt<kIeee>(lr * g, v);
+    }
   } else if constexpr (kOpt == OPT_RMSPROP) {
     // ms <- ms + (g^2 - ms)(1 - decay) ; mom <- momentum mom + lr g / sqrt(ms + eps) ; p <- p - mom
+    // centered: mg <- mg + (g - mg)(1 - decay) ; mom <- momentum mom + g lr / sqrt((ms - mg^2) + eps)  (not clamped: a
+    // negative denominator gives NaN, as in TF)
     v = fmaf(fmaf(g, g, -v), 1.f - P.decay, v);
-    m = fmaf(P.momentum, m, div_sqrt<kIeee>(lr * g, v + P.eps));
+    if (P.centered) {
+      mg = fmaf(g - mg, 1.f - P.decay, mg);
+      m = fmaf(P.momentum, m, div_sqrt<kIeee>(g * lr, fmaf(-mg, mg, v) + P.eps));
+    } else {
+      m = fmaf(P.momentum, m, div_sqrt<kIeee>(lr * g, v + P.eps));
+    }
     p = p - m;
   } else if constexpr (kOpt == OPT_ADADELTA) {
     // accum <- rho accum + (1 - rho) g^2 ; update = sqrt(accum_update + eps) rsqrt(accum + eps) g ; p <- p - lr update ;
@@ -169,19 +193,28 @@ struct ResidentState {
   float p[kQuads][4], m[kQuads][4], v[kQuads][4];
   bool loaded;
 };
-// The moving averages of that item (the averaging instantiations), valid whenever ResidentState::loaded is.
-struct ResidentEma {
+// The moving averages of that item (the averaging instantiations) and, in the RMSProp family, centered RMSProp's mean
+// gradients (P.centered), valid whenever ResidentState::loaded is.
+template <int kFam>
+struct ResidentExtra {
   float e[kQuads][4];
+};
+template <>
+struct ResidentExtra<OPT_RMSPROP> {
+  float e[kQuads][4];
+  float g[kQuads][4];
 };
 // Pending pushes whose gradient loads are in flight together, per instantiation: the largest chunk that ptxas compiles
 // without a spill under __launch_bounds__(kPsThreads, 1) (IEEE Adam / SGD at a constant rate keeps the fast one's 8 and
-// spills 28 bytes). Indexed [family row][kIeee][constant rate, scheduled, averaging]; the family rows are Adam / SGD,
-// then OPT_MOMENTUM .. OPT_PROXIMAL_SGD in enum order. 0: no such instantiation (see serve_kernel).
+// spills 28 bytes; four RMSProp entries and the Adagrad family's IEEE scheduled / averaging ones are one below their
+// earlier values, so that centered RMSProp's third slot and AdagradDA fit). Indexed [family row][kIeee][constant rate,
+// scheduled, averaging]; the family rows are Adam / SGD, then OPT_MOMENTUM .. OPT_PROXIMAL_SGD in enum order. 0: no
+// such instantiation (see serve_kernel).
 constexpr int kServeChunk[8][2][3] = {
     {{8, 7, 6}, {8, 6, 5}},   // Adam / SGD
     {{7, 7, 7}, {0, 0, 0}},   // Momentum
-    {{7, 7, 6}, {7, 7, 6}},   // Adagrad
-    {{7, 7, 7}, {7, 7, 6}},   // RMSProp
+    {{7, 7, 6}, {7, 6, 5}},   // Adagrad (the scheduled / averaging ones also run AdagradDA)
+    {{7, 7, 6}, {6, 6, 5}},   // RMSProp (with centered RMSProp's third slot)
     {{7, 8, 6}, {7, 7, 6}},   // Adadelta
     {{8, 8, 6}, {7, 7, 6}},   // FTRL
     {{7, 7, 7}, {7, 7, 5}},   // ProximalAdagrad
@@ -194,24 +227,31 @@ constexpr int serve_family_row(int fam) { return fam == kFamAdamSgd ? 0 : fam - 
 // kEma (the averaging instantiations, which are also kSched): the item's moving averages P.ema stay in registers for
 // the pass like the parameters, and after the optimizer step that ends at position i every element's shadow moves
 // toward the new parameter by 1 - s_ema[i], the pass's decay table (ema_decay(sched_step + i + 1)).
+// The RMSProp family with P.centered also keeps the third slot P.mg (resident beside the others, in res_extra->g);
+// the Adagrad family's scheduled instantiations also run AdagradDA (P.opt), whose T at the step that ends at position i
+// is sched_step + i + 1.
 template <int kFam, bool kIeee, bool kSched, bool kEma>
 __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItemState st, const uint64_t* s_pend,
                            const uint32_t* s_round, const int n_pend, ResidentState* res, const float* s_lr,
-                           const float* s_ema, ResidentEma* res_ema) {
+                           const float* s_ema, ResidentExtra<kFam>* res_extra) {
   const int tid = threadIdx.x;
   const int total = it.rows * it.cols;
   const bool vec = ((it.cols & 3) == 0) && ((it.ld & 3) == 0) && ((it.offset & 3) == 0);
   const int step = vec ? 4 : 1;
   const bool adam = kFam == kFamAdamSgd && P.opt == OPT_ADAM;
   // the slot buffers this rule reads and writes
-  const bool use_m = kFam == kFamAdamSgd ? adam : opt_uses_m(kFam);
+  bool use_m = kFam == kFamAdamSgd ? adam : opt_uses_m(kFam);
   const bool use_v = kFam == kFamAdamSgd ? adam : opt_uses_v(kFam);
+  if constexpr (kFam == OPT_ADAGRAD && kSched) use_m = opt_uses_m(P.opt);   // AdagradDA's gradient_accumulator
+  bool use_mg = false;   // centered RMSProp's mean gradient
+  if constexpr (kFam == OPT_RMSPROP) use_mg = P.centered != 0u;
   const bool merged = P.apply_mode == APPLY_MERGED;
   for (int e0 = tid * step; e0 < total; e0 += kPsThreads * step * kQuads) {
     uint64_t a[kQuads];
     bool ok[kQuads];
     float pv[kQuads][4], mv[kQuads][4], vv[kQuads][4];
     float ev[kQuads][4];   // kEma: the shadows
+    float gv[kQuads][4];   // use_mg: the mean gradients
 #pragma unroll
     for (int q = 0; q < kQuads; ++q) {
       const int e = e0 + q * kPsThreads * step;
@@ -225,6 +265,10 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
         for (int j = 0; j < 4; ++j) ev[q][j] = 0.f;
       }
+      if constexpr (kFam == OPT_RMSPROP) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) gv[q][j] = 0.f;
+      }
     }
     if (res != nullptr && res->loaded) {
       // the item's parameters and Adam slots never left this thread's registers: no load round trip in this pass
@@ -236,7 +280,15 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
         for (int q = 0; q < kQuads; ++q)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) ev[q][j] = res_ema->e[q][j];
+          for (int j = 0; j < 4; ++j) ev[q][j] = res_extra->e[q][j];
+      }
+      if constexpr (kFam == OPT_RMSPROP) {
+        if (use_mg) {
+#pragma unroll
+          for (int q = 0; q < kQuads; ++q)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) gv[q][j] = res_extra->g[q][j];
+        }
       }
     } else {
 #pragma unroll
@@ -257,11 +309,20 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
             const float4 te = __ldcg(reinterpret_cast<const float4*>(P.ema + a[q]));
             ev[q][0] = te.x; ev[q][1] = te.y; ev[q][2] = te.z; ev[q][3] = te.w;
           }
+          if constexpr (kFam == OPT_RMSPROP) {
+            if (use_mg) {
+              const float4 tg = __ldcg(reinterpret_cast<const float4*>(P.mg + a[q]));
+              gv[q][0] = tg.x; gv[q][1] = tg.y; gv[q][2] = tg.z; gv[q][3] = tg.w;
+            }
+          }
         } else {
           pv[q][0] = __ldcg(P.params + a[q]);
           if (use_m) mv[q][0] = __ldcg(P.adam_m + a[q]);
           if (use_v) vv[q][0] = __ldcg(P.adam_v + a[q]);
           if constexpr (kEma) ev[q][0] = __ldcg(P.ema + a[q]);
+          if constexpr (kFam == OPT_RMSPROP) {
+            if (use_mg) gv[q][0] = __ldcg(P.mg + a[q]);
+          }
         }
       }
     }
@@ -319,15 +380,18 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         }
         float ema_omd = 0.f;   // kEma: 1 - d of this step, in fp32 like TF1's `1.0 - decay`
         if constexpr (kEma) ema_omd = 1.f - s_ema[i];
+        float da_t = 0.f;   // AdagradDA: T = pushes applied to the item after this step (TF's static_cast<float>)
+        if constexpr (kFam == OPT_ADAGRAD && kSched) da_t = static_cast<float>(st.sched_step + static_cast<uint32_t>(i) + 1u);
 #pragma unroll
         for (int q = 0; q < kQuads; ++q) {
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             if (j >= step) continue;
-            const float gv = merged ? gsum[q][j] : g[ci][q][j];
-            if constexpr (kFam != kFamAdamSgd) tf1_step<kFam, kIeee, kSched>(pv[q][j], mv[q][j], vv[q][j], gv, P, lr);
-            else if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gv, lr_t, P.beta1, P.beta2, P.eps);
-            else pv[q][j] = fmaf(-lr, gv, pv[q][j]);
+            const float gr = merged ? gsum[q][j] : g[ci][q][j];
+            if constexpr (kFam != kFamAdamSgd)
+              tf1_step<kFam, kIeee, kSched>(pv[q][j], mv[q][j], vv[q][j], gv[q][j], gr, P, lr, da_t);
+            else if (adam) adam_step<kIeee>(pv[q][j], mv[q][j], vv[q][j], gr, lr_t, P.beta1, P.beta2, P.eps);
+            else pv[q][j] = fmaf(-lr, gr, pv[q][j]);
             // assign_moving_average: shadow -= (shadow - p) * (1 - d), each op rounded as TF1's graph does
             if constexpr (kEma) ev[q][j] = ev[q][j] - __fmul_rn(ev[q][j] - pv[q][j], ema_omd);
             if (merged) gsum[q][j] = 0.f;
@@ -344,7 +408,15 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
 #pragma unroll
         for (int q = 0; q < kQuads; ++q)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) res_ema->e[q][j] = ev[q][j];
+          for (int j = 0; j < 4; ++j) res_extra->e[q][j] = ev[q][j];
+      }
+      if constexpr (kFam == OPT_RMSPROP) {
+        if (use_mg) {
+#pragma unroll
+          for (int q = 0; q < kQuads; ++q)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) res_extra->g[q][j] = gv[q][j];
+        }
       }
       res->loaded = true;
     }
@@ -357,6 +429,9 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         if (use_m) *reinterpret_cast<float4*>(P.adam_m + a[q]) = make_float4(mv[q][0], mv[q][1], mv[q][2], mv[q][3]);
         if (use_v) *reinterpret_cast<float4*>(P.adam_v + a[q]) = make_float4(vv[q][0], vv[q][1], vv[q][2], vv[q][3]);
         if constexpr (kEma) *reinterpret_cast<float4*>(P.ema + a[q]) = make_float4(ev[q][0], ev[q][1], ev[q][2], ev[q][3]);
+        if constexpr (kFam == OPT_RMSPROP) {
+          if (use_mg) *reinterpret_cast<float4*>(P.mg + a[q]) = make_float4(gv[q][0], gv[q][1], gv[q][2], gv[q][3]);
+        }
         if (shadow) {
           __nv_bfloat162 lo = __floats2bfloat162_rn(pv[q][0], pv[q][1]);
           __nv_bfloat162 hi = __floats2bfloat162_rn(pv[q][2], pv[q][3]);
@@ -370,6 +445,9 @@ __device__ void apply_item(const PsServeParams& P, const PsItem it, const PsItem
         if (use_m) P.adam_m[a[q]] = mv[q][0];
         if (use_v) P.adam_v[a[q]] = vv[q][0];
         if constexpr (kEma) P.ema[a[q]] = ev[q][0];
+        if constexpr (kFam == OPT_RMSPROP) {
+          if (use_mg) P.mg[a[q]] = gv[q][0];
+        }
         if (shadow) {
           __nv_bfloat16 b = __float2bfloat16(pv[q][0]);
           P.shadow_bf16[a[q]] = *reinterpret_cast<uint16_t*>(&b);
@@ -431,7 +509,7 @@ __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_co
   // the parameters, checkpoints read the slots — but the three load round trips (~1 us of a ~6.7 us pass) are gone.
   ResidentState resident;
   resident.loaded = false;
-  ResidentEma resident_ema;   // kEma: the shadows beside them
+  ResidentExtra<kFam> resident_extra;   // beside them: the shadows (kEma), centered RMSProp's mean gradients
   bool use_resident = false;
   if (n_own == 1) {
     const PsItem it0 = s_item[0];
@@ -493,7 +571,7 @@ __global__ void __launch_bounds__(kPsThreads, 1) ps_serve_kernel(const __grid_co
         const PsItemState st = s_state[own];
         apply_item<kFam, kIeee, kSched, kEma>(P, s_item[own], st, s_pend, s_round, static_cast<int>(s_npend),
                                               use_resident ? &resident : nullptr, s_lr, s_ema,
-                                              use_resident ? &resident_ema : nullptr);
+                                              use_resident ? &resident_extra : nullptr);
         __syncthreads();   // every thread's parameter stores precede warp 0's release operations below
         const long long c2 = stats_on ? clock64() : 0;
         if (stats_on) {
@@ -598,6 +676,8 @@ ServeKernel serve_kernel(int opt, bool ieee, bool sched, bool ema) {
     case OPT_ADAM: return serve_kernel_of<kFamAdamSgd>(ieee, sched, ema);
     case OPT_MOMENTUM: return serve_kernel_of<OPT_MOMENTUM>(ieee, sched, ema);
     case OPT_ADAGRAD: return serve_kernel_of<OPT_ADAGRAD>(ieee, sched, ema);
+    // AdagradDA's T is the item's sched_step, which only the scheduled and averaging instantiations advance
+    case OPT_ADAGRAD_DA: return serve_kernel_of<OPT_ADAGRAD>(ieee, true, ema);
     case OPT_RMSPROP: return serve_kernel_of<OPT_RMSPROP>(ieee, sched, ema);
     case OPT_ADADELTA: return serve_kernel_of<OPT_ADADELTA>(ieee, sched, ema);
     case OPT_FTRL: return serve_kernel_of<OPT_FTRL>(ieee, sched, ema);
@@ -731,7 +811,7 @@ namespace dm {
 cudaError_t preload_ps_kernels() {
   cudaFuncAttributes a;
   cudaError_t e;
-  for (int opt = OPT_SGD; opt <= OPT_PROXIMAL_SGD; ++opt)
+  for (int opt = OPT_SGD; opt <= OPT_ADAGRAD_DA; ++opt)
     for (const bool ieee : {false, true})
       for (const bool sched : {false, true})
         for (const bool ema : {false, true})

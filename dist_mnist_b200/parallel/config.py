@@ -20,10 +20,13 @@ def _env_flag(name: str, default: bool) -> bool:
 
 _NATIVE_KINDS = {"adam": N.OPT_ADAM, "sgd": N.OPT_SGD, "momentum": N.OPT_MOMENTUM, "adagrad": N.OPT_ADAGRAD,
                  "rmsprop": N.OPT_RMSPROP, "adadelta": N.OPT_ADADELTA, "ftrl": N.OPT_FTRL,
-                 "proximal_adagrad": N.OPT_PROXIMAL_ADAGRAD, "proximal_sgd": N.OPT_PROXIMAL_SGD}
+                 "proximal_adagrad": N.OPT_PROXIMAL_ADAGRAD, "proximal_sgd": N.OPT_PROXIMAL_SGD,
+                 "adagrad_da": N.OPT_ADAGRAD_DA}
 # the kinds after Adam / SGD: their slot buffers hold other state, so ps, chief and checkpoints must agree on the kind
-TF1_SLOT_KINDS = ("momentum", "adagrad", "rmsprop", "adadelta", "ftrl", "proximal_adagrad", "proximal_sgd")
+TF1_SLOT_KINDS = ("momentum", "adagrad", "rmsprop", "adadelta", "ftrl", "proximal_adagrad", "proximal_sgd",
+                  "adagrad_da")
 _PROXIMAL = ("ftrl", "proximal_adagrad", "proximal_sgd")
+_L1_L2 = _PROXIMAL + ("adagrad_da",)   # the kinds with l1 / l2 regularization strengths
 _FTRL_PROX_HPARAMS = ("rho", "l1_regularization_strength", "l2_regularization_strength",
                       "l2_shrinkage_regularization_strength", "learning_rate_power")
 # hyper-parameters beyond lr / beta1 / beta2 / eps, the kinds that use each, and the TF1 default per kind
@@ -31,10 +34,10 @@ _FTRL_PROX_HPARAMS = ("rho", "l1_regularization_strength", "l2_regularization_st
 _EXTRA_DEFAULTS = {
     "momentum": {"momentum": 0.9, "rmsprop": 0.0},
     "decay": {"rmsprop": 0.9},
-    "initial_accumulator_value": {"adagrad": 0.1, "ftrl": 0.1, "proximal_adagrad": 0.1},
+    "initial_accumulator_value": {"adagrad": 0.1, "ftrl": 0.1, "proximal_adagrad": 0.1, "adagrad_da": 0.1},
     "rho": {"adadelta": 0.95},
-    "l1_regularization_strength": {k: 0.0 for k in _PROXIMAL},
-    "l2_regularization_strength": {k: 0.0 for k in _PROXIMAL},
+    "l1_regularization_strength": {k: 0.0 for k in _L1_L2},
+    "l2_regularization_strength": {k: 0.0 for k in _L1_L2},
     "l2_shrinkage_regularization_strength": {"ftrl": 0.0},
     "learning_rate_power": {"ftrl": -0.5},
 }
@@ -314,12 +317,14 @@ class OptimizerConfig:
     north-star "async-SGD" variant. "momentum", "adagrad" and "rmsprop" are TF1's `MomentumOptimizer`,
     `AdagradOptimizer` and (non-centered) `RMSPropOptimizer`, applied on the ps with the `training_ops` formulas;
     "adadelta", "ftrl", "proximal_adagrad" and "proximal_sgd" likewise are `AdadeltaOptimizer`, `FtrlOptimizer` (V2
-    when l2_shrinkage_regularization_strength > 0), `ProximalAdagradOptimizer` and `ProximalGradientDescentOptimizer`.
-    Their l1 / l2 strengths are the ps-side proximal terms of those optimizers, not the worker-side loss term `l2`.
+    when l2_shrinkage_regularization_strength > 0), `ProximalAdagradOptimizer` and `ProximalGradientDescentOptimizer`,
+    and "adagrad_da" is `AdagradDAOptimizer`, whose global step T is the ps's count of pushes applied to each variable.
+    Their l1 / l2 strengths are the ps-side terms of those optimizers, not the worker-side loss term `l2`.
+    `centered` is RMSPropOptimizer(centered=True), which keeps a third slot (the mean gradient, `uses_mg`).
 
     A hyper-parameter left at None takes the kind's TF1 default; giving one that the kind does not use is an error."""
     kind: str = "adam"          # "adam" | "sgd" | "momentum" | "adagrad" | "rmsprop" | "adadelta" | "ftrl" |
-                                # "proximal_adagrad" | "proximal_sgd"
+                                # "proximal_adagrad" | "proximal_sgd" | "adagrad_da"
     lr: float = 1e-4            # --learning_rate default (DS:15)
     beta1: float = 0.9
     beta2: float = 0.999
@@ -331,12 +336,13 @@ class OptimizerConfig:
                                 # Adam). The cpu backend is always IEEE.
     momentum: Optional[float] = None    # "momentum" (0.9), "rmsprop" (0.0)
     use_nesterov: bool = False          # "momentum"
+    centered: bool = False              # "rmsprop": normalise by the variance estimate ms - mg^2 (a third slot, mg)
     decay: Optional[float] = None       # "rmsprop" (0.9)
-    initial_accumulator_value: Optional[float] = None   # "adagrad", "ftrl", "proximal_adagrad" (0.1): the
-                                                        # accumulator slot starts here, not at 0
+    initial_accumulator_value: Optional[float] = None   # "adagrad", "ftrl", "proximal_adagrad", "adagrad_da" (0.1):
+                                                        # the (squared) accumulator slot starts here, not at 0
     rho: Optional[float] = None                         # "adadelta" (0.95)
-    l1_regularization_strength: Optional[float] = None  # "ftrl", "proximal_adagrad", "proximal_sgd" (0.0)
-    l2_regularization_strength: Optional[float] = None  # the same three (0.0)
+    l1_regularization_strength: Optional[float] = None  # "ftrl", "proximal_adagrad", "proximal_sgd", "adagrad_da" (0.0)
+    l2_regularization_strength: Optional[float] = None  # the same four (0.0)
     l2_shrinkage_regularization_strength: Optional[float] = None   # "ftrl" (0.0; > 0: ApplyFtrlV2)
     learning_rate_power: Optional[float] = None         # "ftrl" (-0.5)
     schedule: LrSchedule = LrSchedule()   # learning-rate schedule over the global step (default: constant `lr`)
@@ -364,14 +370,18 @@ class OptimizerConfig:
                 raise ValueError(f"optimizer {self.kind!r} has no hyper-parameter {name!r}")
         if self.use_nesterov and self.kind != "momentum":
             raise ValueError(f"use_nesterov applies to the momentum optimizer, not {self.kind!r}")
-        if self.kind in ("adagrad", "proximal_adagrad") and not self.initial_accumulator_value > 0:
+        if not isinstance(self.centered, bool):
+            raise ValueError(f"centered must be a bool, got {self.centered!r}")
+        if self.centered and self.kind != "rmsprop":
+            raise ValueError(f"centered applies to the rmsprop optimizer, not {self.kind!r}")
+        if self.kind in ("adagrad", "proximal_adagrad", "adagrad_da") and not self.initial_accumulator_value > 0:
             raise ValueError(f"initial_accumulator_value must be positive ({self.kind} divides by its square root)")
-        if self.kind in ("adadelta",) + _PROXIMAL:   # every hyper-parameter finite
-            for name in ("lr", "eps", "initial_accumulator_value") + _FTRL_PROX_HPARAMS:
+        if self.kind in ("adadelta", "adagrad_da") + _PROXIMAL or self.centered:   # every hyper-parameter finite
+            for name in ("lr", "eps", "initial_accumulator_value", "momentum", "decay") + _FTRL_PROX_HPARAMS:
                 x = getattr(self, name)
                 if x is not None and (isinstance(x, bool) or not isinstance(x, (int, float)) or not math.isfinite(x)):
                     raise ValueError(f"{name} must be a finite number, got {x!r}")
-            if self.kind != "adadelta" and not self.lr > 0:   # TF's Apply{Ftrl,Proximal*} kernels: "lr is not positive"
+            if self.kind in _PROXIMAL and not self.lr > 0:   # TF's Apply{Ftrl,Proximal*} kernels: "lr is not positive"
                 raise ValueError(f"optimizer {self.kind!r} needs a positive learning rate, got {self.lr!r}")
         for name in ("l1_regularization_strength", "l2_regularization_strength", "l2_shrinkage_regularization_strength"):
             if getattr(self, name) is not None and getattr(self, name) < 0:
@@ -420,11 +430,17 @@ class OptimizerConfig:
             return _NATIVE_KINDS[self.kind]
         raise ValueError(f"unknown optimizer {self.kind!r} ({' | '.join(_NATIVE_KINDS)})")
 
+    @property
+    def uses_mg(self) -> bool:
+        """Whether the rule has the third slot buffer "mg" (centered RMSProp's mean gradient, which starts at 0)."""
+        return self.kind == "rmsprop" and self.centered
+
     def slot_init(self) -> Tuple[float, float]:
         """Initial values of the two slot buffers (adam_m, adam_v): the accumulator of Adagrad, FTRL and
-        ProximalAdagrad starts at initial_accumulator_value and RMSProp's ms at 1 (TF1's `ones_initializer`); every
-        other slot (FTRL's linear, both of Adadelta's) at 0."""
-        if self.kind in ("adagrad", "ftrl", "proximal_adagrad"):
+        ProximalAdagrad and AdagradDA's squared accumulator start at initial_accumulator_value and RMSProp's ms at 1
+        (TF1's `ones_initializer`); every other slot (FTRL's linear, both of Adadelta's, AdagradDA's gradient
+        accumulator, centered RMSProp's mg) at 0."""
+        if self.kind in ("adagrad", "ftrl", "proximal_adagrad", "adagrad_da"):
             return 0.0, float(self.initial_accumulator_value)
         if self.kind == "rmsprop":
             return 0.0, 1.0
@@ -432,7 +448,7 @@ class OptimizerConfig:
 
     def fill_native_rule(self, P) -> None:
         """Write the rule's hyper-parameters beyond lr / beta1 / beta2 / eps into a PsServeParams (Adadelta's rho rides
-        in `decay`)."""
+        in `decay`). The mg slot's pointer is the caller's."""
         P.momentum = self.momentum or 0.0
         P.decay = self.rho if self.kind == "adadelta" else (self.decay or 0.0)
         P.nesterov = int(self.use_nesterov)
@@ -440,6 +456,7 @@ class OptimizerConfig:
         P.l2 = self.l2_regularization_strength or 0.0
         P.l2_shrinkage = self.l2_shrinkage_regularization_strength or 0.0
         P.lr_power = self.learning_rate_power or 0.0
+        P.centered = int(self.centered)
 
     def as_dict(self) -> dict:
         d = asdict(self)

@@ -59,10 +59,12 @@ def serve_geometry(n_items: int, ps_ctas: int, shares_gpu: bool, engine: str) ->
     return n, 1
 
 
-def shard_carver(shard: ShardLayout, n_workers: int, nslots: int, moving_averages: bool = False) -> Carver:
+def shard_carver(shard: ShardLayout, n_workers: int, nslots: int, moving_averages: bool = False,
+                 centered: bool = False) -> Carver:
     """Byte layout of one PS shard segment (both sides derive pointers from the exported table). `moving_averages`:
-    the shadow variables of ExponentialMovingAverage (region "ema", last and empty when off, so that no other region
-    moves)."""
+    the shadow variables of ExponentialMovingAverage (region "ema", empty when off). `centered`: centered RMSProp's
+    third slot, the mean gradient (region "mg" after "ema", empty when off). Both come last, so that no other region
+    moves."""
     a = shard.arena_elems
     ni = max(shard.n_items, 1)
     nf = max(shard.n_flags, 1)
@@ -81,6 +83,7 @@ def shard_carver(shard: ShardLayout, n_workers: int, nslots: int, moving_average
     c.add("inbox_table", N.MAX_WORKERS * 8)
     c.add("stats", PS_STATS_CTAS * 9 * 8)   # per-CTA serve statistics and SM ids (DM_PS_STATS=1)
     c.add("ema", a * 4 if moving_averages else 0)
+    c.add("mg", a * 4 if centered else 0)
     return c
 
 
@@ -119,7 +122,7 @@ class ParameterServer:
         kind = "cuda" if cfg.backend == "cuda" else "shm"
         if kind == "cuda":
             N.check(self.lib.dm_set_device(self.device), "set device")
-        carver = shard_carver(self.shard, self.n_workers, cfg.nslots, opt.moving_averages)
+        carver = shard_carver(self.shard, self.n_workers, cfg.nslots, opt.moving_averages, opt.uses_mg)
         self.seg = Segment.create(kind, carver.total, device=self.device, table=carver.table(), tag=f"ps{task_index}")
         self._init_tables()
         desc = self.seg.export()
@@ -173,7 +176,8 @@ class ParameterServer:
         P.oneshot = 0
         P.opt, P.apply_mode = opt.native_kind, cfg.native_apply_mode
         P.lr, P.beta1, P.beta2, P.eps = opt.lr, opt.beta1, opt.beta2, opt.eps
-        opt.fill_native_rule(P)   # momentum, decay (Adadelta's rho), nesterov, l1, l2, l2_shrinkage, lr_power
+        opt.fill_native_rule(P)   # momentum, decay (Adadelta's rho), nesterov, l1, l2, l2_shrinkage, lr_power, centered
+        P.mg = s.addr("mg") if opt.uses_mg else None   # centered RMSProp's third slot
         opt.schedule.fill_native(P)   # non-constant: the scheduled serve kernels / the cpu loop's rate table
         P.ieee_math = 1 if opt.math == "ieee" else 0
         # moving averages: the averaging serve kernels / the cpu loop's shadow update

@@ -394,11 +394,17 @@ class Worker:
             raise ValueError("moving averages are off in this run (OptimizerConfig.moving_average_decay is None / "
                              "no --moving_average_decay): there are no shadow variables")
 
-    def write_variables(self, params: Dict[str, torch.Tensor], region: str = "params") -> None:
-        """Write variables into a region of the ps shards: "params", the slots "adam_m" / "adam_v", or "ema" (the
-        moving averages, only when they are on)."""
+    def _require_region(self, region: str) -> None:
         if region == "ema":
             self._require_moving_averages()
+        elif region == "mg" and not self.opt.uses_mg:
+            raise ValueError(f"optimizer {self.opt.kind!r} (centered={self.opt.centered}) has no mg slot: only "
+                             "rmsprop with centered=True / --centered keeps one")
+
+    def write_variables(self, params: Dict[str, torch.Tensor], region: str = "params") -> None:
+        """Write variables into a region of the ps shards: "params", the slots "adam_m" / "adam_v", "mg" (centered
+        RMSProp's third slot, only when centered), or "ema" (the moving averages, only when they are on)."""
+        self._require_region(region)
         for name, t in params.items():
             vl = self.layout.by_name[name]
             if tuple(t.shape) != tuple(vl.spec.shape):
@@ -412,8 +418,7 @@ class Worker:
 
     def read_variables(self, region: str = "params") -> Dict[str, torch.Tensor]:
         """Every variable, [out, in] / [out], from a region of the ps shards (see write_variables)."""
-        if region == "ema":
-            self._require_moving_averages()
+        self._require_region(region)
         out = {}
         for name, vl in self.layout.by_name.items():
             if len({(pc.ps, pc.offset) for pc in vl.pieces}) == 1:   # one owner (whole variable, or all slices there)
@@ -471,6 +476,8 @@ class Worker:
         m0, v0 = self.opt.slot_init()   # Adagrad's accumulator and RMSProp's ms do not start at 0
         self.write_variables({k: torch.full_like(v, m0) for k, v in params.items()}, "adam_m")
         self.write_variables({k: torch.full_like(v, v0) for k, v in params.items()}, "adam_v")
+        if self.opt.uses_mg:   # centered RMSProp's mean gradient starts at 0
+            self.write_variables({k: torch.zeros_like(v) for k, v in params.items()}, "mg")
         if self.opt.moving_averages:   # shadows start at the initial values (TF1 slot_creator, initialized_value())
             self.write_variables(params, "ema")
         self.rdv.put("init/done", {"seed": seed, "by": self.task_index})

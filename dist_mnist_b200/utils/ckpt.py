@@ -52,6 +52,9 @@ def save_checkpoint(worker, directory: str) -> str:
     }
     if worker.opt.moving_averages:   # the shadow variables (TF1 saves `<var>/ExponentialMovingAverage`)
         state["ema"] = worker.read_variables("ema")
+    if worker.opt.uses_mg:   # centered RMSProp's third slot (TF1 saves its `mg` slot variables)
+        state["optimizer"]["centered"] = True
+        state["mg"] = worker.read_variables("mg")
     name = f"model.ckpt-{gstep}.pt"
     path = os.path.join(directory, name)
     tmp = path + ".tmp"
@@ -100,11 +103,16 @@ def restore_latest(worker, directory: Optional[str]) -> Optional[int]:
     if worker.opt.moving_averages and "ema" not in state:
         raise RuntimeError(f"checkpoint {path} has no moving averages, this run keeps them "
                            f"(moving_average_decay={worker.opt.moving_average_decay})")
+    # centered RMSProp's mg slot follows the same rule: a centered run needs it, any other run ignores a saved one
+    if worker.opt.uses_mg and "mg" not in state:
+        raise RuntimeError(f"checkpoint {path} has no centered RMSProp mg slot, this run is centered")
     worker.write_variables(state["variables"], "params")
     worker.write_variables(state["adam_m"], "adam_m")
     worker.write_variables(state["adam_v"], "adam_v")
     if worker.opt.moving_averages:
         worker.write_variables(state["ema"], "ema")
+    if worker.opt.uses_mg:
+        worker.write_variables(state["mg"], "mg")
     # per-item optimizer state (Adam step count / beta powers) is only meaningful for the same item table; with a
     # different shard count, placement or dW tile width the variables and Adam slots are restored and the
     # per-item step counters restart (bias correction re-warms, as after a TF slot-variable reset)
