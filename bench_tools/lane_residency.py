@@ -57,7 +57,8 @@ def run(lanes: int, steps: int, warmup: int, batch: int, dev: int = 0, clip=None
     lib = N.lib()
     N.ensure_prepared(dev)
     max_lanes = C.c_int(0)
-    N.check(lib.dm_fused_max_lanes(dev, batch, C.byref(max_lanes)), "fused occupancy")
+    N.check(lib.dm_fused_max_lanes(dev, batch, int(opt.clip.enabled), int(opt.l2.enabled),
+                                   mlp.activation_code(spec.activation), C.byref(max_lanes)), "fused occupancy")
 
     ds = data_utils.synthetic_mnist(data_utils.TRAIN_SIZE, seed=0)
     dev_x = ds.images.to(torch.float32).to(f"cuda:{dev}").contiguous()

@@ -305,10 +305,7 @@ def _declare(l: C.CDLL) -> None:
         "dm_exec_kernel_launches": (u64, [vp]),
         "dm_exec_destroy": (i, [vp]),
         "dm_launch_fused": (i, [vp, vp, i, vp]),
-        "dm_fused_max_lanes": (i, [i, i, C.POINTER(i)]),
-        "dm_fused_max_lanes_clip": (i, [i, i, C.POINTER(i)]),
-        "dm_fused_max_lanes_l2": (i, [i, i, i, C.POINTER(i)]),
-        "dm_fused_max_lanes_for": (i, [i, i, i, i, i, C.POINTER(i)]),
+        "dm_fused_max_lanes": (i, [i, i, i, i, i, C.POINTER(i)]),
         "dm_launch_grad_clip": (i, [C.c_void_p, i, C.c_void_p]),
         "dm_fused_smem_bytes": (i, [i]),
         "dm_nvls_probe": (i, [i, sz, i, C.c_char_p, sz]),

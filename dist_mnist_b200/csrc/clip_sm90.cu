@@ -152,13 +152,24 @@ __global__ void __launch_bounds__(kClipThreads) grad_clip_release_kernel(const _
   }
 }
 
-cudaError_t preload_grad_clip_kernels() {
+using GradClipKernel = void (*)(const GradClipParams);
+
+// The kernel of clip stage `stage` (0 sums of squares, 1 clip into the mailbox, 2 flags), with or without the L2 term;
+// null for an unknown stage.
+static GradClipKernel grad_clip_kernel(int stage, bool l2) {
+  if (stage == 0 || stage == 1) {
+    if (!l2) return stage == 0 ? grad_clip_ssq_kernel<false> : grad_clip_apply_kernel<false>;
+    return stage == 0 ? grad_clip_ssq_kernel<true> : grad_clip_apply_kernel<true>;
+  }
+  return stage == 2 ? grad_clip_release_kernel : nullptr;
+}
+
+cudaError_t prepare_grad_clip_kernels() {
   cudaFuncAttributes a;
-  cudaError_t e = cudaFuncGetAttributes(&a, grad_clip_ssq_kernel<false>);   // force-load (see preload_ps_kernels)
-  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_apply_kernel<false>);
-  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_ssq_kernel<true>);
-  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_clip_apply_kernel<true>);
-  return e != cudaSuccess ? e : cudaFuncGetAttributes(&a, grad_clip_release_kernel);
+  for (const bool l2 : {false, true})
+    for (const int stage : {0, 1})
+      if (cudaError_t e = cudaFuncGetAttributes(&a, grad_clip_kernel(stage, l2)); e != cudaSuccess) return e;
+  return cudaFuncGetAttributes(&a, grad_clip_kernel(2, false));
 }
 
 cudaError_t launch_grad_clip(const GradClipParams& p, int stage, cudaStream_t stream) {
@@ -167,17 +178,9 @@ cudaError_t launch_grad_clip(const GradClipParams& p, int stage, cudaStream_t st
       p.nslots < 1 || p.kind < (l2 ? CLIP_OFF : CLIP_GLOBAL_NORM) || p.kind > CLIP_VALUE ||
       !(p.l2_scale >= 0.f && p.l2_scale < INFINITY) || (l2 && (p.l2_partials == nullptr || p.result == nullptr)))
     return cudaErrorInvalidValue;
-  if (stage == 0) {
-    if (l2) grad_clip_ssq_kernel<true><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
-    else grad_clip_ssq_kernel<false><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
-  } else if (stage == 1) {
-    if (l2) grad_clip_apply_kernel<true><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
-    else grad_clip_apply_kernel<false><<<kClipBlocks, kClipThreads, 0, stream>>>(p);
-  } else if (stage == 2) {
-    grad_clip_release_kernel<<<1, kClipThreads, 0, stream>>>(p);
-  } else {
-    return cudaErrorInvalidValue;
-  }
+  const GradClipKernel k = grad_clip_kernel(stage, l2);
+  if (k == nullptr) return cudaErrorInvalidValue;
+  k<<<stage == 2 ? 1 : kClipBlocks, kClipThreads, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -48,6 +48,17 @@ inline int device_sm_count() {
   return n;
 }
 
+// One entry per translation unit: opt its kernels into their dynamic shared memory where they need it and force-load
+// every kernel its launchers can pick, so that no first launch needs a lazy load while a persistent serve kernel is
+// resident (DESIGN §7). dm_prepare_kernels calls each once per device.
+cudaError_t prepare_gemm_kernels();
+cudaError_t prepare_head_kernels();
+cudaError_t prepare_grad_clip_kernels();
+cudaError_t prepare_ps_kernels();
+cudaError_t prepare_p2p_kernels();
+cudaError_t prepare_fused_kernels();
+cudaError_t prepare_nvls_kernels();
+
 // ------------------------------------------------------------------------------------------
 // mbarrier
 // ------------------------------------------------------------------------------------------

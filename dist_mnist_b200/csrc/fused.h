@@ -16,13 +16,11 @@ struct FusedMaps {
 };
 
 // Batch B <= 32 runs the one-tile instantiation of the kernel, 32 < B <= 256 the multi-tile one; the functions that
-// take B answer for the instantiation that batch runs.
-cudaError_t prepare_fused_kernel();   // every instantiation: shared-memory opt-in + force-load
+// take B answer for the instantiation that batch runs, with (clip) or without gradient clipping, with (l2) or without
+// L2 regularization, under activation `act` (ActivationKind).
 size_t fused_smem_bytes(int B);
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream);
-cudaError_t fused_max_lanes(int B, int* out);
-cudaError_t fused_max_lanes_clip(int B, int* out);   // the same for the gradient-clipping instantiations
-// ... with or without clip / L2, under activation `act` (ActivationKind)
-cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int act, int* out);
+// how many clusters of that instantiation can be co-resident on the device (upper bound for `lanes`)
+cudaError_t fused_max_lanes(int B, bool clip, bool l2, int act, int* out);
 
 }  // namespace dm

@@ -1062,35 +1062,6 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-template <int kMaxTiles, bool kClip, bool kL2, bool kAct>
-static cudaError_t prepare_fused_instance() {
-  cudaError_t e = cudaFuncSetAttribute(fused_step_kernel<kMaxTiles, kClip, kL2, kAct>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(fs_smem_bytes<kMaxTiles>()));
-  if (e != cudaSuccess) return e;
-  cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, fused_step_kernel<kMaxTiles, kClip, kL2, kAct>);   // force-load (see preload_ps_kernels)
-}
-
-template <bool kClip, bool kL2, bool kAct>
-static cudaError_t prepare_fused_pair() {
-  cudaError_t e = prepare_fused_instance<1, kClip, kL2, kAct>();
-  return e != cudaSuccess ? e : prepare_fused_instance<kFsMaxTiles, kClip, kL2, kAct>();
-}
-
-template <bool kAct>
-static cudaError_t prepare_fused_act() {
-  cudaError_t e = prepare_fused_pair<false, false, kAct>();
-  if (e == cudaSuccess) e = prepare_fused_pair<true, false, kAct>();
-  if (e == cudaSuccess) e = prepare_fused_pair<false, true, kAct>();
-  return e != cudaSuccess ? e : prepare_fused_pair<true, true, kAct>();
-}
-
-cudaError_t prepare_fused_kernel() {
-  cudaError_t e = prepare_fused_act<false>();
-  return e != cudaSuccess ? e : prepare_fused_act<true>();
-}
-
 static bool fused_multi_tile(int B) { return B > 32; }
 
 size_t fused_smem_bytes(int B) { return fused_multi_tile(B) ? fs_smem_bytes<kFsMaxTiles>() : fs_smem_bytes<1>(); }
@@ -1113,21 +1084,36 @@ static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t str
 
 using FusedKernel = void (*)(const FusedMaps, const FusedParams);
 
-template <bool kAct>
-static FusedKernel fused_kernel_act(bool multi, bool clip, bool l2) {
-  if (l2) {
-    if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, true, kAct> : fused_step_kernel<1, true, true, kAct>;
-    return multi ? fused_step_kernel<kFsMaxTiles, false, true, kAct> : fused_step_kernel<1, false, true, kAct>;
-  }
-  if (clip) return multi ? fused_step_kernel<kFsMaxTiles, true, false, kAct> : fused_step_kernel<1, true, false, kAct>;
-  return multi ? fused_step_kernel<kFsMaxTiles, false, false, kAct> : fused_step_kernel<1, false, false, kAct>;
+// The instantiation that runs batch B, with or without the clip and the L2 term, under activation `act`
+// (ActivationKind; ACT_NONE, the value of a zero-initialised FusedParams, and ACT_RELU run the ReLU instantiations).
+static FusedKernel fused_kernel(int B, bool clip, bool l2, int act) {
+  static const FusedKernel table[2][2][2][2] = {   // [act > ACT_RELU][l2][clip][multi-tile], in load order
+      {{{fused_step_kernel<1, false, false, false>, fused_step_kernel<kFsMaxTiles, false, false, false>},
+        {fused_step_kernel<1, true, false, false>, fused_step_kernel<kFsMaxTiles, true, false, false>}},
+       {{fused_step_kernel<1, false, true, false>, fused_step_kernel<kFsMaxTiles, false, true, false>},
+        {fused_step_kernel<1, true, true, false>, fused_step_kernel<kFsMaxTiles, true, true, false>}}},
+      {{{fused_step_kernel<1, false, false, true>, fused_step_kernel<kFsMaxTiles, false, false, true>},
+        {fused_step_kernel<1, true, false, true>, fused_step_kernel<kFsMaxTiles, true, false, true>}},
+       {{fused_step_kernel<1, false, true, true>, fused_step_kernel<kFsMaxTiles, false, true, true>},
+        {fused_step_kernel<1, true, true, true>, fused_step_kernel<kFsMaxTiles, true, true, true>}}}};
+  return table[act > ACT_RELU][l2][clip][fused_multi_tile(B)];
 }
 
-// The instantiation batch B runs with or without the clip and the L2 term, under activation `act` (ACT_NONE, the
-// value of a zero-initialised FusedParams, and ACT_RELU run the ReLU instantiations).
-static FusedKernel fused_kernel_for(int B, bool clip, bool l2, int act) {
-  const bool multi = fused_multi_tile(B);
-  return act > ACT_RELU ? fused_kernel_act<true>(multi, clip, l2) : fused_kernel_act<false>(multi, clip, l2);
+// Every instantiation: shared-memory opt-in + force-load (DESIGN §7). A one-tile (32) and a multi-tile batch, under
+// the ReLU and under one of the other activations, stand for all.
+cudaError_t prepare_fused_kernels() {
+  for (const int act : {ACT_RELU, ACT_TANH})
+    for (const bool l2 : {false, true})
+      for (const bool clip : {false, true})
+        for (const int B : {32, 32 * kFsMaxTiles}) {
+          const FusedKernel k = fused_kernel(B, clip, l2, act);
+          cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(fused_smem_bytes(B)));
+          cudaFuncAttributes a;
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, k);
+          if (e != cudaSuccess) return e;
+        }
+  return cudaSuccess;
 }
 
 cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int lanes, cudaStream_t stream) {
@@ -1140,19 +1126,14 @@ cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int l
     if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
-  return cudaLaunchKernelEx(&cfg, fused_kernel_for(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f, p.act), maps, p);
+  return cudaLaunchKernelEx(&cfg, fused_kernel(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f, p.act), maps, p);
 }
 
-// How many clusters of the fused kernel that runs batch B can be co-resident on the device (upper bound for `lanes`).
-cudaError_t fused_max_lanes(int B, int* out) { return fused_max_lanes_for(B, false, false, ACT_RELU, out); }
-
-cudaError_t fused_max_lanes_clip(int B, int* out) { return fused_max_lanes_for(B, true, false, ACT_RELU, out); }
-
-cudaError_t fused_max_lanes_for(int B, bool clip, bool l2, int act, int* out) {
+cudaError_t fused_max_lanes(int B, bool clip, bool l2, int act, int* out) {
   if (!act_valid(act)) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  return cudaOccupancyMaxActiveClusters(out, fused_kernel_for(B, clip, l2, act), &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_kernel(B, clip, l2, act), &cfg);
 }
 
 }  // namespace dm

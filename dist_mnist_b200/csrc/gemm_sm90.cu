@@ -613,33 +613,40 @@ size_t gemm_bt_bytes(int bn) { return static_cast<size_t>(bn) * 128 + 1024; }
 
 constexpr int kMaxDynSmem = 226 * 1024;  // 227 KB per-block limit minus the kernel's static shared memory
 
-template <typename T, bool A_MN, bool B_MN>
-static cudaError_t prepare_one() {
-  return cudaFuncSetAttribute(gemm_wgmma_kernel<T, A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              kMaxDynSmem);
+using GemmKernel = void (*)(const CUtensorMap, const CUtensorMap, const GemmParams);
+
+template <typename T>
+static GemmKernel gemm_kernel_of(bool a_mn, bool b_mn) {
+  if (!a_mn && !b_mn) return gemm_wgmma_kernel<T, false, false>;
+  if (a_mn && b_mn) return gemm_wgmma_kernel<T, true, true>;
+  if (a_mn) return gemm_wgmma_kernel<T, true, false>;
+  return gemm_wgmma_kernel<T, false, true>;
+}
+
+// The instantiation for operands of `dtype` (0 = fp32 (tf32 MMA), 1 = bf16), A and B MN-major or K-major.
+static GemmKernel gemm_kernel(int dtype, bool a_mn, bool b_mn) {
+  return dtype == 0 ? gemm_kernel_of<float>(a_mn, b_mn) : gemm_kernel_of<__nv_bfloat16>(a_mn, b_mn);
 }
 
 // Opt every instantiation into the full 227 KB of dynamic shared memory once per device, outside of any
-// stream capture (launches themselves then carry no attribute calls and are graph-capturable).
+// stream capture (launches themselves then carry no attribute calls and are graph-capturable), and force-load it.
 cudaError_t prepare_gemm_kernels() {
-  cudaError_t e;
-#define DM_PREP(T)                                              \
-  if ((e = prepare_one<T, false, false>()) != cudaSuccess) return e; \
-  if ((e = prepare_one<T, true, true>()) != cudaSuccess) return e;   \
-  if ((e = prepare_one<T, true, false>()) != cudaSuccess) return e;  \
-  if ((e = prepare_one<T, false, true>()) != cudaSuccess) return e;
-  DM_PREP(float)
-  DM_PREP(__nv_bfloat16)
-#undef DM_PREP
+  static const bool kLayouts[4][2] = {{false, false}, {true, true}, {true, false}, {false, true}};   // (A, B) MN-major
+  for (const int dtype : {0, 1})
+    for (const auto& mn : kLayouts) {
+      const GemmKernel k = gemm_kernel(dtype, mn[0], mn[1]);
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+      cudaFuncAttributes a;
+      if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, k);
+      if (e != cudaSuccess) return e;
+    }
   return cudaSuccess;
 }
 
-template <typename T, bool A_MN, bool B_MN>
-static cudaError_t launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, dim3 grid,
-                              cudaStream_t stream) {
-  auto kern = gemm_wgmma_kernel<T, A_MN, B_MN>;
+static cudaError_t launch_one(GemmKernel kern, bool b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                              const GemmParams& p, dim3 grid, cudaStream_t stream) {
   const bool cluster = p.splitk_cluster != 0 && grid.z > 1;
-  const size_t smem = gemm_smem_bytes(p.bn, p.stages, cluster ? 1 : 0) + (B_MN ? gemm_bt_bytes(p.bn) : 0);
+  const size_t smem = gemm_smem_bytes(p.bn, p.stages, cluster ? 1 : 0) + (b_mn ? gemm_bt_bytes(p.bn) : 0);
   if (smem > static_cast<size_t>(kMaxDynSmem) || p.bn < 16 || p.bn > 16 * kMaxNB || (p.bn & 15)) return cudaErrorInvalidValue;
   if (!cluster && !p.pdl) {
     kern<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, p);
@@ -675,17 +682,7 @@ cudaError_t launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Ge
                         bool b_mn, int splits, cudaStream_t stream) {
   if (!act_valid(p.act)) return cudaErrorInvalidValue;
   dim3 grid((p.M + kTileM - 1) / kTileM, (p.N + p.bn - 1) / p.bn, splits);
-#define DM_DISPATCH(T)                                                                  \
-  if (!a_mn && !b_mn) return launch_one<T, false, false>(tmA, tmB, p, grid, stream);   \
-  if (a_mn && b_mn) return launch_one<T, true, true>(tmA, tmB, p, grid, stream);       \
-  if (a_mn && !b_mn) return launch_one<T, true, false>(tmA, tmB, p, grid, stream);     \
-  return launch_one<T, false, true>(tmA, tmB, p, grid, stream);
-  if (dtype == 0) {
-    DM_DISPATCH(float)
-  } else {
-    DM_DISPATCH(__nv_bfloat16)
-  }
-#undef DM_DISPATCH
+  return launch_one(gemm_kernel(dtype, a_mn, b_mn), b_mn, tmA, tmB, p, grid, stream);
 }
 
 }  // namespace dm

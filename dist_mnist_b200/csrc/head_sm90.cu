@@ -346,10 +346,6 @@ size_t head_smem_bytes(int B_pad, int H, int C) {
 
 constexpr int kHeadMaxSmem = 224 * 1024;
 
-cudaError_t prepare_head_kernel() {
-  return cudaFuncSetAttribute(head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHeadMaxSmem);
-}
-
 cudaError_t launch_head(const HeadParams& p, cudaStream_t stream) {
   if (p.C > kMaxC || p.B > kMaxB || p.B_pad > kMaxB || !act_valid(p.act)) return cudaErrorInvalidValue;
   const size_t smem = head_smem_bytes(p.B_pad, p.H, p.C);
@@ -420,12 +416,11 @@ cudaError_t launch_accuracy(const float* logits, const float* labels, int B, int
   return cudaGetLastError();
 }
 
-cudaError_t preload_head_kernels() {
+cudaError_t prepare_head_kernels() {
+  cudaError_t e = cudaFuncSetAttribute(head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHeadMaxSmem);
   cudaFuncAttributes a;
-  cudaError_t e;
-  if ((e = cudaFuncGetAttributes(&a, head_kernel)) != cudaSuccess) return e;
-  if ((e = cudaFuncGetAttributes(&a, accuracy_kernel)) != cudaSuccess) return e;
-  return cudaSuccess;
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, head_kernel);
+  return e != cudaSuccess ? e : cudaFuncGetAttributes(&a, accuracy_kernel);
 }
 
 }  // namespace dm

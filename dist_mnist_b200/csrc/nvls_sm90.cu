@@ -77,7 +77,7 @@ __global__ void unicast_reduce_kernel(float4* const* __restrict__ srcs, int n_sr
   }
 }
 
-cudaError_t preload_nvls_kernels() {
+cudaError_t prepare_nvls_kernels() {
   cudaFuncAttributes a;
   cudaError_t e;
   if ((e = cudaFuncGetAttributes(&a, multimem_publish_kernel)) != cudaSuccess) return e;

@@ -146,7 +146,7 @@ cudaError_t launch_pingpong(uint32_t* local_flag, uint32_t* remote_flag, int ite
 }  // namespace dm
 
 namespace dm {
-cudaError_t preload_p2p_kernels() {
+cudaError_t prepare_p2p_kernels() {
   cudaFuncAttributes a;
   cudaError_t e;
   if ((e = cudaFuncGetAttributes(&a, p2p_copy_ldst_kernel)) != cudaSuccess) return e;

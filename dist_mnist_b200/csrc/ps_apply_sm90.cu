@@ -804,11 +804,9 @@ cudaError_t launch_worker_done(uint32_t* done_slot, const uint32_t* seq_ptr, cud
 }  // namespace dm
 
 namespace dm {
-// Force-load every kernel of this translation unit. With CUDA's lazy module loading the *first* launch of a
-// kernel may need a context-wide synchronisation; if that first launch happens while the persistent serve
-// kernel is resident (and the serve kernel is waiting for the new kernel's flags) the process deadlocks. The serve
-// kernels are enumerated through serve_kernel, so every one that launch_ps_serve can pick is loaded here.
-cudaError_t preload_ps_kernels() {
+// Force-load every kernel of this translation unit (DESIGN §7). The serve kernels are enumerated through serve_kernel,
+// so every one that launch_ps_serve can pick is loaded here.
+cudaError_t prepare_ps_kernels() {
   cudaFuncAttributes a;
   cudaError_t e;
   for (int opt = OPT_SGD; opt <= OPT_ADAGRAD_DA; ++opt)

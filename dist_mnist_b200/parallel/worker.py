@@ -787,9 +787,9 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
-        N.check(self.lib.dm_fused_max_lanes_for(self.device, self.batch, int(self.opt.clip.enabled),
-                                                int(self.opt.l2.enabled), mlp.activation_code(spec.activation),
-                                                C.byref(max_lanes)), "fused occupancy")
+        N.check(self.lib.dm_fused_max_lanes(self.device, self.batch, int(self.opt.clip.enabled),
+                                            int(self.opt.l2.enabled), mlp.activation_code(spec.activation),
+                                            C.byref(max_lanes)), "fused occupancy")
         free = max_lanes.value
         if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
             # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots

@@ -46,9 +46,6 @@ float checksum(const float* p, size_t n) {
 }  // namespace
 
 namespace dm {
-cudaError_t prepare_fused_kernel() { return cudaSuccess; }
-size_t fused_smem_bytes(int) { return 0; }
-cudaError_t fused_max_lanes(int, int* out) { *out = 16; return cudaSuccess; }
 // Stand-in for the kernel: same launch-state protocol as fused_step_kernel (step claiming is sequential here).
 cudaError_t launch_fused_step(const FusedMaps&, const FusedParams& p, int, cudaStream_t stream) {
   const FusedParams q = p;

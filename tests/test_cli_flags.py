@@ -89,6 +89,28 @@ def test_adam_math_flag_selects_the_ieee_serve_kernel_instantiation():
         assert len(set(re.findall(r"ps_serve_kernelI\w+?EEEv", syms))) == 42
 
 
+def test_library_holds_the_instantiations_the_fused_gemm_and_clip_selectors_name():
+    """16 fused step kernels ((B <= 32, B > 32) x clip x L2 x (ReLU, other activation)), 8 GEMM kernels (fp32 / bf16 x
+    A, B MN- or K-major), and the gradient clip's sums of squares and apply (with and without L2) and release."""
+    import re
+    import subprocess
+
+    from dist_mnist_b200 import _build
+    from dist_mnist_b200 import _native as N
+
+    N.lib()
+    syms = subprocess.run([str(_build._cuda_home() / "bin" / "cuobjdump"), "-symbols", str(N.lib_path())],
+                          capture_output=True, text=True, check=True).stdout
+    kernels = re.findall(r"STO_ENTRY\s+(\S+)", syms)
+
+    def count(pattern):
+        return sum(re.match(pattern, k) is not None for k in kernels)
+
+    assert count(r"_ZN2dm17fused_step_kernelI") == 16
+    assert count(r"_ZN2dm17gemm_wgmma_kernelI") == 8
+    assert count(r"_ZN2dm\d+grad_clip_\w+_kernelI") == 4 and count(r"_ZN2dm\d+grad_clip_\w+_kernelE") == 1
+
+
 def test_package_is_runnable_as_a_module():
     import os
     import subprocess

@@ -3,7 +3,7 @@ activation against torch (bench_tools/gpu_check); every pushed element against t
 bench_tools/fused_push_ref, over the fused engine's batch, hidden, input and class edges, 4 pipelined lanes, a 2-shard
 row split, the atomic push, a clip and L2 (so that every activation instantiation of the fused kernel runs), and the
 graph engine at 784-H-10; lock-step trajectories against fp32 torch (300 strict fused steps, 100 graph-engine zhihu
-steps, one bf16 run); `evaluate` on both engines; and the fused lane cap."""
+steps, one bf16 run); and `evaluate` on both engines."""
 import pytest
 
 from bench_tools import fused_push_ref as R
@@ -24,27 +24,6 @@ def test_kernel_epilogues_and_head(name):
     assert gpu_check.check_gemm_fwd(name)
     assert gpu_check.check_gemm_dx(name)
     assert gpu_check.check_head(name)
-
-
-def test_fused_lane_cap_is_that_of_the_relu_kernels():
-    """The activation instantiations have the shared memory and (<= 255) registers of the ReLU ones: the same cluster
-    count fits on the device, and so the same lanes beside the ps serve kernel."""
-    import ctypes as C
-
-    from dist_mnist_b200 import _native as N
-
-    lib = N.lib()
-    N.ensure_prepared(0)
-    for B in (32, 256):
-        for clip in (0, 1):
-            for l2 in (0, 1):
-                relu = C.c_int(0)
-                N.check(lib.dm_fused_max_lanes_for(0, B, clip, l2, N.ACT_RELU, C.byref(relu)))
-                assert relu.value > 0
-                for name in ACTS:
-                    got = C.c_int(0)
-                    N.check(lib.dm_fused_max_lanes_for(0, B, clip, l2, mlp.activation_code(name), C.byref(got)))
-                    assert got.value == relu.value, (B, clip, l2, name, relu.value, got.value)
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -2,7 +2,7 @@
 plus fl(S * w) (isolating the L2 term from tf32 error), alone and under every clip kind, over the fused engine's batch
 sizes, hidden sizes and shardings and on the graph engine (book and zhihu, fp32 and bf16); the reported loss against
 the unregularized one plus the fp64 L2 term; lock-step trajectories against fp32 PyTorch with the reference L2 (300
-fused steps, 100 graph steps); bit-identical repeated runs; group graphs; and the fused lane cap beside the ps."""
+fused steps, 100 graph steps); bit-identical repeated runs; and group graphs."""
 import pytest
 
 from bench_tools.fused_push_ref import pushed
@@ -238,20 +238,3 @@ def test_graph_l2_pipelined_runs_with_group_graphs(model, dtype):
         last = sum(o.loss for o in outs[-20:]) / 20
         assert last < 0.7 * first, (first, last)
 
-
-def test_l2_fused_lane_cap_is_that_of_the_unregularized_kernels():
-    """The L2 instantiations have the shared memory and (<= 255) registers of the others: the same cluster count fits
-    on the device, and so the same lanes beside the ps serve kernel."""
-    import ctypes as C
-
-    from dist_mnist_b200 import _native as N
-
-    lib = N.lib()
-    N.ensure_prepared(0)
-    for B in (32, 256):
-        plain = C.c_int(0)
-        N.check(lib.dm_fused_max_lanes(0, B, C.byref(plain)))
-        for clip in (0, 1):
-            reg = C.c_int(0)
-            N.check(lib.dm_fused_max_lanes_l2(0, B, clip, C.byref(reg)))
-            assert reg.value == plain.value, (B, clip, plain.value, reg.value)
