@@ -37,9 +37,9 @@ def _clip(name):
 
 
 def measure(batch: int, lanes: int, steps: int, warmup: int, clip_name: str, dev: int = 0, engine: str = "fused",
-            model: str = None, l2=None, activation: str = "relu") -> float:
+            model: str = None, l2=None, activation: str = "relu", loss: str = None, label_smoothing: float = 0.0) -> float:
     """Device-timed steps/s of `steps` steps beside the resident ps (`l2`: an L2Regularization, default off;
-    `activation`: of the hidden layers)."""
+    `activation`: of the hidden layers; `loss`, `label_smoothing`: of the head, default the model's own loss)."""
 
     import torch
 
@@ -51,7 +51,7 @@ def measure(batch: int, lanes: int, steps: int, warmup: int, clip_name: str, dev
     from dist_mnist_b200.utils.metrics import StreamTimer
 
     args = bench.parse_args(["--gpus", "1", "--lanes", str(lanes), "--batch_size", str(batch)])
-    spec = mlp.get_model(model or args.model, args.hidden_units, activation)
+    spec = mlp.get_model(model or args.model, args.hidden_units, activation, loss, label_smoothing)
     opt = OptimizerConfig(args.optimizer, args.learning_rate, clip=_clip(clip_name),
                           **({"l2": l2} if l2 is not None else {}))
     cfg = dataclasses.replace(bench.engine_config(args), engine=engine)

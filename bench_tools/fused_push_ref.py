@@ -69,6 +69,28 @@ RND_ACT |f'|), with the jump of f' across the kink (relu: 1, giving the |dh| + d
 that every branch is taken: both signs for leaky_relu, elu and selu, pre above 6 for relu6, |pre| > 3 in saturated
 units for sigmoid and tanh (`_cover_activation`, asserted by `check_case`).
 
+Other losses (`--loss`, `--label_smoothing`; case builder and bound take `loss` and `label_smoothing`)
+--------------------------------------------------------------------------------------------------
+The labels the loss sees are y' = smooth(y), formed in fp32 exactly as the kernels form them (csrc/loss.cuh); that
+rounding is TF's too, so the fp64 reference takes the fp32 y' as its labels. The correct count uses the raw y. For
+the elementwise losses k = 1 / (B C), and dz_bc (not its row maximum) bounds the error of logit z_bc.
+* xent on smoothed labels: y' is no longer one-hot, so the cancellation in p S - y' (S = sum_c y'_c, about 1) sits at
+  every class where p_c is near y'_c, not only at the true one; the rounding stays absolute: E_bc = k (p_c (2 dz_b +
+  ep_c) S + EPS_F (p_c S + y'_c)) plus EPS_F p_c S for fl(S) (exact for one-hot labels). Loss per row: sum_c y'_c (2 dz_b + 2^-20 (1 + ln esum)
+  + EPS_F (|z_c| + |zmax| + ln esum)), the one-hot terms above at every class.
+* sigmoid_xent: dl = k (s - y') with s = sigmoid(z) from e = expf(-|z|) (2 ulp), 1 + e and an IEEE divide, so s errs
+  by s' dz_bc <= dz_bc / 4 plus RND_LOSS s (RND_LOSS = 2^-20, 4x the roundings); the subtraction adds EPS_F (s + y'):
+  E = k (dz / 4 + RND_LOSS s + EPS_F (s + y')). Loss element: its slope in z is s - y' in [-1, 1], so dz, plus
+  log1pf's 2 ulp and the roundings, EPS_F (|z| (1 + y') + 1).
+* mse: dl = 2k (z - y), so the error is absolute in |z - y|: E = 2k (dz + EPS_F |z - y|) (the fp32 k and the exact
+  doubling add u). Loss element (z - y)^2: 2 |z - y| dz + dz^2 + EPS_F (z - y)^2.
+* hinge: dl = -k y+- where m = 1 - y+- z > 0 (y+- = 2y - 1 = +-1), else 0. m errs by hedge = dz + EPS_F (|z| + 1),
+  so, as at the ReLU's kink, pairs with |m| <= 2 hedge are *ambiguous*: the kernel may take either branch, E = k (the
+  jump); elsewhere only k's fp32 rounding, E = EPS_F k. Loss element relu(m), 1-Lipschitz: hedge + EPS_F relu(m). A
+  kernel that took m >= 0 for m > 0 differs only at m = 0 exactly, inside the band, so no mutant can show it; the
+  hinge mutant drops the mask instead. The builder scales W_last by HINGE_SCALE so that logits pass +-1 and both
+  branches are taken beyond the band (`check_case`).
+
 The graph engine computes the same quantities with the same or tighter fp32 operations (IEEE division in the head, an
 fp32 dW GEMM on tf32 operands), so the same bound applies to it unchanged.
 
@@ -81,12 +103,14 @@ and every reported correct count lies in its range.
 round-to-nearest; tests/test_fused_push_bound_cpu.py shows it inside the bound and each of a set of mutants (a dropped
 batch row, a zeroed k-chunk, ...) far outside it at every case whose coverage admits the mutant, and
 tests/test_activations_cpu.py does the same for every activation with the activation's own mutants (f or f' not
-applied, f' of the pre-activation, relu6's f' without its upper kink).
+applied, f' of the pre-activation, relu6's f' without its upper kink), and tests/test_losses_cpu.py for every loss
+and smoothing (LOSS_MUTANTS: smoothing not applied, the correct count taken of the smoothed labels, the sigmoid's
+gradient negated, mse's factor 2 dropped, hinge's mask dropped).
 """
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -104,6 +128,9 @@ CLAMP = 1e-10            # the book loss's clip of p
 CHUNK = 32               # features per k-chunk of the fused kernel
 VARS = ("hid_w", "hid_b", "sm_w", "sm_b")
 RND_ACT = 2.0 ** -20     # relative rounding of f and f' (expf / tanhf 2 ulp + a few roundings, 4x margin)
+RND_LOSS = 2.0 ** -20    # relative rounding of the sigmoid of sigmoid_xent (expf 2 ulp + two roundings, 4x margin)
+HINGE_SCALE = 10.0       # W_last scale of hinge cases: logits past +-1, so that both branches of the hinge are taken
+ELEMENTWISE = ("sigmoid_xent", "mse", "hinge")
 
 
 @dataclass(frozen=True)
@@ -153,9 +180,9 @@ class Case:
         return H, C, I, self.batch, self.spec.loss
 
 
-def spec_for(H: int, C: int, I: int, loss: str, activation: str = "relu") -> mlp.MLPSpec:
+def spec_for(H: int, C: int, I: int, loss: str, activation: str = "relu", label_smoothing: float = 0.0) -> mlp.MLPSpec:
     return mlp.MLPSpec(name="book", in_features=I, hidden=(H,), num_classes=C, loss=loss, init="book",
-                       activation=activation)
+                       activation=activation, label_smoothing=label_smoothing)
 
 
 def tf32_exact(t: torch.Tensor) -> torch.Tensor:
@@ -185,12 +212,14 @@ def _draw_batch(g: torch.Generator, protos: torch.Tensor, B: int) -> Tuple[torch
 
 
 def make_case(H: int, C: int, I: int, B: int, loss: str, seed: int, n_batches: int = 1, saturate: float = 0.0,
-              name: Optional[str] = None, activation: str = "relu") -> Case:
+              name: Optional[str] = None, activation: str = "relu", label_smoothing: float = 0.0) -> Case:
     """A tf32-exact case at shape (H, C, I, B, loss), redrawn from `seed` until `check_case` passes (coverage, the
-    clamp margin). `saturate` scales W_last so that some rows' true-class p fall far below the clamp. Under an
-    activation other than relu, biases are then moved so that every branch of it is taken (`_cover_activation`); relu
-    cases are drawn exactly as they were before activations existed."""
-    spec = spec_for(H, C, I, loss, activation)
+    clamp margin). `saturate` scales W_last so that some rows' true-class p fall far below the clamp (hinge cases
+    scale it by HINGE_SCALE). Under an activation other than relu, biases are then moved so that every branch of it is
+    taken (`_cover_activation`); relu cases are drawn exactly as they were before activations existed."""
+    spec = spec_for(H, C, I, loss, activation, label_smoothing)
+    if loss == "hinge" and not saturate:
+        saturate = HINGE_SCALE
     for attempt in range(64):
         sub = seed * 1000 + attempt
         g = torch.Generator().manual_seed(sub)
@@ -208,9 +237,10 @@ def make_case(H: int, C: int, I: int, B: int, loss: str, seed: int, n_batches: i
         params["hid_b"] = torch.maximum(params["hid_b"], (0.02 - top).float())
         if activation != "relu":
             _cover_activation(activation, params, batches)
-        case = Case(name or f"H{H}-C{C}-I{I}-B{B}-{loss}" + ("-sat" if saturate else "") +
-                    ("" if activation == "relu" else f"-{activation}"), spec, params, batches, sub,
-                    saturated=bool(saturate))
+        case = Case(name or f"H{H}-C{C}-I{I}-B{B}-{loss}" + ("-sat" if saturate and loss != "hinge" else "") +
+                    ("" if activation == "relu" else f"-{activation}") +
+                    (f"-ls{label_smoothing:g}" if label_smoothing else ""), spec, params, batches, sub,
+                    saturated=bool(saturate) and loss != "hinge")
         if all(not check_case(case, x, y) for x, y in batches):
             assert exact_inputs(case) == [], exact_inputs(case)
             return case
@@ -283,8 +313,9 @@ def shape_matrix() -> List[Tuple[str, Tuple[int, int, int, int, str], float]]:
 
 
 def case_for(shape: Tuple[int, int, int, int, str], saturate: float = 0.0, n_batches: int = 1, seed: int = 1,
-             activation: str = "relu") -> Case:
-    return make_case(*shape, seed=seed, n_batches=n_batches, saturate=saturate, activation=activation)
+             activation: str = "relu", label_smoothing: float = 0.0) -> Case:
+    return make_case(*shape, seed=seed, n_batches=n_batches, saturate=saturate, activation=activation,
+                     label_smoothing=label_smoothing)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -308,18 +339,24 @@ class Reference:
     p_true: torch.Tensor = field(repr=False, default=None)
     active: torch.Tensor = field(repr=False, default=None)   # f' != 0, away from every kink
     hv: torch.Tensor = field(repr=False, default=None)       # f(pre)
+    z: torch.Tensor = field(repr=False, default=None)        # logits
+    hinge_m: torch.Tensor = field(repr=False, default=None)  # hinge: 1 - y+- z
+    hinge_edge: torch.Tensor = field(repr=False, default=None)  # hinge: half-width of the ambiguity band at m = 0
 
 
 def _k(spec: mlp.MLPSpec, B: int) -> float:
-    return 1.0 / (B * spec.num_classes) if spec.loss == "book" else 1.0 / B
+    return 1.0 / B if spec.loss == "xent" else 1.0 / (B * spec.num_classes)
 
 
 def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor, y: torch.Tensor) -> Reference:
     """The fp64 step on (x, y) and the per-element bounds of the module docstring."""
     d = torch.float64
     P = {k: v.to(d) for k, v in params.items()}
-    x64, y64 = x.to(d), y.to(d)
-    loss, grads, logits = mlp.manual_loss_and_grads(spec, P, x64, y64)
+    yraw = y.to(d)
+    # the smoothed labels are rounded to fp32 as TF (and the kernels) round them: they are the fp64 step's labels
+    spec0 = replace(spec, label_smoothing=0.0)
+    x64, y64 = x.to(d), mlp.smooth_labels(spec, y.float()).to(d)
+    loss, grads, logits = mlp.manual_loss_and_grads(spec0, P, x64, y64)
     W, b, Wl, bl = P["hid_w"], P["hid_b"], P["sm_w"], P["sm_b"]
     B, C = y.shape
     k = _k(spec, B)
@@ -345,15 +382,32 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
     zmax = z.amax(dim=1, keepdim=True)
     ee = (2.0 + 1.173 * (zmax - z)) * ULP1
     ep = ee + (p * ee).sum(dim=1, keepdim=True) + 16 * U + 2.0 ** -22 + EXP_SLACK
-    p_true = (p * y64).sum(dim=1)
-    live = torch.ones(B, dtype=torch.bool) if spec.loss == "xent" else p_true >= CLAMP
-    E = k * (p * (2 * dz + ep) + EPS_F * (p + y64)) * live[:, None].to(d)
+    p_true = (p * yraw).sum(dim=1)
+    live = p_true >= CLAMP if spec.loss == "book" else torch.ones(B, dtype=torch.bool)
+    S = y64.sum(dim=1, keepdim=True)
+    hm = hedge = None
     if spec.loss == "book":
+        E = k * (p * (2 * dz + ep) + EPS_F * (p + y64)) * live[:, None].to(d)
         passes = p >= CLAMP
         g = torch.where(passes, -k * y64 / p.clamp_min(1e-300), torch.zeros_like(p))
         dl = p * (g - (g * p).sum(dim=1, keepdim=True))
-    else:
-        dl = (p * y64.sum(dim=1, keepdim=True) - y64) * k
+    elif spec.loss == "xent":
+        fl_s = EPS_F * p * S if spec.label_smoothing else 0.0   # fl(S): exact for one-hot labels
+        E = k * (p * (2 * dz + ep) * S + EPS_F * (p * S + y64) + fl_s)
+        dl = (p * S - y64) * k
+    elif spec.loss == "sigmoid_xent":
+        sig = torch.sigmoid(z)
+        E = k * (dzc / 4 + RND_LOSS * sig + EPS_F * (sig + y64))
+        dl = k * (sig - y64)
+    elif spec.loss == "mse":
+        E = 2 * k * (dzc + EPS_F * (z - y64).abs())
+        dl = 2 * k * (z - y64)
+    else:   # hinge
+        ypm = 2 * y64 - 1
+        hm = 1 - ypm * z
+        hedge = 2 * (dzc + EPS_F * (z.abs() + 1))
+        E = k * torch.where(hm.abs() <= hedge, torch.ones_like(hm), torch.full_like(hm, EPS_F))
+        dl = torch.where(hm > 0, -k * ypm, torch.zeros_like(hm))
     dh = dl @ Wl
     dpre = mlp.activation_grad(spec.activation, hv, dh)
     ddh = E @ aWl + EPS_F * (dl.abs() @ aWl)
@@ -370,10 +424,16 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
         "sm_b": (E + EPS_F * dl.abs()).sum(dim=0),
     }
     esum = torch.exp(z - zmax).sum(dim=1)
-    zt = (z * y64).sum(dim=1)
     dzr = dz[:, 0]
     if spec.loss == "xent":
-        lrow = 2 * dzr + EXP_SLACK * (1 + esum.log()) + EPS_F * (zt.abs() + zmax[:, 0].abs() + esum.log())
+        lrow = (y64 * (2 * dz + EXP_SLACK * (1 + esum.log()[:, None]) +
+                       EPS_F * (z.abs() + zmax.abs() + esum.log()[:, None]))).sum(dim=1)
+    elif spec.loss == "sigmoid_xent":
+        lrow = (dzc + EPS_F * (z.abs() * (1 + y64) + 1)).sum(dim=1)
+    elif spec.loss == "mse":
+        lrow = (2 * (z - y64).abs() * dzc + dzc * dzc + EPS_F * (z - y64) ** 2).sum(dim=1)
+    elif spec.loss == "hinge":
+        lrow = (hedge / 2 + EPS_F * hm.clamp(min=0.0)).sum(dim=1)
     else:
         ep_t = (ep * y64).sum(dim=1)
         lrow = torch.where(live, 2 * dzr + ep_t + EXP_SLACK + EPS_F * p_true.clamp_min(CLAMP).log().abs(),
@@ -382,10 +442,10 @@ def reference(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tenso
     top2 = z.topk(min(2, C), dim=1).values
     gap = top2[:, 0] - top2[:, 1] if C > 1 else torch.full((B,), math.inf, dtype=d)
     unsure = gap <= 2 * dzr + EPS_F * z.abs().amax(dim=1)
-    right = z.argmax(dim=1) == y64.argmax(dim=1)
+    right = z.argmax(dim=1) == yraw.argmax(dim=1)
     lo = int((right & ~unsure).sum())
     return Reference({n: grads[n] for n in VARS}, bounds, float(loss), loss_bound, lo, lo + int(unsure.sum()),
-                     x64, pre, edge, dh, dpre, dl, p_true, act, hv)
+                     x64, pre, edge, dh, dpre, dl, p_true, act, hv, z, hm, hedge)
 
 
 def check_case(case: Case, x: torch.Tensor, y: torch.Tensor) -> List[str]:
@@ -396,7 +456,8 @@ def check_case(case: Case, x: torch.Tensor, y: torch.Tensor) -> List[str]:
     loss keeps every true-class p outside [1e-10 / 2, 2e-10]; the saturated case has clamped and unclamped rows.
     "Active" is f' != 0 outside the ambiguity bands (the ReLU: pre above the band). Each branch of the activation is
     taken (beyond the band) where a single pre-activation does not rule it out: both signs for leaky_relu, elu and
-    selu, pre above 6 for relu6 (with H > 1), saturated |pre| > 3 for sigmoid and tanh."""
+    selu, pre above 6 for relu6 (with H > 1), saturated |pre| > 3 for sigmoid and tanh. The hinge has margins on both
+sides of its kink, beyond the ambiguity band."""
     spec = case.spec
     r = reference(spec, case.params, x, y)
     act = r.pre > r.edge if spec.activation == "relu6" else r.active   # (units above 6 are not dead)
@@ -412,7 +473,10 @@ def check_case(case: Case, x: torch.Tensor, y: torch.Tensor) -> List[str]:
         bad.append(f"{a}: no saturated pre-activation")
     if not bool(act.any(dim=0).all()):
         bad.append(f"hidden units never active: {(~act.any(dim=0)).nonzero().flatten().tolist()}")
-    live = torch.ones(x.shape[0], dtype=torch.bool) if spec.loss == "xent" else r.p_true >= CLAMP
+    live = r.p_true >= CLAMP if spec.loss == "book" else torch.ones(x.shape[0], dtype=torch.bool)
+    if spec.loss == "hinge" and r.z.numel() > 1 and not (bool((r.hinge_m > r.hinge_edge).any()) and
+                                                          bool((r.hinge_m < -r.hinge_edge).any())):
+        bad.append("hinge: margins of one side only")
     rows_ok = (x.abs().sum(dim=1) > 0) & (~live | (r.dl.abs().sum(dim=1) > 0) | torch.tensor(spec.num_classes == 1))
     if not bool(rows_ok.all()):
         bad.append(f"batch rows without a contribution: {(~rows_ok).nonzero().flatten().tolist()}")
@@ -456,20 +520,34 @@ def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
     elif mutant == "drop_tile":
         live[32 * arg:32 * (arg + 1)] = 0.0
     nb = 32 * ((B + 31) // 32) if mutant == "loss_32T" else B
+    ys = y if mutant == "smoothing_missing" else mlp.smooth_labels(spec, y)
     pre = x @ W.t() + b
     a = spec.activation
     hv = pre if mutant == "act_forward_missing" else mlp.activate(a, pre)
     z = hv @ Wl.t() + bl
     p = torch.softmax(z, dim=1)
+    k = torch.tensor(1.0, dtype=f) / (torch.tensor(float(nb), dtype=f) * torch.tensor(float(C), dtype=f))
     if spec.loss == "book":
-        k = torch.tensor(1.0, dtype=f) / (torch.tensor(float(nb), dtype=f) * torch.tensor(float(C), dtype=f))
         g = torch.where((p >= 1e-10) & (p <= 1.0), -k * y / p, torch.zeros_like(p))
         dl = p * (g - (g * p).sum(dim=1, keepdim=True))
         lc = -k * y * torch.log(p.clamp(1e-10, 1.0))
-    else:
+    elif spec.loss == "xent":
         k = torch.tensor(1.0, dtype=f) / torch.tensor(float(nb), dtype=f)
-        dl = k * (p * y.sum(dim=1, keepdim=True) - y)
-        lc = -k * y * torch.log_softmax(z, dim=1)
+        dl = k * (p * ys.sum(dim=1, keepdim=True) - ys)
+        lc = -k * ys * torch.log_softmax(z, dim=1)
+    elif spec.loss == "sigmoid_xent":
+        elem, sig = mlp._sigmoid_xent_terms(z, ys)
+        dl = k * (ys - sig) if mutant == "sigmoid_grad_sign" else k * (sig - ys)
+        lc = k * elem
+    elif spec.loss == "mse":
+        dz = z - ys
+        dl = (k if mutant == "mse_factor_two_missing" else 2 * k) * dz
+        lc = k * (dz * dz)
+    else:   # hinge
+        ypm = 2 * ys - 1
+        m = 1 - ypm * z
+        dl = (-k) * ypm if mutant == "hinge_mask_missing" else torch.where(m > 0, (-k) * ypm, torch.zeros_like(m))
+        lc = k * torch.relu(m)
     dl = dl * live
     if a == "relu":
         mask = (hv > 0).to(f)
@@ -494,15 +572,20 @@ def emulate(spec: mlp.MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tensor,
         dWl = dWl.t().contiguous().reshape(dWl.shape)
     elif mutant == "sm_w_class_shift":
         dWl = torch.roll(dWl, 1, dims=0)
-    correct = int(((z.argmax(dim=1) == y.argmax(dim=1)) & (live[:, 0] > 0)).sum())
+    yc = ys if mutant == "smoothing_in_accuracy" else y
+    correct = int(((z.argmax(dim=1) == yc.argmax(dim=1)) & (live[:, 0] > 0)).sum())
     return Step({"hid_w": dW, "hid_b": dpre.sum(dim=0), "sm_w": dWl, "sm_b": dl.sum(dim=0)},
                 float((lc * live).sum()), correct)
 
 
 MUTANTS = ("drop_row", "drop_tile", "zero_chunk", "zero_hidden_row", "relu_missing", "loss_32T", "sm_w_transposed",
-           "sm_w_class_shift", "act_forward_missing", "act_grad_missing", "act_grad_from_pre", "relu6_upper_kink_missing")
-ACT_MUTANTS = MUTANTS[-4:]   # the activation's own: f not applied, f' not applied, f' of pre, relu6's f' without its
+           "sm_w_class_shift", "act_forward_missing", "act_grad_missing", "act_grad_from_pre", "relu6_upper_kink_missing",
+           "smoothing_missing", "smoothing_in_accuracy", "sigmoid_grad_sign", "mse_factor_two_missing",
+           "hinge_mask_missing")
+ACT_MUTANTS = MUTANTS[8:12]  # the activation's own: f not applied, f' not applied, f' of pre, relu6's f' without its
                              # upper kink
+LOSS_MUTANTS = MUTANTS[12:]  # the loss's own: labels not smoothed, the correct count of the smoothed labels, the
+                             # sigmoid's gradient negated, mse's factor 2 dropped, the hinge's mask dropped
 
 
 def mutant_instances(case: Case, ref: Reference) -> List[Tuple[str, int]]:
@@ -530,6 +613,7 @@ def mutant_instances(case: Case, ref: Reference) -> List[Tuple[str, int]]:
     def moves(change: torch.Tensor) -> bool:   # f' changed by `change`, by 5 % of the largest |dpre| |x| somewhere
         return float(((change.abs() * ref.dh.abs()) * rows).max()) > 0.05 * float((ref.dpre.abs() * rows).max())
 
+    out += _loss_mutants(case, ref)
     if a == "relu":
         off = (ref.pre < -ref.edge).to(torch.float64)
         weight = ((off * ref.dh.abs()) * rows).sum(dim=0)
@@ -546,6 +630,26 @@ def mutant_instances(case: Case, ref: Reference) -> List[Tuple[str, int]]:
         out.append(("act_grad_from_pre", 0))
     if a == "relu6" and moves((ref.pre > 6 + ref.edge).to(torch.float64)):
         out.append(("relu6_upper_kink_missing", 0))
+    return out
+
+
+def _loss_mutants(case: Case, ref: Reference) -> List[Tuple[str, int]]:
+    """LOSS_MUTANTS this batch admits: the smoothing ones under a smoothing (the correct count of the smoothed labels
+    only where it falls outside the reference's range: ls = 1, where every y' is equal and argmax says class 0), each
+    loss's own mutant under that loss (the hinge's dropped mask where some margin lies beyond the band on the inactive
+    side)."""
+    spec, out = case.spec, []
+    if spec.label_smoothing:
+        out.append(("smoothing_missing", 0))
+        z0 = int((ref.z.argmax(dim=1) == 0).sum())
+        if not ref.correct_lo <= z0 <= ref.correct_hi and spec.label_smoothing == 1.0:
+            out.append(("smoothing_in_accuracy", 0))
+    if spec.loss == "sigmoid_xent":
+        out.append(("sigmoid_grad_sign", 0))
+    elif spec.loss == "mse":
+        out.append(("mse_factor_two_missing", 0))
+    elif spec.loss == "hinge" and bool((ref.hinge_m < -ref.hinge_edge).any()):
+        out.append(("hinge_mask_missing", 0))
     return out
 
 

@@ -15,6 +15,7 @@ import subprocess
 import sys
 import time
 import traceback
+from typing import Optional
 
 import torch
 
@@ -201,15 +202,18 @@ def check_gemm_dx(activation: str = "relu") -> bool:
     return ok
 
 
-def check_head(activation: str = "relu") -> bool:
-    """The head kernel on h = f(random) of `activation` f: loss, correct count, small gradients and dpre = dh * f'(h)."""
+def check_head(activation: str = "relu", loss: Optional[str] = None, label_smoothing: float = 0.0) -> bool:
+    """The head kernel on h = f(random) of `activation` f: loss, correct count, small gradients and dpre = dh * f'(h),
+    under `loss` with `label_smoothing` (loss None: book and xent, unsmoothed)."""
     from dist_mnist_b200 import _native as N
     from dist_mnist_b200.models import mlp
     from dist_mnist_b200.ops import gemm, head
     ok = True
     dev = "cuda"
+    loss_names = ("book", "xent") if loss is None else (loss,)   # (`loss` names the reference's value below)
     for act_bf16 in (False, True):
-        for loss_kind, loss_name in ((N.LOSS_BOOK, "book"), (N.LOSS_XENT, "xent")):
+        for loss_name in loss_names:
+            loss_kind = mlp.loss_code(loss_name)
             for (H, B) in ((100, 32), (1024, 100), (500, 256), (37, 5)):
                 Cn = 10
                 B_pad = gemm.round_up(B, 16)
@@ -230,7 +234,8 @@ def check_head(activation: str = "relu") -> bool:
                 plan = head.head_plan(h_ptr=hq.data_ptr(), labels_ptr=labels.data_ptr(), w_last_ptr=w.data_ptr(),
                                       b_last_ptr=b.data_ptr(), dpre_ptr=dpre.data_ptr(), result_ptr=res.data_ptr(),
                                       B=B, B_pad=B_pad, H=H, num_classes=Cn, loss_kind=loss_kind, act_bf16=act_bf16,
-                                      act=mlp.activation_code(activation), push=gemm.local_push(g.data_ptr()), off_w_last=off_w, off_b_last=off_b,
+                                      act=mlp.activation_code(activation), label_smoothing=label_smoothing,
+                                      push=gemm.local_push(g.data_ptr()), off_w_last=off_w, off_b_last=off_b,
                                       off_b_hidden=off_bh)
                 plan.launch()
                 torch.cuda.synchronize()
@@ -239,7 +244,7 @@ def check_head(activation: str = "relu") -> bool:
                 wr = w.clone().requires_grad_(True)
                 br = b.clone().requires_grad_(True)
                 logits = hf @ wr.t() + br
-                spec = mlp.MLPSpec(loss=loss_name)
+                spec = mlp.MLPSpec(loss=loss_name, label_smoothing=label_smoothing)
                 loss = mlp.loss_from_logits(spec, logits, labels[:B])
                 gh, gw, gb_ = torch.autograd.grad(loss, [hf, wr, br])
                 dpre_ref = mlp.activation_grad(activation, hf.detach(), gh)
@@ -255,7 +260,8 @@ def check_head(activation: str = "relu") -> bool:
                 tol = 2e-2 if act_bf16 else 1e-4
                 good = (e_loss < 1e-4 and e_w < 1e-4 and e_b < 1e-4 and e_bh < tol and e_dp < tol and pad_ok
                         and got_correct == corr_ref)
-                ok &= report(f"head bf16={act_bf16} loss={loss_name} H={H} B={B} act={activation}", good,
+                ok &= report(f"head bf16={act_bf16} loss={loss_name} ls={label_smoothing:g} H={H} B={B} "
+                             f"act={activation}", good,
                              f"loss {got_loss:.6f}/{loss.item():.6f} e_w={e_w:.1e} e_b={e_b:.1e} e_bh={e_bh:.1e} "
                              f"e_dpre={e_dp:.1e} pad_ok={pad_ok} correct {got_correct}/{corr_ref}")
     return ok

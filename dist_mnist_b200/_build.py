@@ -26,7 +26,7 @@ CUDA_SOURCES = ["gemm_sm90.cu", "head_sm90.cu", "ps_apply_sm90.cu", "p2p_sm90.cu
                 "clip_sm90.cu", "nvls_sm90.cu", "executor.cu", "fused_exec.cu", "api.cu"]
 CXX_SOURCES = ["host_runtime.cpp", "loader_api.cpp"]
 HEADERS = ["common.cuh", "protocol.h", "fused.h", "loader.h", "trace.h", "lr_schedule.h", "grad_clip.cuh",
-           "activation.cuh"]
+           "activation.cuh", "loss.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

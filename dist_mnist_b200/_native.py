@@ -22,7 +22,7 @@ MAX_WORKERS = 32
 
 PUSH_LOCAL, PUSH_MAILBOX, PUSH_ATOMIC = 0, 1, 2
 EPI_TRANSPOSED, EPI_ROWMAJOR_PUSH = 0, 1
-LOSS_BOOK, LOSS_XENT = 0, 1
+LOSS_BOOK, LOSS_XENT, LOSS_SIGMOID_XENT, LOSS_MSE, LOSS_HINGE = range(5)   # protocol.h LossKind
 OPT_SGD, OPT_ADAM, OPT_MOMENTUM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3, 4
 OPT_ADADELTA, OPT_FTRL, OPT_PROXIMAL_ADAGRAD, OPT_PROXIMAL_SGD = 5, 6, 7, 8
 OPT_ADAGRAD_DA = 9
@@ -32,6 +32,11 @@ LR_CONSTANT, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_NATURAL_EXP, LR_POLYNOMIAL, LR_
 MAX_LR_BOUNDARIES = 8   # protocol.h kMaxLrBoundaries
 CLIP_OFF, CLIP_GLOBAL_NORM, CLIP_NORM, CLIP_VALUE = range(4)   # protocol.h GradClipKind
 ACT_NONE, ACT_RELU, ACT_RELU6, ACT_LEAKY_RELU, ACT_ELU, ACT_SELU, ACT_SIGMOID, ACT_TANH = range(8)   # protocol.h ActivationKind
+
+
+def fused_head_code(act: int, loss_kind: int, label_smoothing: float) -> int:
+    """The `head` argument of dm_fused_max_lanes: the activation, the loss and whether the labels are smoothed."""
+    return act + 256 * loss_kind + 65536 * int(label_smoothing != 0.0)
 
 
 class PushTarget(C.Structure):
@@ -89,7 +94,7 @@ class HeadParams(C.Structure):
         ("seq_ptr", C.c_void_p), ("inbox", C.c_void_p), ("ps_global_step", C.c_void_p),
         ("nslots", C.c_uint32), ("n_inbox", C.c_uint32),
         ("debug_ts", C.c_void_p),
-        ("act", C.c_int), ("act_pad_", C.c_int),
+        ("act", C.c_int), ("label_smoothing", C.c_float),
     ]
 
 
@@ -166,7 +171,7 @@ class FusedParams(C.Structure):
         ("clear_stop", C.c_uint32), ("wait_acks", C.c_uint32),
         ("clip_kind", C.c_int), ("clip_norm", C.c_float), ("clip_min", C.c_float), ("clip_max", C.c_float),
         ("l2_scale", C.c_float), ("l2_biases", C.c_uint32),
-        ("act", C.c_int), ("act_pad_", C.c_uint32),
+        ("act", C.c_int), ("label_smoothing", C.c_float),
     ]
 
 

@@ -19,8 +19,9 @@ image has no network). New flags select what the reference cannot express (optim
 from __future__ import annotations
 
 import argparse
+import math
 import sys
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import torch
 
@@ -123,6 +124,19 @@ def l2_regularization_from_args(args) -> L2Regularization:
     if args.l2_variables is not None and args.l2_regularization is None:
         raise ValueError("--l2_variables needs --l2_regularization (L2 regularization is off)")
     return L2Regularization(args.l2_regularization, args.l2_variables or "weights")
+
+
+def loss_from_args(args) -> Tuple[Optional[str], float]:
+    """The workers' loss (None: the model's own) and label smoothing of `--loss` and `--label_smoothing`; a smoothing
+    the loss does not take, or one outside [0, 1], is an error."""
+    loss = args.loss if args.loss is not None else mlp.get_model(args.model, args.hidden_units).loss
+    ls = args.label_smoothing
+    if ls is not None:
+        if loss not in mlp.SMOOTHED_LOSSES:
+            raise ValueError(f"--label_smoothing does not apply to --loss {loss} (only {', '.join(mlp.SMOOTHED_LOSSES)})")
+        if not (math.isfinite(ls) and 0.0 <= ls <= 1.0):
+            raise ValueError(f"--label_smoothing must be finite and in [0, 1], got {ls}")
+    return args.loss, 0.0 if ls is None else ls
 
 
 def optimizer_config_from_args(args) -> OptimizerConfig:
@@ -239,6 +253,14 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--activation", choices=list(mlp.ACTIVATIONS), default="relu",
                    help="of every hidden layer (never the logits): TF1's tf.nn.relu, relu6, leaky_relu (alpha 0.2), "
                         "elu, selu, sigmoid or tanh; worker-side only (a ps task ignores it, checkpoints do not store it)")
+    p.add_argument("--loss", choices=list(mlp.LOSSES), default=None,
+                   help="of the workers' classifier head: book (the reference's clipped log loss), xent "
+                        "(tf.losses.softmax_cross_entropy), sigmoid_xent (tf.losses.sigmoid_cross_entropy), mse "
+                        "(tf.losses.mean_squared_error on the logits) or hinge (tf.losses.hinge_loss); unset: the "
+                        "model's own (book for book, xent for zhihu and wide); worker-side only")
+    p.add_argument("--label_smoothing", type=float, default=None,
+                   help="xent / sigmoid_xent: tf.losses' label_smoothing, finite, in [0, 1] (unset: 0); the accuracy "
+                        "still compares with the raw labels; worker-side only")
     p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
     p.add_argument("--backend", choices=["auto", "cuda", "cpu"], default="auto")
     p.add_argument("--push_mode", choices=["mailbox", "atomic"], default="mailbox")
@@ -312,8 +334,13 @@ def run(args: argparse.Namespace) -> int:
         raise ValueError(f"unknown job name {args.job_name!r} (expected 'ps' or 'worker')")
     cluster.task_endpoint(args.job_name, args.task_index)
     backend = resolve_backend(args.backend)
-    # the activation is the workers' alone: the ps stores and applies variables whatever computed their gradients
-    spec = mlp.get_model(args.model, args.hidden_units, args.activation if args.job_name == "worker" else "relu")
+    # the activation and the loss are the workers' alone: the ps stores and applies variables whatever computed their
+    # gradients
+    if args.job_name == "worker":
+        loss, label_smoothing = loss_from_args(args)
+        spec = mlp.get_model(args.model, args.hidden_units, args.activation, loss, label_smoothing)
+    else:
+        spec = mlp.get_model(args.model, args.hidden_units)
     opt = optimizer_config_from_args(args)
     cfg = engine_config_from_args(args, backend)
     cfg.validate(opt)

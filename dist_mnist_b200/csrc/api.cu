@@ -11,8 +11,10 @@
 #include <stdio.h>
 #include <string>
 
+#include "activation.cuh"
 #include "common.cuh"
 #include "fused.h"
+#include "loss.cuh"
 #include "protocol.h"
 
 namespace dm {
@@ -273,10 +275,15 @@ int dm_launch_fused(const void* maps, const void* params, int lanes, void* strea
   return 0;
 }
 // How many clusters of the fused step a batch of `batch` rows runs can be co-resident on the device: with (clip != 0)
-// or without gradient clipping, with (l2 != 0) or without L2 regularization, under activation `act` (ActivationKind)
-int dm_fused_max_lanes(int dev, int batch, int clip, int l2, int act, int* out) {
+// or without gradient clipping, with (l2 != 0) or without L2 regularization, and with the head `head` selects:
+// head = act + 256 loss_kind + 65536 smoothed, the ActivationKind of the hidden layer, the LossKind, and 1 if the labels
+// are smoothed (so a plain ActivationKind asks for LOSS_BOOK without smoothing)
+int dm_fused_max_lanes(int dev, int batch, int clip, int l2, int head, int* out) {
+  const int act = head & 255, loss_kind = (head >> 8) & 255, smoothed = head >> 16;
+  if (!dm::act_valid(act) || !dm::loss_valid(loss_kind) || (smoothed != 0 && smoothed != 1))
+    return fail("dm_fused_max_lanes(head)", cudaErrorInvalidValue);
   DM_CUDA(cudaSetDevice(dev));
-  DM_CUDA(dm::fused_max_lanes(batch, clip != 0, l2 != 0, act, out));
+  DM_CUDA(dm::fused_max_lanes(batch, clip != 0, l2 != 0, dm::fused_general_head(act, loss_kind, smoothed), out));
   return 0;
 }
 int dm_fused_smem_bytes(int batch) { return static_cast<int>(dm::fused_smem_bytes(batch)); }

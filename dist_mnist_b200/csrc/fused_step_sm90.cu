@@ -48,6 +48,7 @@
 #include "activation.cuh"
 #include "fused.h"
 #include "grad_clip.cuh"
+#include "loss.cuh"
 
 namespace dm {
 
@@ -198,10 +199,12 @@ __device__ __forceinline__ void fs_wait_acks(const FusedParams& p, uint32_t need
 // handed the staging tile over (named barrier 2) instead of after its barrier #1. Every CTA sums w*w over what it
 // owns (its W k-slice, W_last / b of its 16 hidden units, b_last on CTA 0) into one partial on CTA 0, whose publisher
 // adds the 8 partials in a fixed order and reports loss + S * sum / 2.
-// kAct: the hidden layer's activation is FusedParams::act (activation.cuh) instead of the ReLU: f where the hidden
-// values hv are formed, f'(hv) where dpre is. Units >= H stay 0; padding rows (>= B) hold f(bias), which nothing
-// reads: their dlogits are 0, so they add 0 to dpre and to every sum, and the loss and correct count mask them.
-template <int kMaxTiles, bool kClip, bool kL2, bool kAct>
+// kGeneral: the general head. The hidden layer's activation is FusedParams::act (activation.cuh) instead of the ReLU:
+// f where the hidden values hv are formed, f'(hv) where dpre is. Units >= H stay 0; padding rows (>= B) hold f(bias),
+// which nothing reads: their dlogits are 0, so they add 0 to dpre and to every sum, and the loss and correct count mask
+// them. The loss is any LossKind (loss.cuh) and the labels the head reads are smoothed by FusedParams::label_smoothing;
+// the correct count compares with the raw labels. Without it the head runs LOSS_BOOK or an unsmoothed LOSS_XENT.
+template <int kMaxTiles, bool kClip, bool kL2, bool kGeneral>
 __global__ void __launch_bounds__(kFsThreads, 1)
 fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant__ FusedParams p) {
   constexpr bool kMulti = kMaxTiles > 1;
@@ -655,7 +658,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             const float4 t = *reinterpret_cast<const float4*>(red + (s * 128 + et) * 4);
             acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
           }
-          if constexpr (kAct) {
+          if constexpr (kGeneral) {
             hv[0] = unit_ok ? act_forward(p.act, acc.x + bias) : 0.f;
             hv[1] = unit_ok ? act_forward(p.act, acc.y + bias) : 0.f;
             hv[2] = unit_ok ? act_forward(p.act, acc.z + bias) : 0.f;
@@ -688,16 +691,18 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
           }
           float dot = (a0 + a1) + (a2 + a3);
           dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-          const float y = ylab;
+          // the label the loss sees: smoothed (general head) for real classes, still 0 for padded ones
+          float y = ylab;
+          if constexpr (kGeneral) y = hc_ok ? smooth_label(p.loss_kind, ylab, p.label_smoothing, C) : 0.f;
           const float z = hc_ok ? dot + blast : -INFINITY;
-          float zmax = z, ybest = hc_ok ? y : -INFINITY, ysum = y;
+          float zmax = z, ybest = hc_ok ? ylab : -INFINITY, ysum = y;
 #pragma unroll
           for (int o = 16; o > 1; o >>= 1) {   // over the 16 classes (lane bit 0 is the k-half: both halves hold the same)
             zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
             ybest = fmaxf(ybest, __shfl_xor_sync(0xffffffffu, ybest, o));
             ysum += __shfl_xor_sync(0xffffffffu, ysum, o);
           }
-          int zarg = (hc_ok && z == zmax) ? hc : kFsMaxC, yarg = (hc_ok && y == ybest) ? hc : kFsMaxC;  // first maximum wins
+          int zarg = (hc_ok && z == zmax) ? hc : kFsMaxC, yarg = (hc_ok && ylab == ybest) ? hc : kFsMaxC;  // first maximum wins
           const float e = hc_ok ? __expf(z - zmax) : 0.f;
           float esum = e;
 #pragma unroll
@@ -718,11 +723,13 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             for (int o = 16; o > 1; o >>= 1) gp += __shfl_xor_sync(0xffffffffu, gp, o);
             dl = pc * (g - gp);
             lc = hc_ok ? -k * y * __logf(fminf(fmaxf(pc, 1e-10f), 1.0f)) : 0.f;
-          } else {
+          } else if (!kGeneral || p.loss_kind == LOSS_XENT) {
             // L = (1/B) sum_b -sum_c y*log_softmax(z);  dz = (p*sum(y) - y)/B   (DS:35)
             const float k = 1.f / static_cast<float>(B);
             dl = k * (pc * ysum - y);
             lc = hc_ok ? -k * y * (z - (zmax + __logf(esum))) : 0.f;
+          } else if (hc_ok) {
+            elementwise_loss(p.loss_kind, z, y, 1.f / (static_cast<float>(B) * static_cast<float>(C)), dl, lc);
           }
           if (kh == 0) dls[q * kFsMaxC + hc] = (hrow_ok && hc_ok) ? dl : 0.f;
           float loss_part = (hrow_ok && kh == 0) ? lc : 0.f;
@@ -753,7 +760,7 @@ fused_step_kernel(const __grid_constant__ FusedMaps maps, const __grid_constant_
             if (4 * c4 + 2 < kFsPart - 1) dw[4 * c4 + 2] = fmaf(d.z, hv[i], dw[4 * c4 + 2]);
             if (4 * c4 + 3 < kFsPart - 1) dw[4 * c4 + 3] = fmaf(d.w, hv[i], dw[4 * c4 + 3]);
           }
-          if constexpr (kAct) dp[i] = act_backward(p.act, hv[i], dh);   // (finite f': 0 for rows >= B as well)
+          if constexpr (kGeneral) dp[i] = act_backward(p.act, hv[i], dh);   // (finite f': 0 for rows >= B as well)
           else dp[i] = hv[i] > 0.f ? dh : 0.f;       // rows >= B carry dlogits == 0 -> dp == 0
           dbh += dp[i];
         }
@@ -1084,10 +1091,9 @@ static cudaLaunchConfig_t fused_launch_config(int lanes, int B, cudaStream_t str
 
 using FusedKernel = void (*)(const FusedMaps, const FusedParams);
 
-// The instantiation that runs batch B, with or without the clip and the L2 term, under activation `act`
-// (ActivationKind; ACT_NONE, the value of a zero-initialised FusedParams, and ACT_RELU run the ReLU instantiations).
-static FusedKernel fused_kernel(int B, bool clip, bool l2, int act) {
-  static const FusedKernel table[2][2][2][2] = {   // [act > ACT_RELU][l2][clip][multi-tile], in load order
+// The instantiation that runs batch B, with or without the clip, the L2 term and the general head (fused_general_head).
+static FusedKernel fused_kernel(int B, bool clip, bool l2, bool general) {
+  static const FusedKernel table[2][2][2][2] = {   // [general][l2][clip][multi-tile], in load order
       {{{fused_step_kernel<1, false, false, false>, fused_step_kernel<kFsMaxTiles, false, false, false>},
         {fused_step_kernel<1, true, false, false>, fused_step_kernel<kFsMaxTiles, true, false, false>}},
        {{fused_step_kernel<1, false, true, false>, fused_step_kernel<kFsMaxTiles, false, true, false>},
@@ -1096,17 +1102,17 @@ static FusedKernel fused_kernel(int B, bool clip, bool l2, int act) {
         {fused_step_kernel<1, true, false, true>, fused_step_kernel<kFsMaxTiles, true, false, true>}},
        {{fused_step_kernel<1, false, true, true>, fused_step_kernel<kFsMaxTiles, false, true, true>},
         {fused_step_kernel<1, true, true, true>, fused_step_kernel<kFsMaxTiles, true, true, true>}}}};
-  return table[act > ACT_RELU][l2][clip][fused_multi_tile(B)];
+  return table[general][l2][clip][fused_multi_tile(B)];
 }
 
-// Every instantiation: shared-memory opt-in + force-load (DESIGN §7). A one-tile (32) and a multi-tile batch, under
-// the ReLU and under one of the other activations, stand for all.
+// Every instantiation: shared-memory opt-in + force-load (DESIGN §7). A one-tile (32) and a multi-tile batch, with and
+// without the general head, stand for all.
 cudaError_t prepare_fused_kernels() {
-  for (const int act : {ACT_RELU, ACT_TANH})
+  for (const bool general : {false, true})
     for (const bool l2 : {false, true})
       for (const bool clip : {false, true})
         for (const int B : {32, 32 * kFsMaxTiles}) {
-          const FusedKernel k = fused_kernel(B, clip, l2, act);
+          const FusedKernel k = fused_kernel(B, clip, l2, general);
           cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                static_cast<int>(fused_smem_bytes(B)));
           cudaFuncAttributes a;
@@ -1120,20 +1126,21 @@ cudaError_t launch_fused_step(const FusedMaps& maps, const FusedParams& p, int l
   if (lanes < 1 || p.B < 1 || p.B > 32 * kFsMaxTiles || p.H < 1 || p.H > 128 || p.C < 1 || p.C > kFsPart - 1 ||
       (p.I & 3) || p.n_shards < 1 || p.n_shards > kFusedMaxShards || p.nslots < 1 || p.clip_kind < CLIP_OFF ||
       p.clip_kind > CLIP_VALUE || !(p.l2_scale >= 0.f && p.l2_scale < INFINITY) ||
-      (p.l2_scale != 0.f && p.shard[0].push.mode == PUSH_ATOMIC) || !act_valid(p.act))
+      (p.l2_scale != 0.f && p.shard[0].push.mode == PUSH_ATOMIC) || !act_valid(p.act) || !loss_valid(p.loss_kind) ||
+      !label_smoothing_valid(p.loss_kind, p.label_smoothing))
     return cudaErrorInvalidValue;
   for (int r = 0; r < kFusedCluster; ++r)
     if (p.slice[r].kc_count < 0 || p.slice[r].kc_count > kFusedMaxChunks) return cudaErrorInvalidValue;
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(lanes, p.B, stream, attr);
-  return cudaLaunchKernelEx(&cfg, fused_kernel(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f, p.act), maps, p);
+  const bool general = fused_general_head(p.act, p.loss_kind, p.label_smoothing);
+  return cudaLaunchKernelEx(&cfg, fused_kernel(p.B, p.clip_kind != CLIP_OFF, p.l2_scale != 0.f, general), maps, p);
 }
 
-cudaError_t fused_max_lanes(int B, bool clip, bool l2, int act, int* out) {
-  if (!act_valid(act)) return cudaErrorInvalidValue;
+cudaError_t fused_max_lanes(int B, bool clip, bool l2, bool general, int* out) {
   cudaLaunchAttribute attr[1];
   const cudaLaunchConfig_t cfg = fused_launch_config(1, B, nullptr, attr);
-  return cudaOccupancyMaxActiveClusters(out, fused_kernel(B, clip, l2, act), &cfg);
+  return cudaOccupancyMaxActiveClusters(out, fused_kernel(B, clip, l2, general), &cfg);
 }
 
 }  // namespace dm

@@ -6,7 +6,9 @@
 //   p      = softmax(logits)
 //   loss   = LOSS_BOOK: -mean_{B x C}(labels * log(clip(p, 1e-10, 1)))     reference DS:52-53
 //            LOSS_XENT: mean_B(softmax_cross_entropy_with_logits)           reference DS:35
-//   correct= #(argmax logits == argmax labels)                              (accuracy numerator, SURVEY K12)
+//            LOSS_SIGMOID_XENT, LOSS_MSE, LOSS_HINGE: mean_{B x C} of the element's loss (loss.cuh)
+//            (the cross-entropies on labels smoothed by label_smoothing)
+//   correct= #(argmax logits == argmax raw labels)                          (accuracy numerator, SURVEY K12)
 //   dlogits, dW_last = dlogits^T . h, db_last = sum_B dlogits
 //   dpre   = (dlogits . W_last) * act'(h)       -> [B][H] buffer consumed by the wgmma dW / dX GEMMs
 //   db_hid = sum_B dpre
@@ -20,6 +22,7 @@
 // Replaces reference ops DS:52-53 + their gradients from DS:103 (SURVEY K3, K4, K5, part of K6, K12).
 #include "activation.cuh"
 #include "common.cuh"
+#include "loss.cuh"
 #include "protocol.h"
 
 namespace dm {
@@ -167,7 +170,7 @@ __global__ void __launch_bounds__(kHeadThreads, 1) head_kernel(const __grid_cons
       const int b = b0 + (lane >> 4);
       const bool row_ok = b < B;
       const int bs = row_ok ? b : B - 1;
-      const float y = (c_ok && row_ok) ? p.labels[static_cast<size_t>(bs) * C + c] : 0.f;  // in flight during the dot
+      const float ylab = (c_ok && row_ok) ? p.labels[static_cast<size_t>(bs) * C + c] : 0.f;  // in flight during the dot
       float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
       if (h_smem) {
         const float* hrow = sHs + bs * kHeadSlice;
@@ -191,15 +194,17 @@ __global__ void __launch_bounds__(kHeadThreads, 1) head_kernel(const __grid_cons
         for (int k = H4; k < H; ++k) a0 = fmaf(ld_act(p.h, rowoff + k, p.act_bf16), wrow[k], a0);
       }
       const float z = c_ok ? (a0 + a1) + (a2 + a3) + bias : -INFINITY;
+      // the label the loss sees (smoothed, for a real class); the correct count compares with the raw one
+      const float y = c_ok && p.label_smoothing != 0.f ? smooth_label(p.loss_kind, ylab, p.label_smoothing, C) : ylab;
       // row reductions over the 16-lane group
-      float zmax = z, ybest = c_ok ? y : -INFINITY, ysum = y;
+      float zmax = z, ybest = c_ok ? ylab : -INFINITY, ysum = y;
 #pragma unroll
       for (int o = 8; o > 0; o >>= 1) {
         zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
         ybest = fmaxf(ybest, __shfl_xor_sync(0xffffffffu, ybest, o));
         ysum += __shfl_xor_sync(0xffffffffu, ysum, o);
       }
-      int zarg = (c_ok && z == zmax) ? c : kMaxC, yarg = (c_ok && y == ybest) ? c : kMaxC;  // first maximum wins
+      int zarg = (c_ok && z == zmax) ? c : kMaxC, yarg = (c_ok && ylab == ybest) ? c : kMaxC;  // first maximum wins
       const float e = c_ok ? __expf(z - zmax) : 0.f;
       float esum = e;
 #pragma unroll
@@ -220,11 +225,13 @@ __global__ void __launch_bounds__(kHeadThreads, 1) head_kernel(const __grid_cons
         for (int o = 8; o > 0; o >>= 1) gp += __shfl_xor_sync(0xffffffffu, gp, o);
         dl = pc * (g - gp);
         lc = c_ok ? -k * y * __logf(fminf(fmaxf(pc, 1e-10f), 1.0f)) : 0.f;
-      } else {
+      } else if (p.loss_kind == LOSS_XENT) {
         // L = (1/B) sum_b -sum_c y*log_softmax(z);  dz = (p*sum(y) - y)/B
         const float k = 1.f / static_cast<float>(B);
         dl = k * (pc * ysum - y);
         lc = c_ok ? -k * y * (z - (zmax + __logf(esum))) : 0.f;
+      } else if (c_ok) {
+        elementwise_loss(p.loss_kind, z, y, 1.f / (static_cast<float>(B) * static_cast<float>(C)), dl, lc);
       }
       if (row_ok) {
         sLogit[b * kMaxC + c] = c_ok ? dl : 0.f;
@@ -347,7 +354,9 @@ size_t head_smem_bytes(int B_pad, int H, int C) {
 constexpr int kHeadMaxSmem = 224 * 1024;
 
 cudaError_t launch_head(const HeadParams& p, cudaStream_t stream) {
-  if (p.C > kMaxC || p.B > kMaxB || p.B_pad > kMaxB || !act_valid(p.act)) return cudaErrorInvalidValue;
+  if (p.C > kMaxC || p.B > kMaxB || p.B_pad > kMaxB || !act_valid(p.act) || !loss_valid(p.loss_kind) ||
+      !label_smoothing_valid(p.loss_kind, p.label_smoothing))
+    return cudaErrorInvalidValue;
   const size_t smem = head_smem_bytes(p.B_pad, p.H, p.C);
   if (smem > static_cast<size_t>(kHeadMaxSmem)) return cudaErrorInvalidValue;
   const int grid = (p.H + kHeadSlice - 1) / kHeadSlice;

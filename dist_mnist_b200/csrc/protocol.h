@@ -97,10 +97,14 @@ enum ActivationKind : int {
   ACT_TANH = 7,
 };
 
-// Softmax-cross-entropy head (last dense layer + loss + its gradients), see head_sm90.cu
+// Loss of the classifier head (last dense layer + loss + its gradients), see head_sm90.cu; loss.cuh has the ones after
+// LOSS_XENT and the label smoothing, models/mlp.py the reference
 enum LossKind : int {
-  LOSS_BOOK = 0,  // -mean over B x C of labels * log(clip(softmax, 1e-10, 1))   (reference DS:52-53)
-  LOSS_XENT = 1,  // mean over B of softmax_cross_entropy_with_logits               (reference DS:35)
+  LOSS_BOOK = 0,          // -mean over B x C of labels * log(clip(softmax, 1e-10, 1))   (reference DS:52-53)
+  LOSS_XENT = 1,          // mean over B of softmax_cross_entropy_with_logits               (reference DS:35)
+  LOSS_SIGMOID_XENT = 2,  // mean over B x C of sigmoid_cross_entropy_with_logits (tf.losses.sigmoid_cross_entropy)
+  LOSS_MSE = 3,           // mean over B x C of (logits - labels)^2 (tf.losses.mean_squared_error)
+  LOSS_HINGE = 4,         // mean over B x C of relu(1 - (2 labels - 1) logits) (tf.losses.hinge_loss)
 };
 
 struct StepResult {  // written once per worker step, read back by the host (D2H)
@@ -142,7 +146,8 @@ struct HeadParams {
   long long* debug_ts;       // optional clock64() phase stamps of CTA 0; null in production
   int act;                   // ActivationKind of the last hidden layer, whose act'(h) gives dpre (appended; ACT_NONE,
                              // the value of a zero-initialised block, is read as ACT_RELU)
-  int act_pad_;
+  float label_smoothing;     // LOSS_XENT, LOSS_SIGMOID_XENT: labels y' = y (1 - ls) + ls / C or + 0.5 ls (loss.cuh);
+                             // the correct count still compares with the raw labels. 0 for every other loss
 };
 
 // One unit of PS apply work.
@@ -354,10 +359,11 @@ struct FusedParams {
   // weights (and, with l2_biases, the biases) before the clip. 0 runs the unregularized instantiations.
   float l2_scale;          // finite, >= 0
   uint32_t l2_biases;      // 1: the biases are regularized too
-  // activation of the hidden layer (ActivationKind, appended): ACT_NONE (a zero-initialised block) and ACT_RELU run
-  // the ReLU instantiations, any other the ones that read this field
+  // activation of the hidden layer (ActivationKind, appended), and the label smoothing of the loss (appended; see
+  // HeadParams::label_smoothing): ACT_NONE (a zero-initialised block) or ACT_RELU under LOSS_BOOK or an unsmoothed
+  // LOSS_XENT runs the ReLU instantiations, anything else the general-head ones, which read act, loss_kind and this
   int act;
-  uint32_t act_pad_;
+  float label_smoothing;
 };
 enum GradClipKind : int {
   CLIP_OFF = 0,

@@ -55,19 +55,38 @@ def activation_code(name: str) -> int:
     return ACTIVATIONS.index(name) + 1
 
 
+# Losses of the classifier head (`--loss`). The index of a name is its protocol.h LossKind code. "book" is the
+# reference's clipped log loss (DS:52-53), the others are TF 1.15's tf.losses functions on the logits with weight 1:
+# softmax_cross_entropy, sigmoid_cross_entropy, mean_squared_error and hinge_loss.
+LOSSES = ("book", "xent", "sigmoid_xent", "mse", "hinge")
+SMOOTHED_LOSSES = ("xent", "sigmoid_xent")   # the losses that take a label_smoothing
+
+
+def loss_code(name: str) -> int:
+    """protocol.h LossKind of a loss (LOSS_BOOK = 0, LOSS_XENT = 1, ...)."""
+    return LOSSES.index(name)
+
+
 @dataclass(frozen=True)
 class MLPSpec:
     name: str = "book"
     in_features: int = IMAGE_PIXELS * IMAGE_PIXELS
     hidden: Tuple[int, ...] = (100,)
     num_classes: int = 10
-    loss: str = "book"   # "book" | "xent"
+    loss: str = "book"   # one of LOSSES
     init: str = "book"   # "book" (truncated normal, DS:41-47) | "glorot" (tf.layers.dense default)
     activation: str = "relu"   # of every hidden layer, one of ACTIVATIONS (the logits layer has none)
+    label_smoothing: float = 0.0   # xent / sigmoid_xent: tf.losses' label_smoothing, in [0, 1]
 
     def __post_init__(self):
         if self.activation not in ACTIVATIONS:
             raise ValueError(f"unknown activation {self.activation!r} (expected {' | '.join(ACTIVATIONS)})")
+        if self.loss not in LOSSES:
+            raise ValueError(f"unknown loss {self.loss!r} (expected {' | '.join(LOSSES)})")
+        if not (math.isfinite(self.label_smoothing) and 0.0 <= self.label_smoothing <= 1.0):
+            raise ValueError(f"label_smoothing must be finite and in [0, 1], got {self.label_smoothing}")
+        if self.label_smoothing != 0.0 and self.loss not in SMOOTHED_LOSSES:
+            raise ValueError(f"label_smoothing does not apply to loss {self.loss} (only {', '.join(SMOOTHED_LOSSES)})")
 
     @property
     def layer_sizes(self) -> List[Tuple[int, int]]:
@@ -123,7 +142,10 @@ def wide_model() -> MLPSpec:
     return MLPSpec(name="wide", hidden=(1024, 1024), loss="xent", init="glorot")
 
 
-def get_model(name: str, hidden_units: int = 100, activation: str = "relu") -> MLPSpec:
+def get_model(name: str, hidden_units: int = 100, activation: str = "relu", loss: str | None = None,
+              label_smoothing: float = 0.0) -> MLPSpec:
+    """The model `name` with a hidden-layer activation and a loss (None: the model's own, book for book, xent for
+    zhihu and wide) smoothed by `label_smoothing`."""
     if name == "book":
         spec = book_model(hidden_units)
     elif name == "zhihu":
@@ -132,7 +154,8 @@ def get_model(name: str, hidden_units: int = 100, activation: str = "relu") -> M
         spec = wide_model()
     else:
         raise ValueError(f"unknown model {name!r} (expected book | zhihu | wide)")
-    return spec if activation == "relu" else replace(spec, activation=activation)
+    return replace(spec, activation=activation, loss=spec.loss if loss is None else loss,
+                   label_smoothing=float(label_smoothing))
 
 
 # ----------------------------------------------------------------------------------------------
@@ -245,12 +268,46 @@ def forward_logits(spec: MLPSpec, params: Dict[str, torch.Tensor], x: torch.Tens
     raise AssertionError("unreachable")
 
 
-def loss_from_logits(spec: MLPSpec, logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
-    if spec.loss == "book":
-        y = torch.softmax(logits, dim=-1)
-        return -(labels * torch.log(torch.clamp(y, 1e-10, 1.0))).mean()  # DS:52-53 (mean over B x C)
+def smooth_labels(spec: MLPSpec, labels: torch.Tensor) -> torch.Tensor:
+    """The labels the loss sees: tf.losses' label smoothing of `spec.loss`, in fp32, with ls its fp32 value:
+    y' = y * fl(1 - ls) + ls / C (xent, an fp32 division) or y * fl(1 - ls) + fl(0.5 * ls) (sigmoid_xent), the constants
+    formed in double as TF forms them, the multiply and the add rounded separately (so fp64 labels get the fp32 y' as
+    well). ls = 0 returns the labels."""
+    if spec.label_smoothing == 0.0:
+        return labels
+    f32 = torch.float32
+    ls = torch.tensor(spec.label_smoothing, dtype=f32)
+    keep = torch.tensor(1.0 - float(ls), dtype=f32)
     if spec.loss == "xent":
-        return -(labels * torch.log_softmax(logits, dim=-1)).sum(dim=-1).mean()  # DS:35
+        add = ls / torch.tensor(float(labels.shape[-1]), dtype=f32)
+    else:
+        add = torch.tensor(0.5 * float(ls), dtype=f32)
+    return (labels.to(f32) * keep + add).to(labels.dtype)
+
+
+def _sigmoid_xent_terms(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(per-element loss, sigmoid(z)) of tf.nn.sigmoid_cross_entropy_with_logits: max(z, 0) - z y + log1p(exp(-|z|)),
+    and the sigmoid formed from the same e = exp(-|z|) <= 1 (1 / (1 + e) for z >= 0, e / (1 + e) below), so nothing
+    overflows."""
+    e = torch.exp(-z.abs())
+    d = 1 + e
+    return torch.clamp(z, min=0.0) - z * y + torch.log1p(e), torch.where(z >= 0, 1 / d, e / d)
+
+
+def loss_from_logits(spec: MLPSpec, logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+    """The mean loss of `spec.loss` (labels smoothed by `spec.label_smoothing`), as TF's loss tensor computes it."""
+    y = smooth_labels(spec, labels)
+    if spec.loss == "book":
+        p = torch.softmax(logits, dim=-1)
+        return -(labels * torch.log(torch.clamp(p, 1e-10, 1.0))).mean()  # DS:52-53 (mean over B x C)
+    if spec.loss == "xent":
+        return -(y * torch.log_softmax(logits, dim=-1)).sum(dim=-1).mean()  # DS:35
+    if spec.loss == "sigmoid_xent":
+        return _sigmoid_xent_terms(logits, y)[0].mean()
+    if spec.loss == "mse":
+        return ((logits - y) * (logits - y)).mean()
+    if spec.loss == "hinge":
+        return torch.relu(1 - (2 * y - 1) * logits).mean()
     raise ValueError(spec.loss)
 
 
@@ -273,15 +330,31 @@ def manual_loss_and_grads(spec: MLPSpec, params: Dict[str, torch.Tensor], x: tor
     logits, acts = forward_logits(spec, params, x)
     B, Cn = logits.shape
     p = torch.softmax(logits, dim=-1)
+    y = smooth_labels(spec, labels)
+    k = 1.0 / (B * Cn)   # the elementwise losses' 1 / (B C)
     if spec.loss == "book":
-        k = 1.0 / (B * Cn)
         loss = -(labels * torch.log(torch.clamp(p, 1e-10, 1.0))).sum() * k
         passes = (p >= 1e-10) & (p <= 1.0)
         g = torch.where(passes, -k * labels / p.clamp_min(1e-38), torch.zeros_like(p))
         dz = p * (g - (g * p).sum(dim=-1, keepdim=True))
+    elif spec.loss == "xent":
+        loss = -(y * torch.log_softmax(logits, dim=-1)).sum(dim=-1).mean()
+        dz = (p * y.sum(dim=-1, keepdim=True) - y) / B
+    elif spec.loss == "sigmoid_xent":
+        elem, sig = _sigmoid_xent_terms(logits, y)
+        loss = elem.mean()
+        dz = k * (sig - y)
+    elif spec.loss == "mse":
+        d = logits - y
+        loss = (d * d).mean()
+        dz = (2 * k) * d   # TF's SquaredDifference gradient: (2 grad)(z - y)
+    elif spec.loss == "hinge":
+        ypm = 2 * y - 1
+        m = 1 - ypm * logits
+        loss = torch.relu(m).mean()
+        dz = torch.where(m > 0, (-k) * ypm, torch.zeros_like(m))
     else:
-        loss = -(labels * torch.log_softmax(logits, dim=-1)).sum(dim=-1).mean()
-        dz = (p * labels.sum(dim=-1, keepdim=True) - labels) / B
+        raise ValueError(spec.loss)
     grads: Dict[str, torch.Tensor] = {}
     d = dz
     for i in range(len(names) - 1, -1, -1):

@@ -2,7 +2,8 @@
 accuracy + small-variable gradients + their parameter-server push.
 
 Reference parity: /root/reference/distributed_server-basic.py:52-53 (book loss), :35 (xent loss),
-and the gradient ops `minimize` builds for them at :103.
+and the gradient ops `minimize` builds for them at :103; the other losses are TF 1.15's tf.losses functions
+(models/mlp.py).
 """
 from __future__ import annotations
 
@@ -33,6 +34,7 @@ class HeadPlan:
 
 def head_plan(*, h_ptr: int, labels_ptr: int, w_last_ptr: int, b_last_ptr: int, dpre_ptr: int, result_ptr: int,
               B: int, B_pad: int, H: int, num_classes: int, loss_kind: int, act_bf16: bool, act: int = N.ACT_RELU,
+              label_smoothing: float = 0.0,
               push: Optional[N.PushTarget] = None, push_bh: Optional[N.PushTarget] = None,
               push_bl: Optional[N.PushTarget] = None,
               off_w_last: int = 0, off_b_last: int = 0, off_b_hidden: int = 0,
@@ -42,7 +44,8 @@ def head_plan(*, h_ptr: int, labels_ptr: int, w_last_ptr: int, b_last_ptr: int, 
     assert num_classes <= MAX_CLASSES and B <= B_pad <= MAX_BATCH
     p = N.HeadParams()
     p.B, p.B_pad, p.H, p.C = B, B_pad, H, num_classes
-    p.loss_kind = loss_kind
+    p.loss_kind = loss_kind   # LossKind; the cross-entropies see labels smoothed by label_smoothing
+    p.label_smoothing = label_smoothing
     p.act_bf16 = int(act_bf16)
     p.act = act   # ActivationKind of the last hidden layer: dpre = (dlogits . W_last) * act'(h)
     p.ldh = H if ldh is None else ldh

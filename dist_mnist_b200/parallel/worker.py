@@ -617,7 +617,7 @@ class Worker:
             w_last_ptr=self.ps_segs[wl.ps].addr("params", wl.offset * 4),
             b_last_ptr=self.ps_segs[bl.ps].addr("params", bl.offset * 4), dpre_ptr=self.dact[L - 1].data_ptr(),
             result_ptr=self._eval_res.data_ptr(), B=self.batch, B_pad=self.B_pad, H=sizes[L - 1][0],
-            num_classes=spec.num_classes, loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT,
+            num_classes=spec.num_classes, loss_kind=mlp.loss_code(spec.loss), label_smoothing=spec.label_smoothing,
             act_bf16=cfg.dtype == "bf16", act=act_code, compute_grads=False, ldh=self.act[L - 1].shape[1]))
         torch.cuda.synchronize(self.device)
         clip = self.opt.clip.enabled or self.opt.l2.enabled
@@ -672,7 +672,7 @@ class Worker:
                 b_last_ptr=self.ps_segs[bl.ps].addr("params", bl.offset * 4),
                 dpre_ptr=dact[L - 1].data_ptr(), result_ptr=rd.value, B=self.batch, B_pad=self.B_pad,
                 H=sizes[L - 1][0], num_classes=spec.num_classes,
-                loss_kind=N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT, act_bf16=cfg.dtype == "bf16",
+                loss_kind=mlp.loss_code(spec.loss), label_smoothing=spec.label_smoothing, act_bf16=cfg.dtype == "bf16",
                 act=act_code, push=push(wl.ps), push_bh=push(hb.ps), push_bl=push(bl.ps),
                 off_w_last=wl.offset, off_b_last=bl.offset, off_b_hidden=hb.offset,
                 item_w_last_base=wl.item_base, item_b_last=bl.item_base, item_b_hidden_base=hb.item_base,
@@ -787,9 +787,9 @@ class Worker:
         I, H = spec.layer_sizes[0]
         Cn = spec.num_classes
         max_lanes = C.c_int(0)
+        head = N.fused_head_code(mlp.activation_code(spec.activation), mlp.loss_code(spec.loss), spec.label_smoothing)
         N.check(self.lib.dm_fused_max_lanes(self.device, self.batch, int(self.opt.clip.enabled),
-                                            int(self.opt.l2.enabled), mlp.activation_code(spec.activation),
-                                            C.byref(max_lanes)), "fused occupancy")
+                                            int(self.opt.l2.enabled), head, C.byref(max_lanes)), "fused occupancy")
         free = max_lanes.value
         if cfg.push_mode == "mailbox" and cfg.ps_mode == "persistent":
             # a resident serve kernel packed into clusters on our GPU holds that many of the device's cluster slots
@@ -825,7 +825,7 @@ class Worker:
         hw = lay.by_name[names[0][0]]
         p = N.FusedParams()
         p.B, p.H, p.C, p.I = self.batch, H, Cn, I
-        p.loss_kind = N.LOSS_BOOK if spec.loss == "book" else N.LOSS_XENT
+        p.loss_kind = mlp.loss_code(spec.loss)
         p.ldw = hw.ld
         p.strict = int(cfg.strict_steps)
         # shards this worker pushes to, the global-step owner first (same order as the inbox entries)
@@ -858,7 +858,8 @@ class Worker:
                             if cfg.push_mode == "atomic" else None)
         self.opt.clip.fill_native(p)   # CLIP_OFF: the unclipped kernels
         self.opt.l2.fill_native(p)     # l2_scale 0: the unregularized kernels
-        p.act = mlp.activation_code(spec.activation)   # ACT_RELU: the ReLU kernels
+        p.act = mlp.activation_code(spec.activation)   # ACT_RELU, book / xent, no smoothing: the ReLU kernels
+        p.label_smoothing = spec.label_smoothing
         if os.environ.get("DM_FUSED_DEBUG_TS") == "1":
             self._fx_dbg = torch.zeros(64, dtype=torch.int64, device=f"cuda:{self.device}")
             p.debug_ts = self._fx_dbg.data_ptr()
