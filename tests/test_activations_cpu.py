@@ -3,11 +3,8 @@ against hand-computed TF1 values at the kinks, at +-0 and at saturation; the han
 in fp64; flag and config validation; the fp64 push checker's bound and its activation mutants; lock-step cpu runs;
 and a multi-process CLI run."""
 import math
-import os
-import socket
-import subprocess
-import sys
 
+import _harness
 import pytest
 import torch
 
@@ -19,7 +16,6 @@ from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
 from dist_mnist_b200.session import InProcessCluster
 from dist_mnist_b200.utils import data
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = torch.float32
 S, SA = mlp.SELU_SCALE, mlp.SELU_SCALE_ALPHA
 
@@ -252,44 +248,14 @@ def test_lockstep_trajectory(name, kind, shards):
 # ---------------------------------------------------------------------------------------------------------------
 # the CLI
 # ---------------------------------------------------------------------------------------------------------------
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(900)
 def test_cli_sigmoid_one_ps_two_workers():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--learning_rate", "0.001", "--log_every", "1000", "--lanes", "1", "--activation", "sigmoid"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in (1, 0)]
-    try:
-        outs = [_finish(w, 780) for w in ws]
-        outp = _finish(ps, 60)
-    finally:
-        for p in [ps, *ws]:   # a failed run leaves no task behind
-            if p.poll() is None:
-                p.kill()
-                p.wait()
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in (1, 0)]
+        outs = [t.finish(w, 780) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
         assert "done: local_steps=" in o, o

@@ -4,6 +4,7 @@ bench_tools/fused_push_ref, over the fused engine's batch, hidden, input and cla
 row split, the atomic push, a clip and L2 (so that every activation instantiation of the fused kernel runs), and the
 graph engine at 784-H-10; lock-step trajectories against fp32 torch (300 strict fused steps, 100 graph-engine zhihu
 steps, one bf16 run); and `evaluate` on both engines."""
+import _harness
 import pytest
 
 from bench_tools import fused_push_ref as R
@@ -29,33 +30,6 @@ def test_kernel_epilogues_and_head(name):
 # ---------------------------------------------------------------------------------------------------------------
 # pushes against fp64
 # ---------------------------------------------------------------------------------------------------------------
-def _cluster(case, nps=1, sharding="round_robin", engine="fused", lanes=1, nslots=4, strict=True,
-             push_mode="mailbox", lr=0.0, clip=None, l2=None):
-    from dist_mnist_b200.parallel.config import EngineConfig, GradClip, L2Regularization, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-
-    kw = {"strict_steps": strict} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=lanes, nslots=nslots, sharding=sharding,
-                       push_mode=push_mode, **kw)
-    opt = OptimizerConfig("sgd", lr, clip=clip or GradClip(), l2=l2 or L2Regularization())
-    cl = InProcessCluster(case.spec, opt, cfg, batch_size=case.batch, num_ps=nps, params=case.params)
-    assert cl.worker.engine == engine
-    return cl
-
-
-def _step(w, x, y):
-    out = w.step(x, y)
-    w.wait_applied()
-    return R.Step(R.pushed(w, out.seq), float(out.loss), int(out.correct))
-
-
-def _check(tag, got, case, x, y, ref=None):
-    assert R.check_case(case, x, y) == [], tag
-    v = R.compare(got, ref or R.reference(case.spec, case.params, x, y))
-    print(f"[{tag}] {v.line()}", flush=True)
-    assert v.ok, (tag, v.worst, v.where)
-
-
 # every batch edge at H = 100, hidden-size and input edges, C = 2 / 10 / 11, both losses
 SHAPES = [(100, 10, 784, b, "book") for b in (1, 32, 33, 100, 256)]
 SHAPES += [(1, 2, 228, 32, "xent"), (128, 11, 1024, 256, "xent"), (1, 10, 784, 33, "book"), (128, 2, 228, 1, "xent"),
@@ -67,9 +41,9 @@ SHAPES += [(1, 2, 228, 32, "xent"), (128, 11, 1024, 256, "xent"), (1, 10, 784, 3
 def test_fused_push_is_inside_the_fp64_bound(name, shape):
     case = R.case_for(shape, activation=name)
     x, y = case.batches[0]
-    with _cluster(case) as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused {case.name} seed {case.seed}", got, case, x, y)
+    with _harness.cluster(case) as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused {case.name} seed {case.seed}", got, case, x, y)
 
 
 @pytest.mark.parametrize("name", ACTS)
@@ -78,7 +52,7 @@ def test_fused_pipelined_sharded_and_atomic_pushes(name):
     import torch
 
     case = R.case_for((100, 10, 784, 100, "book"), n_batches=8, seed=3, activation=name)
-    with _cluster(case, lanes=4, nslots=8, strict=False) as cl:
+    with _harness.cluster(case, lanes=4, nslots=8, strict=False) as cl:
         w = cl.worker
         loader = w.make_loader(torch.cat([b[0] for b in case.batches]), torch.cat([b[1] for b in case.batches]),
                                seed=0, shuffle=False)
@@ -90,11 +64,11 @@ def test_fused_pipelined_sharded_and_atomic_pushes(name):
     assert hits == list(range(8)), hits
 
     x, y = case.batches[0]
-    with _cluster(case, nps=2, sharding="row_split") as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused row_split 2 ps {case.name}", got, case, x, y)
+    with _harness.cluster(case, nps=2, sharding="row_split") as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused row_split 2 ps {case.name}", got, case, x, y)
 
-    with _cluster(case, push_mode="atomic", lr=1.0) as cl:
+    with _harness.cluster(case, push_mode="atomic", lr=1.0) as cl:
         w = cl.worker
         out = w.step(x, y)
         w.wait_applied()
@@ -104,7 +78,7 @@ def test_fused_pipelined_sharded_and_atomic_pushes(name):
     for n in R.VARS:
         ref.bounds[n] = ref.bounds[n] + 2.0 ** -24 * torch.maximum(p0[n].double().abs(), p1[n].double().abs())
     g = {n: p0[n].double() - p1[n].double() for n in R.VARS}
-    _check(f"fused atomic {case.name}", R.Step(g, float(out.loss), int(out.correct)), case, x, y, ref)
+    _harness.check(f"fused atomic {case.name}", R.Step(g, float(out.loss), int(out.correct)), case, x, y, ref)
 
 
 @pytest.mark.parametrize("B", [32, 33])
@@ -121,8 +95,8 @@ def test_fused_clip_and_l2_instantiations(name, B):
     wide = GradClip("value", value_min=-1e3, value_max=1e3)
     l2 = L2Regularization(1e-3, "all")
     for clip, reg in ((wide, None), (None, l2), (wide, l2)):
-        with _cluster(case, clip=clip, l2=reg) as cl:
-            got = _step(cl.worker, x, y)
+        with _harness.cluster(case, clip=clip, l2=reg) as cl:
+            got = _harness.step(cl.worker, x, y)
         ref = R.reference(case.spec, case.params, x, y)
         if reg is not None:
             for n in R.VARS:
@@ -132,7 +106,7 @@ def test_fused_clip_and_l2_instantiations(name, B):
             term = reg.scale * sum(float((case.params[n].double() ** 2).sum()) / 2 for n in R.VARS)
             ref.loss += term
             ref.loss_bound += 2.0 ** -16 * (term + abs(ref.loss))   # the fp32 sum of S w w / 2 over the variables
-        _check(f"fused clip={clip and clip.kind} l2={reg is not None} {case.name}", got, case, x, y, ref)
+        _harness.check(f"fused clip={clip and clip.kind} l2={reg is not None} {case.name}", got, case, x, y, ref)
         assert torch.isfinite(got.grads["hid_w"]).all()
 
 
@@ -141,52 +115,19 @@ def test_fused_clip_and_l2_instantiations(name, B):
 def test_graph_push_is_inside_the_fp64_bound(name, H, B):
     case = R.case_for((H, 10, 784, B, "book"), activation=name)
     x, y = case.batches[0]
-    with _cluster(case, engine="graph") as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"graph {case.name}", got, case, x, y)
+    with _harness.cluster(case, engine="graph") as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"graph {case.name}", got, case, x, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # trajectories and evaluate
 # ---------------------------------------------------------------------------------------------------------------
 def _lockstep(name, engine, model, steps, dtype="fp32", loss_tol=1e-2, param_tol=5e-3):
-    from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-    from dist_mnist_b200.utils import data
+    from dist_mnist_b200.parallel.config import OptimizerConfig
 
-    ds = data.synthetic_mnist(8192, seed=5)
-    spec = mlp.get_model(model, 100, name)
-    params = mlp.init_params(spec, seed=11)
-    ref_p = {k: t.clone() for k, t in params.items()}
-    opt = OptimizerConfig("sgd", 5e-2)
-    kw = {"strict_steps": True} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=1, nslots=8, dtype=dtype, **kw)
-    worst = 0.0
-    with InProcessCluster(spec, opt, cfg, batch_size=32, num_ps=1, params=params) as cl:
-        w = cl.worker
-        assert w.engine == engine
-        if engine == "fused":
-            loader = w.make_loader(ds.images, ds.labels, seed=7)
-            twin = w.make_loader(ds.images, ds.labels, seed=7, epoch_feed=False)
-            outs = []
-            for n in (7, 93, steps - 100):
-                outs += list(w.run_steps(n, loader, wait_applied=True))
-            batches = [twin.next_batch() for _ in outs]
-        else:
-            it = data.BatchIterator(ds, seed=3)
-            outs, batches = [], []
-            for _ in range(steps):
-                batches.append(it.next_batch(32))
-                outs.append(w.step(*batches[-1]))
-                w.wait_applied()
-        assert len(outs) == steps and w.read_global_step() == steps
-        for o, (x, y) in zip(outs, batches):
-            loss, grads, _ = mlp.manual_loss_and_grads(spec, ref_p, x, y)
-            for k in ref_p:
-                ref_p[k] = ref_p[k] - opt.lr * grads[k]
-            worst = max(worst, abs(o.loss - float(loss)) / abs(float(loss)))
-        got = w.read_variables()
-    errs = {k: float((got[k] - ref_p[k]).norm() / (ref_p[k].norm() + 1e-9)) for k in got}
+    worst, errs = _harness.gpu_lockstep(mlp.get_model(model, 100, name), OptimizerConfig("sgd", 5e-2), engine, steps,
+                                        dtype)
     perr = max(errs.values())
     print(f"[{engine} {model} {dtype} {name}] {steps} steps: worst per-step loss rel err {worst:.2e}, "
           f"param rel err {perr:.2e} ({max(errs, key=errs.get)})")

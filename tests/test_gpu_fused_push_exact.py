@@ -7,6 +7,7 @@ Fused engine: one strict step at every shape of the matrix; 3 x nslots steps in 
 with every mailbox slot reused; 4 lanes in flight (pushes matched to batches as a multiset); both 2-shard layouts;
 push == apply (atomic); and a push against the next batch's reference, which must fail. Graph engine: the same checker
 at 784-H-10. Every check prints the worst err / bound per variable."""
+import _harness
 import pytest
 
 from bench_tools import fused_push_ref as R
@@ -16,42 +17,13 @@ pytestmark = pytest.mark.gpu
 MATRIX = R.shape_matrix()
 
 
-def _cluster(case, nps=1, sharding="round_robin", engine="fused", lanes=1, nslots=4, strict=True,
-             push_mode="mailbox", lr=0.0):
-    from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-
-    kw = {"strict_steps": strict} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=lanes, nslots=nslots, sharding=sharding,
-                       push_mode=push_mode, **kw)
-    cl = InProcessCluster(case.spec, OptimizerConfig("sgd", lr), cfg,
-                          batch_size=case.batch, num_ps=nps, params=case.params)
-    assert cl.worker.engine == engine
-    return cl
-
-
-def _step(w, x, y):
-    """One step; what it pushed, the loss and the correct count it reported."""
-    out = w.step(x, y)
-    w.wait_applied()
-    return R.Step(R.pushed(w, out.seq), float(out.loss), int(out.correct))
-
-
-def _check(tag, got, case, x, y, expect_ok=True):
-    assert R.check_case(case, x, y) == [], tag
-    v = R.compare(got, R.reference(case.spec, case.params, x, y))
-    print(f"[{tag}] {v.line()}", flush=True)
-    assert v.ok == expect_ok, (tag, v.worst, v.where)
-    return v
-
-
 @pytest.mark.parametrize("name,shape,saturate", MATRIX, ids=[m[0] for m in MATRIX])
 def test_fused_push_is_inside_the_fp64_bound(name, shape, saturate):
     case = R.case_for(shape, saturate)
     x, y = case.batches[0]
-    with _cluster(case) as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused {name} seed {case.seed} (random shapes from seed {R.RANDOM_SEED})", got, case, x, y)
+    with _harness.cluster(case) as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused {name} seed {case.seed} (random shapes from seed {R.RANDOM_SEED})", got, case, x, y)
     if shape[1] == 1:   # one class: softmax is 1, every gradient and the loss are exactly zero
         assert all(float(g.abs().max()) == 0.0 for g in got.grads.values()) and got.loss == 0.0
 
@@ -77,7 +49,7 @@ def test_fused_pushes_of_consecutive_steps_in_one_launch(B):
 
     ns = 4
     case = R.case_for((100, 10, 784, B, "book"), n_batches=3 * ns, seed=2)
-    with _cluster(case, nslots=ns) as cl:
+    with _harness.cluster(case, nslots=ns) as cl:
         w = cl.worker
         loader, twin = _loader_batches(w, case)
         seq = 0
@@ -91,10 +63,10 @@ def test_fused_pushes_of_consecutive_steps_in_one_launch(B):
                 x, y = twin.next_batch()
                 assert torch.equal(x, case.batches[i][0])
                 got = R.Step(R.pushed(w, o.seq), float(o.loss), int(o.correct))
-                _check(f"fused B{B} step {o.seq} strict={strict}", got, case, x, y)
+                _harness.check(f"fused B{B} step {o.seq} strict={strict}", got, case, x, y)
                 if i >= ns:   # what the slot held before this push: it must not pass for this step's
-                    _check(f"fused B{B} step {o.seq} vs the batch of the slot's previous push (must fail)", got,
-                           case, *case.batches[i - ns], expect_ok=False)
+                    _harness.check(f"fused B{B} step {o.seq} vs the batch of the slot's previous push (must fail)",
+                                   got, case, *case.batches[i - ns], expect_ok=False)
             seq += ns
 
 
@@ -103,7 +75,7 @@ def test_fused_pipelined_pushes_match_their_batches(B):
     """4 lanes in flight, not strict, 8 steps into 8 mailbox slots: the 8 pushes and the 8 batches match one to one,
     whichever lane ran which step."""
     case = R.case_for((100, 10, 784, B, "book"), n_batches=8, seed=3)
-    with _cluster(case, lanes=4, nslots=8, strict=False) as cl:
+    with _harness.cluster(case, lanes=4, nslots=8, strict=False) as cl:
         w = cl.worker
         loader, twin = _loader_batches(w, case)
         outs = list(w.run_steps(8, loader, wait_applied=True))
@@ -130,9 +102,9 @@ SHARDED = [((100, 10, 784, 100, "book"), 2, "row_split"), ((72, 10, 1024, 256, "
 def test_fused_sharded_push_is_inside_the_fp64_bound(shape, nps, sharding):
     case = R.case_for(shape)
     x, y = case.batches[0]
-    with _cluster(case, nps=nps, sharding=sharding) as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused {sharding} over {nps} ps {shape}", got, case, x, y)
+    with _harness.cluster(case, nps=nps, sharding=sharding) as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused {sharding} over {nps} ps {shape}", got, case, x, y)
 
 
 @pytest.mark.parametrize("shape", [(100, 10, 784, 32, "book"), (128, 11, 1024, 256, "xent")],
@@ -144,7 +116,7 @@ def test_fused_atomic_push_is_inside_the_fp64_bound(shape):
 
     case = R.case_for(shape)
     x, y = case.batches[0]
-    with _cluster(case, push_mode="atomic", lr=1.0) as cl:
+    with _harness.cluster(case, push_mode="atomic", lr=1.0) as cl:
         w = cl.worker
         out = w.step(x, y)
         w.wait_applied()
@@ -168,17 +140,17 @@ def test_graph_push_is_inside_the_fp64_bound(H, B):
     operands, head with IEEE division, dW GEMM on tf32 dpre. The bound needs no change (see the module docstring)."""
     case = R.case_for((H, 10, 784, B, "book"))
     x, y = case.batches[0]
-    with _cluster(case, engine="graph") as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"graph H{H} B{B}", got, case, x, y)
+    with _harness.cluster(case, engine="graph") as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"graph H{H} B{B}", got, case, x, y)
 
 
 def test_push_against_the_next_batch_fails_the_bound():
     """Negative control on real pushes: a fused push is far outside the bound of the batch after it."""
     case = R.case_for((100, 10, 784, 32, "book"), n_batches=2, seed=4)
     (x0, y0), (x1, y1) = case.batches
-    with _cluster(case) as cl:
-        got = _step(cl.worker, x0, y0)
-    _check("fused push of batch 0 vs its own batch", got, case, x0, y0)
-    v = _check("fused push of batch 0 vs batch 1 (must fail)", got, case, x1, y1, expect_ok=False)
+    with _harness.cluster(case) as cl:
+        got = _harness.step(cl.worker, x0, y0)
+    _harness.check("fused push of batch 0 vs its own batch", got, case, x0, y0)
+    v = _harness.check("fused push of batch 0 vs batch 1 (must fail)", got, case, x1, y1, expect_ok=False)
     assert v.max > 10.0, v.worst

@@ -3,6 +3,7 @@ plus fl(S * w) (isolating the L2 term from tf32 error), alone and under every cl
 sizes, hidden sizes and shardings and on the graph engine (book and zhihu, fp32 and bf16); the reported loss against
 the unregularized one plus the fp64 L2 term; lock-step trajectories against fp32 PyTorch with the reference L2 (300
 fused steps, 100 graph steps); bit-identical repeated runs; and group graphs."""
+import _harness
 import pytest
 
 from bench_tools.fused_push_ref import pushed
@@ -140,42 +141,14 @@ def _ref_l2_step(spec, params, x, y, lr, l2):
 
 def _lockstep(engine, steps):
     from dist_mnist_b200.models import mlp
-    from dist_mnist_b200.parallel.config import EngineConfig, L2Regularization, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-    from dist_mnist_b200.utils import data
+    from dist_mnist_b200.parallel.config import L2Regularization, OptimizerConfig
 
-    ds = data.synthetic_mnist(8192, seed=5)
     spec = mlp.book_model(100)
-    params = mlp.init_params(spec, seed=11)
-    ref_p = {k: t.clone() for k, t in params.items()}
     l2 = L2Regularization(5e-3, "all")
     opt = OptimizerConfig("sgd", 5e-2, l2=l2)
-    kw = {"strict_steps": True} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=1, nslots=8, **kw)
-    worst = 0.0
-    with InProcessCluster(spec, opt, cfg, batch_size=32, num_ps=1, params=params) as cl:
-        w = cl.worker
-        assert w.engine == engine
-        if engine == "fused":
-            loader = w.make_loader(ds.images, ds.labels, seed=7)
-            twin = w.make_loader(ds.images, ds.labels, seed=7, epoch_feed=False)
-            outs = []
-            for n in (7, 93, 200):
-                outs += list(w.run_steps(n, loader, wait_applied=True))
-            batches = [twin.next_batch() for _ in outs]
-        else:
-            it = data.BatchIterator(ds, seed=3)
-            outs, batches = [], []
-            for _ in range(steps):
-                batches.append(it.next_batch(32))
-                outs.append(w.step(*batches[-1]))
-                w.wait_applied()
-        assert len(outs) == steps and w.read_global_step() == steps
-        for o, (x, y) in zip(outs, batches):
-            lref = _ref_l2_step(spec, ref_p, x, y, opt.lr, l2)
-            worst = max(worst, abs(o.loss - lref) / abs(lref))
-        got = w.read_variables()
-    perr = max(float((got[k] - ref_p[k]).norm() / (ref_p[k].norm() + 1e-9)) for k in got)
+    worst, errs = _harness.gpu_lockstep(spec, opt, engine, steps,
+                                        ref_update=lambda p, x, y: _ref_l2_step(spec, p, x, y, opt.lr, l2))
+    perr = max(errs.values())
     print(f"[{engine} lock-step L2] {steps} steps: worst per-step loss rel err {worst:.2e}, param rel err {perr:.2e}")
     assert worst < 1e-2
     assert perr < 5e-3

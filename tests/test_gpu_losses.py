@@ -4,6 +4,7 @@ bench_tools/fused_push_ref, at fused batches 32, 100 and 256, 4 pipelined lanes,
 a clip and L2, under the ReLU and tanh (so that every general-head instantiation of the fused kernel runs), and the graph
 engine at 784-H-10; lock-step trajectories against fp32 torch (300 strict fused steps, 100 graph-engine zhihu steps, one
 bf16 run); and `evaluate` on both engines and of the moving averages."""
+import _harness
 import pytest
 
 from bench_tools import fused_push_ref as R
@@ -27,33 +28,6 @@ def test_head_kernel(loss, ls):
 # ---------------------------------------------------------------------------------------------------------------
 # pushes against fp64
 # ---------------------------------------------------------------------------------------------------------------
-def _cluster(case, nps=1, sharding="round_robin", engine="fused", lanes=1, nslots=4, strict=True,
-             push_mode="mailbox", lr=0.0, clip=None, l2=None):
-    from dist_mnist_b200.parallel.config import EngineConfig, GradClip, L2Regularization, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-
-    kw = {"strict_steps": strict} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=lanes, nslots=nslots, sharding=sharding,
-                       push_mode=push_mode, **kw)
-    opt = OptimizerConfig("sgd", lr, clip=clip or GradClip(), l2=l2 or L2Regularization())
-    cl = InProcessCluster(case.spec, opt, cfg, batch_size=case.batch, num_ps=nps, params=case.params)
-    assert cl.worker.engine == engine
-    return cl
-
-
-def _step(w, x, y):
-    out = w.step(x, y)
-    w.wait_applied()
-    return R.Step(R.pushed(w, out.seq), float(out.loss), int(out.correct))
-
-
-def _check(tag, got, case, x, y, ref=None):
-    assert R.check_case(case, x, y) == [], tag
-    v = R.compare(got, ref or R.reference(case.spec, case.params, x, y))
-    print(f"[{tag}] {v.line()}", flush=True)
-    assert v.ok, (tag, v.worst, v.where)
-
-
 SHAPES = [(100, 10, 784, b) for b in (32, 100, 256)] + [(1, 2, 228, 1), (128, 11, 1024, 33)]
 
 
@@ -63,9 +37,9 @@ SHAPES = [(100, 10, 784, b) for b in (32, 100, 256)] + [(1, 2, 228, 1), (128, 11
 def test_fused_push_is_inside_the_fp64_bound(loss, ls, shape, act):
     case = R.case_for((*shape, loss), activation=act, label_smoothing=ls)
     x, y = case.batches[0]
-    with _cluster(case) as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused {case.name} seed {case.seed}", got, case, x, y)
+    with _harness.cluster(case) as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused {case.name} seed {case.seed}", got, case, x, y)
 
 
 @pytest.mark.parametrize("loss,ls", SETTINGS, ids=IDS)
@@ -74,7 +48,7 @@ def test_fused_pipelined_sharded_and_atomic_pushes(loss, ls):
     import torch
 
     case = R.case_for((100, 10, 784, 100, loss), n_batches=8, seed=3, label_smoothing=ls)
-    with _cluster(case, lanes=4, nslots=8, strict=False) as cl:
+    with _harness.cluster(case, lanes=4, nslots=8, strict=False) as cl:
         w = cl.worker
         loader = w.make_loader(torch.cat([b[0] for b in case.batches]), torch.cat([b[1] for b in case.batches]),
                                seed=0, shuffle=False)
@@ -86,11 +60,11 @@ def test_fused_pipelined_sharded_and_atomic_pushes(loss, ls):
     assert hits == list(range(8)), hits
 
     x, y = case.batches[0]
-    with _cluster(case, nps=2, sharding="row_split") as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"fused row_split 2 ps {case.name}", got, case, x, y)
+    with _harness.cluster(case, nps=2, sharding="row_split") as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"fused row_split 2 ps {case.name}", got, case, x, y)
 
-    with _cluster(case, push_mode="atomic", lr=1.0) as cl:
+    with _harness.cluster(case, push_mode="atomic", lr=1.0) as cl:
         w = cl.worker
         out = w.step(x, y)
         w.wait_applied()
@@ -100,7 +74,7 @@ def test_fused_pipelined_sharded_and_atomic_pushes(loss, ls):
     for n in R.VARS:
         ref.bounds[n] = ref.bounds[n] + 2.0 ** -24 * torch.maximum(p0[n].double().abs(), p1[n].double().abs())
     g = {n: p0[n].double() - p1[n].double() for n in R.VARS}
-    _check(f"fused atomic {case.name}", R.Step(g, float(out.loss), int(out.correct)), case, x, y, ref)
+    _harness.check(f"fused atomic {case.name}", R.Step(g, float(out.loss), int(out.correct)), case, x, y, ref)
 
 
 @pytest.mark.parametrize("act", ["relu", "tanh"])
@@ -118,8 +92,8 @@ def test_fused_clip_and_l2_instantiations(loss, ls, B, act):
     wide = GradClip("value", value_min=-1e3, value_max=1e3)
     l2 = L2Regularization(1e-3, "all")
     for clip, reg in ((wide, None), (None, l2), (wide, l2)):
-        with _cluster(case, clip=clip, l2=reg) as cl:
-            got = _step(cl.worker, x, y)
+        with _harness.cluster(case, clip=clip, l2=reg) as cl:
+            got = _harness.step(cl.worker, x, y)
         ref = R.reference(case.spec, case.params, x, y)
         if reg is not None:
             for n in R.VARS:
@@ -129,7 +103,7 @@ def test_fused_clip_and_l2_instantiations(loss, ls, B, act):
             term = reg.scale * sum(float((case.params[n].double() ** 2).sum()) / 2 for n in R.VARS)
             ref.loss += term
             ref.loss_bound += 2.0 ** -16 * (term + abs(ref.loss))   # the fp32 sum of S w w / 2 over the variables
-        _check(f"fused clip={clip and clip.kind} l2={reg is not None} {case.name}", got, case, x, y, ref)
+        _harness.check(f"fused clip={clip and clip.kind} l2={reg is not None} {case.name}", got, case, x, y, ref)
         assert torch.isfinite(got.grads["hid_w"]).all()
 
 
@@ -138,52 +112,19 @@ def test_fused_clip_and_l2_instantiations(loss, ls, B, act):
 def test_graph_push_is_inside_the_fp64_bound(loss, ls, H, B):
     case = R.case_for((H, 10, 784, B, loss), label_smoothing=ls)
     x, y = case.batches[0]
-    with _cluster(case, engine="graph") as cl:
-        got = _step(cl.worker, x, y)
-    _check(f"graph {case.name}", got, case, x, y)
+    with _harness.cluster(case, engine="graph") as cl:
+        got = _harness.step(cl.worker, x, y)
+    _harness.check(f"graph {case.name}", got, case, x, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # trajectories and evaluate
 # ---------------------------------------------------------------------------------------------------------------
 def _lockstep(loss, ls, engine, model, steps, dtype="fp32", loss_tol=1e-2, param_tol=5e-3):
-    from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
-    from dist_mnist_b200.session import InProcessCluster
-    from dist_mnist_b200.utils import data
+    from dist_mnist_b200.parallel.config import OptimizerConfig
 
-    ds = data.synthetic_mnist(8192, seed=5)
     spec = mlp.get_model(model, 100, loss=loss, label_smoothing=ls)
-    params = mlp.init_params(spec, seed=11)
-    ref_p = {k: t.clone() for k, t in params.items()}
-    opt = OptimizerConfig("sgd", 5e-2)
-    kw = {"strict_steps": True} if engine == "fused" else {}
-    cfg = EngineConfig(backend="cuda", engine=engine, lanes=1, nslots=8, dtype=dtype, **kw)
-    worst = 0.0
-    with InProcessCluster(spec, opt, cfg, batch_size=32, num_ps=1, params=params) as cl:
-        w = cl.worker
-        assert w.engine == engine
-        if engine == "fused":
-            loader = w.make_loader(ds.images, ds.labels, seed=7)
-            twin = w.make_loader(ds.images, ds.labels, seed=7, epoch_feed=False)
-            outs = []
-            for n in (7, 93, steps - 100):
-                outs += list(w.run_steps(n, loader, wait_applied=True))
-            batches = [twin.next_batch() for _ in outs]
-        else:
-            it = data.BatchIterator(ds, seed=3)
-            outs, batches = [], []
-            for _ in range(steps):
-                batches.append(it.next_batch(32))
-                outs.append(w.step(*batches[-1]))
-                w.wait_applied()
-        assert len(outs) == steps and w.read_global_step() == steps
-        for o, (x, y) in zip(outs, batches):
-            loss_ref, grads, _ = mlp.manual_loss_and_grads(spec, ref_p, x, y)
-            for k in ref_p:
-                ref_p[k] = ref_p[k] - opt.lr * grads[k]
-            worst = max(worst, abs(o.loss - float(loss_ref)) / abs(float(loss_ref)))
-        got = w.read_variables()
-    errs = {k: float((got[k] - ref_p[k]).norm() / (ref_p[k].norm() + 1e-9)) for k in got}
+    worst, errs = _harness.gpu_lockstep(spec, OptimizerConfig("sgd", 5e-2), engine, steps, dtype)
     perr = max(errs.values())
     print(f"[{engine} {model} {dtype} {loss} ls {ls}] {steps} steps: worst per-step loss rel err {worst:.2e}, "
           f"param rel err {perr:.2e} ({max(errs, key=errs.get)})")

@@ -4,15 +4,12 @@ row_split sharding that end with every item at the global step, and a 1 ps + 2 w
 import json
 import os
 import re
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _schedules():
@@ -168,45 +165,21 @@ def test_eight_lanes_over_two_ps_end_at_the_global_step(layout):
         assert last < 0.5 * first, (first, last)
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cuda", "--gpu", "0", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(420)
 def test_cosine_decay_one_ps_two_workers_three_processes_one_gpu():
     """As tests/test_gpu_optimizers.py::test_nesterov_one_ps_two_workers_three_processes_one_gpu, and the metrics
     file's learning_rate is lr_at(global_step)."""
     from dist_mnist_b200.parallel.config import LrSchedule
 
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "240", "--learning_rate", "0.01", "--log_every", "80", "--lanes", "4",
               "--optimizer", "momentum", "--lr_schedule", "cosine_decay", "--decay_steps", "240", "--alpha", "0.1"]
     d = tempfile.mkdtemp()
     files = [os.path.join(d, f"w{i}.jsonl") for i in range(2)]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common + ["--metrics_file", files[i]]) for i in range(2)]
-    outs_w = [_finish(w, 300) for w in ws]
-    out_p = _finish(ps, 90)
+    with _harness.Tasks(backend="cuda", gpu=0) as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common + ["--metrics_file", files[i]]) for i in range(2)]
+        outs_w = [t.finish(w, 300) for w in ws]
+        out_p = t.finish(ps, 90)
     for w, o in zip(ws, outs_w):
         assert w.returncode == 0, o
         assert "engine=fused" in o, o

@@ -2,17 +2,18 @@
 handles through the rendezvous and train over NVLink peer memory."""
 import json
 import os
-import socket
 import subprocess
 import sys
 import time
 
+import _harness
 import pytest
 import torch
 
+from dist_mnist_b200.session import free_port
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SCRIPT = os.path.join(ROOT, "distributed_server-basic.py")
 
 
 def _need_gpus(n):
@@ -20,28 +21,15 @@ def _need_gpus(n):
         pytest.skip(f"needs {n} GPUs")
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, SCRIPT, "--job_name", job, "--task_index", str(idx), "--ps_hosts", ps_hosts,
-           "--worker_hosts", worker_hosts, "--backend", "cuda", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
 @pytest.mark.parametrize("extra", [[], ["--optimizer", "sgd", "--push_mode", "atomic", "--learning_rate", "0.05"]])
 def test_cli_one_ps_one_worker_two_gpus(extra):
     _need_gpus(2)
-    ps_hosts, worker_hosts = f"127.0.0.1:{_free_port()}", f"127.0.0.1:{_free_port()}"
     common = ["--train_steps", "400", "--learning_rate", "0.001", *extra]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    out0, _ = w0.communicate(timeout=240)
-    outp, _ = ps.communicate(timeout=60)
+    with _harness.Tasks(backend="cuda", n_workers=1) as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        w0 = t.spawn("worker", 0, common)
+        out0 = t.finish(w0, 240)
+        outp = t.finish(ps, 60)
     assert w0.returncode == 0, out0
     assert ps.returncode == 0, outp
     logged = [l for l in out0.splitlines() if l.startswith("Train step ")]
@@ -52,7 +40,7 @@ def test_cli_one_ps_one_worker_two_gpus(extra):
 
 def test_bench_two_gpus_contract():
     _need_gpus(2)
-    port = _free_port()
+    port = free_port()
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr",
            "127.0.0.1", "--master-port", str(port), os.path.join(ROOT, "bench.py"), "--gpus", "2", "--steps", "300",
            "--warmup", "10"]
@@ -80,13 +68,12 @@ def test_documented_topology_one_process_per_gpu(n_ps, extra):
     GPU (3 GPUs; 4 with two row-split ps shards): the shared step counter equals the number of pushes."""
     import re
     _need_gpus(n_ps + 2)
-    ps_hosts = ",".join(f"127.0.0.1:{_free_port()}" for _ in range(n_ps))
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "2000", "--learning_rate", "0.001", "--log_every", "500", *extra]
-    pss = [_spawn("ps", k, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"]) for k in range(n_ps)]
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in range(2)]
-    outs_w = [w.communicate(timeout=300)[0] for w in ws]
-    outs_p = [p.communicate(timeout=90)[0] for p in pss]
+    with _harness.Tasks(backend="cuda", n_ps=n_ps) as t:
+        pss = [t.spawn("ps", k, common + ["--ps_exit_when_done"]) for k in range(n_ps)]
+        ws = [t.spawn("worker", i, common) for i in range(2)]
+        outs_w = [t.finish(w, 300) for w in ws]
+        outs_p = [t.finish(p, 90) for p in pss]
     for w, o in zip(ws, outs_w):
         assert w.returncode == 0 and "engine=fused" in o, o
     for p, o in zip(pss, outs_p):

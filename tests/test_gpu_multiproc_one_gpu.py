@@ -7,40 +7,12 @@ Asserted: the shared step counter equals the number of pushes the workers made (
 training converges, the ps exits once the workers are done; with 2 ps tasks; with async-SGD red.add pushes; and the
 failure path on the cuda backend: a worker crashes (fault injection), is declared dead after --worker_timeout, is
 started again and re-admitted (stop / patch / relaunch of the serve kernel)."""
-import os
 import re
-import socket
-import subprocess
-import sys
 
+import _harness
 import pytest
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SCRIPT = os.path.join(ROOT, "distributed_server-basic.py")
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, SCRIPT, "--job_name", job, "--task_index", str(idx), "--ps_hosts", ps_hosts,
-           "--worker_hosts", worker_hosts, "--backend", "cuda", "--gpu", "0", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
 
 
 def _local_steps(out):
@@ -59,17 +31,16 @@ def _ps_gstep(out):
 @pytest.mark.parametrize("mode", ["mailbox_adam", "atomic_sgd", "two_ps_row_split"])
 def test_one_ps_two_workers_three_processes_one_gpu(mode):
     n_ps = 2 if mode == "two_ps_row_split" else 1
-    ps_hosts = ",".join(f"127.0.0.1:{_free_port()}" for _ in range(n_ps))
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "240", "--learning_rate", "0.001", "--log_every", "80", "--lanes", "4"]
     if mode == "atomic_sgd":
         common += ["--optimizer", "sgd", "--push_mode", "atomic", "--learning_rate", "0.05"]
     if mode == "two_ps_row_split":
         common += ["--sharding", "row_split"]
-    pss = [_spawn("ps", k, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"]) for k in range(n_ps)]
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in range(2)]
-    outs_w = [_finish(w, 300) for w in ws]
-    outs_p = [_finish(p, 90) for p in pss]
+    with _harness.Tasks(backend="cuda", n_ps=n_ps, gpu=0) as t:
+        pss = [t.spawn("ps", k, common + ["--ps_exit_when_done"]) for k in range(n_ps)]
+        ws = [t.spawn("worker", i, common) for i in range(2)]
+        outs_w = [t.finish(w, 300) for w in ws]
+        outs_p = [t.finish(p, 90) for p in pss]
     for w, o in zip(ws, outs_w):
         assert w.returncode == 0, o
         assert "engine=fused" in o, o
@@ -91,23 +62,22 @@ def test_one_ps_two_workers_three_processes_one_gpu(mode):
 
 @pytest.mark.timeout(600)
 def test_worker_crash_timeout_and_restart_on_cuda_one_gpu():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     # --chunk_sleep throttles the workers to <= 1000 steps/s each, so the run (40 000 global steps) outlives the
     # crash, the 6 s failure-detection window and the restart whatever the GPU's time-slicing speed is
     common = ["--train_steps", "40000", "--learning_rate", "0.001", "--log_every", "10000", "--lanes", "2",
               "--chunk_sleep", "0.05"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done", "--worker_timeout", "6"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common + ["--inject_fault", "40"])
-    out1 = _finish(w1, 240)
-    assert w1.returncode == 42 and "[fault injection] worker 1 dies" in out1, out1
-    import time
-    time.sleep(9)      # > --worker_timeout: the ps declares worker 1 dead (mark_worker_dead on the cuda backend)
-    w1b = _spawn("worker", 1, ps_hosts, worker_hosts, common)
-    out1b = _finish(w1b, 300)
-    out0 = _finish(w0, 300)
-    outp = _finish(ps, 90)
+    with _harness.Tasks(backend="cuda", gpu=0) as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done", "--worker_timeout", "6"])
+        w0 = t.spawn("worker", 0, common)
+        w1 = t.spawn("worker", 1, common + ["--inject_fault", "40"])
+        out1 = t.finish(w1, 240)
+        assert w1.returncode == 42 and "[fault injection] worker 1 dies" in out1, out1
+        import time
+        time.sleep(9)      # > --worker_timeout: the ps declares worker 1 dead (mark_worker_dead on the cuda backend)
+        w1b = t.spawn("worker", 1, common)
+        out1b = t.finish(w1b, 300)
+        out0 = t.finish(w0, 300)
+        outp = t.finish(ps, 90)
     assert w1b.returncode == 0, out1b
     assert w0.returncode == 0, out0
     assert ps.returncode == 0, outp

@@ -4,18 +4,14 @@ AdagradDA from a sched_step where fp32 T starts to round), the fused engine in l
 2 ps on the graph engine and with row_split, a 1 ps + 2 worker run in three processes, and a checkpoint resume that
 keeps the mg slot."""
 import dataclasses
-import os
 import re
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _opts():
@@ -178,43 +174,19 @@ def test_checkpoint_resume_keeps_mg():
         assert any(not torch.equal(after[k].cpu(), before["mg"][k].cpu()) for k in after)
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cuda", "--gpu", "0", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(420)
 def test_centered_rmsprop_one_ps_two_workers_three_processes_one_gpu():
     """As tests/test_gpu_multiproc_one_gpu.py: every push applied exactly once, the loss falls, the ps exits. At lr
     1e-3 one such run on an H100 logged 0.23 then 0.97: with 8 pushes in flight, ms - mg^2 of an element whose gradient
     barely varies falls towards epsilon (1e-10) and the normalised step grows, as it can in TF. The run uses the
     reference's default rate, 1e-4, and the batch losses logged every 40 steps must dip below the first."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "240", "--learning_rate", "0.0001", "--log_every", "40", "--lanes", "4",
               "--optimizer", "rmsprop", "--centered"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in range(2)]
-    outs_w = [_finish(w, 300) for w in ws]
-    out_p = _finish(ps, 90)
+    with _harness.Tasks(backend="cuda", gpu=0) as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in range(2)]
+        outs_w = [t.finish(w, 300) for w in ws]
+        out_p = t.finish(ps, 90)
     for w, o in zip(ws, outs_w):
         assert w.returncode == 0, o
         assert "engine=fused" in o, o

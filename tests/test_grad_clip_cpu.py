@@ -2,11 +2,7 @@
 `clip_by_norm` / `clip_by_value` -> `apply_gradients`), cpu backend: the fp32 reference clip against hand-computed TF1
 values, validation of `GradClip` and the CLI flags, lock-step runs checked after every step against an fp32 torch loop
 that clips with the reference, a clipping worker against a ps started without clipping, and a multi-process CLI run."""
-import os
-import socket
-import subprocess
-import sys
-
+import _harness
 import pytest
 import torch
 
@@ -17,10 +13,9 @@ from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, GradClip, OptimizerConfig
 from dist_mnist_b200.parallel.ps import ParameterServer
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster
+from dist_mnist_b200.session import InProcessCluster, free_port
 from dist_mnist_b200.utils import data
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = torch.float32
 
 
@@ -268,18 +263,11 @@ def test_nan_propagates_like_tf1():
     assert all(torch.isnan(v).all() for v in out.values())
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 @pytest.mark.parametrize("kind", ["adam", "momentum"])   # momentum: the ps / worker optimizer dicts are compared
 def test_clipping_worker_connects_to_a_ps_without_clipping(kind):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, OptimizerConfig(kind, 1e-3), cfg)
     try:
         w = Worker(cluster, 0, spec, OptimizerConfig(kind, 1e-3, clip=GradClip("global_norm", clip_norm=1.0)), cfg)
@@ -291,39 +279,15 @@ def test_clipping_worker_connects_to_a_ps_without_clipping(kind):
         ps.close()
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(900)
 def test_cli_clip_by_global_norm_one_ps_two_workers():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--learning_rate", "0.001", "--log_every", "1000", "--lanes", "1", "--clip_gradients", "global_norm",
               "--clip_norm", "0.1"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in (1, 0)]
-    try:
-        outs = [_finish(w, 780) for w in ws]
-        outp = _finish(ps, 60)
-    finally:
-        for p in [ps, *ws]:   # a failed run leaves no task behind
-            if p.poll() is None:
-                p.kill()
-                p.wait()
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in (1, 0)]
+        outs = [t.finish(w, 780) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
         assert "done: local_steps=" in o, o

@@ -1,11 +1,8 @@
 """The workers' classification losses (`--loss`, `--label_smoothing`) on the cpu backend and in the fp64 push checker:
 TF 1.15's tf.losses values, the hand-derived gradients against autograd, the flags, lock-step runs and the CLI."""
 import math
-import os
-import socket
-import subprocess
-import sys
 
+import _harness
 import pytest
 import torch
 import torch.nn.functional as F
@@ -17,8 +14,6 @@ from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, GradClip, L2Regularization, OptimizerConfig
 from dist_mnist_b200.session import InProcessCluster
 from dist_mnist_b200.utils import data
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _head(loss, z, y, ls=0.0):
@@ -314,48 +309,16 @@ def test_evaluate_reports_the_smoothed_loss():
 # ---------------------------------------------------------------------------------------------------------------
 # the CLI
 # ---------------------------------------------------------------------------------------------------------------
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(900)
 def test_cli_sigmoid_xent_smoothed_one_ps_two_workers():
     """The workers train with sigmoid_xent smoothed by 0.1; the ps is given a combination a worker would refuse (mse
     takes no smoothing) and ignores it."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--learning_rate", "0.001", "--log_every", "1000", "--lanes", "1"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts,
-                common + ["--ps_exit_when_done", "--loss", "mse", "--label_smoothing", "0.5"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common + ["--loss", "sigmoid_xent", "--label_smoothing", "0.1"])
-          for i in (1, 0)]
-    try:
-        outs = [_finish(w, 780) for w in ws]
-        outp = _finish(ps, 60)
-    finally:
-        for p in [ps, *ws]:   # a failed run leaves no task behind
-            if p.poll() is None:
-                p.kill()
-                p.wait()
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done", "--loss", "mse", "--label_smoothing", "0.5"])
+        ws = [t.spawn("worker", i, common + ["--loss", "sigmoid_xent", "--label_smoothing", "0.1"]) for i in (1, 0)]
+        outs = [t.finish(w, 780) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
         assert "done: local_steps=" in o, o

@@ -5,11 +5,9 @@ CLI run with a metrics file."""
 import json
 import math
 import os
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
@@ -20,11 +18,9 @@ from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, LrSchedule, OptimizerConfig
 from dist_mnist_b200.parallel.ps import ParameterServer
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster, train_loop
+from dist_mnist_b200.session import InProcessCluster, free_port, train_loop
 from dist_mnist_b200.utils import ckpt, data
 from dist_mnist_b200.utils.metrics import TrainMetricsWriter
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _close(a, b, rel=1e-6):
@@ -252,12 +248,6 @@ def test_lockstep_trajectory_under_a_schedule(rule, sched, mode):
         assert w.read_global_step() == 8
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 @pytest.mark.parametrize("ps_sched,w_sched", [
     (LrSchedule("exponential_decay", decay_steps=10, decay_rate=0.5), LrSchedule()),
     (LrSchedule(), LrSchedule("cosine_decay", decay_steps=10)),
@@ -269,8 +259,7 @@ def _free_port():
 def test_worker_refuses_a_ps_with_another_schedule(ps_sched, w_sched):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, OptimizerConfig("adam", 1e-3, schedule=ps_sched), cfg)
     try:
         w = Worker(cluster, 0, spec, OptimizerConfig("adam", 1e-3, schedule=w_sched), cfg)
@@ -339,36 +328,18 @@ def test_restore_under_another_schedule_is_allowed():
         assert set(cl.worker.read_sched_steps(0)) == {10}
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_cli_exponential_staircase_one_ps_two_workers_metrics_learning_rate():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     sched_flags = ["--lr_schedule", "exponential_decay", "--decay_steps", "100", "--decay_rate", "0.5", "--staircase"]
     common = ["--train_steps", "400", "--learning_rate", "0.05", "--optimizer", "sgd", "--log_every", "50",
               *sched_flags]
     d = tempfile.mkdtemp()
     files = [os.path.join(d, f"w{i}.jsonl") for i in range(2)]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common + ["--metrics_file", files[i]]) for i in (1, 0)]
-    outs = [_finish(w, 120) for w in ws]
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common + ["--metrics_file", files[i]]) for i in (1, 0)]
+        outs = [t.finish(w, 120) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
     assert ps.returncode == 0, outp

@@ -3,12 +3,9 @@ after every optimizer step), cpu backend: `ema_decay_at` against hand-computed T
 the CLI flags, lock-step runs that check parameters, both slot buffers, the shadows and every item's step count after
 every step, the ps / worker agreement on averaging, checkpoint round trips, `evaluate(moving_averages=True)` and a
 multi-process CLI run whose checkpoint holds the shadows."""
-import os
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
@@ -19,10 +16,8 @@ from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, LrSchedule, OptimizerConfig
 from dist_mnist_b200.parallel.ps import ParameterServer
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster, train_loop
+from dist_mnist_b200.session import InProcessCluster, free_port, train_loop
 from dist_mnist_b200.utils import ckpt, data
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _f32(x):
@@ -160,12 +155,6 @@ def test_constant_rate_without_averaging_keeps_the_step_counter_at_zero():
             cl.worker.evaluate(x, y, moving_averages=True)
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 @pytest.mark.parametrize("ps_avg,w_avg", [
     ({"moving_average_decay": 0.99}, {}),
     ({}, {"moving_average_decay": 0.99}),
@@ -175,8 +164,7 @@ def _free_port():
 def test_worker_refuses_a_ps_with_other_moving_averages(ps_avg, w_avg):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, OptimizerConfig("adam", 1e-3, **ps_avg), cfg)
     try:
         w = Worker(cluster, 0, spec, OptimizerConfig("adam", 1e-3, **w_avg), cfg)
@@ -287,34 +275,16 @@ def test_load_variables_reads_either_set():
             assert torch.equal(v[k], before["params"][k]) and torch.equal(e[k], before["ema"][k]), k
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_cli_moving_averages_one_ps_two_workers_checkpoint():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     d = tempfile.mkdtemp()
     common = ["--train_steps", "300", "--learning_rate", "0.05", "--optimizer", "sgd", "--log_every", "100",
               "--moving_average_decay", "0.99"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common + ["--checkpoint_dir", d]) for i in (1, 0)]
-    outs = [_finish(w, 120) for w in ws]
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common + ["--checkpoint_dir", d]) for i in (1, 0)]
+        outs = [t.finish(w, 120) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
     assert ps.returncode == 0, outp

@@ -5,16 +5,13 @@ third slot; checkpoints of the third slot and their refusals; the worker / ps ag
 import ctypes as C
 import dataclasses
 import math
-import os
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
-from bench_tools.gpu_e2e import ref_slots, ref_step, tf1_apply
+from bench_tools.gpu_e2e import tf1_apply
 from dist_mnist_b200 import _native as N
 from dist_mnist_b200 import cli
 from dist_mnist_b200.cluster import ClusterSpec
@@ -23,10 +20,8 @@ from dist_mnist_b200.parallel.config import EngineConfig, LrSchedule, OptimizerC
 from dist_mnist_b200.parallel.ps import ParameterServer, shard_carver
 from dist_mnist_b200.parallel.sharding import build_layout
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster, train_loop
+from dist_mnist_b200.session import InProcessCluster, free_port, train_loop
 from dist_mnist_b200.utils import ckpt, data
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 RULES = {
     "centered": OptimizerConfig("rmsprop", 1e-3, centered=True),
@@ -35,12 +30,6 @@ RULES = {
     "adagrad_da_l1_l2": OptimizerConfig("adagrad_da", 0.1, l1_regularization_strength=1e-4,
                                         l2_regularization_strength=1e-2),
 }
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
 
 
 # ---- config and CLI ---------------------------------------------------------------------------------------------
@@ -292,52 +281,18 @@ def test_shard_carver_adds_mg_last():
             assert on["mg"][0] >= off["ema"][0] + off["ema"][1]
 
 
-def _lockstep(opt, nps, apply_mode, steps=8):
-    spec = mlp.book_model(100)
-    cfg = EngineConfig(backend="cpu", apply_mode=apply_mode)
-    ds = data.synthetic_mnist(512, seed=2)
-    it = data.BatchIterator(ds, seed=0)
-    params = mlp.init_params(spec, seed=5)
-    rp = {k: v.clone() for k, v in params.items()}
-    rm, rv, rg = ref_slots(opt, params, with_mg=True)
-    t = 0
-    with InProcessCluster(spec, opt, cfg, batch_size=32, num_ps=nps, params=params) as cl:
-        w = cl.worker
-        losses = []
-        for i in range(steps):
-            x, y = it.next_batch(32)
-            r = w.step(x, y)
-            w.wait_applied()
-            lref, t = ref_step(spec, rp, rm, rv, t, x, y, opt, lr=opt.lr_at(i), mg=rg)
-            losses.append(r.loss)
-            assert r.loss == pytest.approx(lref, rel=1e-4)
-            got, gm, gv = w.read_variables(), w.read_variables("adam_m"), w.read_variables("adam_v")
-            gg = w.read_variables("mg") if opt.uses_mg else None
-            for k in got:
-                assert torch.allclose(got[k], rp[k], rtol=1e-4, atol=1e-6), (i, k)
-                assert torch.allclose(gm[k], rm[k], rtol=1e-4, atol=1e-7), (i, k)
-                assert torch.allclose(gv[k], rv[k], rtol=1e-4, atol=1e-7), (i, k)
-                if gg is not None:
-                    assert torch.allclose(gg[k], rg[k], rtol=1e-4, atol=1e-7), (i, k)
-            if opt.kind == "adagrad_da":
-                for k in range(nps):
-                    assert set(w.read_sched_steps(k)) == {i + 1}
-        assert w.read_global_step() == steps
-    return losses
-
-
 @pytest.mark.parametrize("apply_mode", ["per_push", "merged"])
 @pytest.mark.parametrize("nps", [1, 2])
 @pytest.mark.parametrize("rule", list(RULES))
 def test_lockstep_trajectory_matches_tf1_formulas(rule, nps, apply_mode):
-    _lockstep(RULES[rule], nps, apply_mode)
+    _harness.cpu_optimizer_lockstep(RULES[rule], nps, apply_mode)
 
 
 @pytest.mark.parametrize("rule", ["centered_momentum", "adagrad_da_l1_l2"])
 def test_lockstep_under_a_schedule_and_moving_averages(rule):
     opt = dataclasses.replace(RULES[rule], schedule=LrSchedule("exponential_decay", decay_steps=2, decay_rate=0.5),
                               moving_average_decay=0.9)
-    _lockstep(opt, 2, "per_push")
+    _harness.cpu_optimizer_lockstep(opt, 2, "per_push")
 
 
 @pytest.mark.parametrize("rule", ["centered", "adagrad_da"])
@@ -430,8 +385,7 @@ def test_checkpoint_refusals_and_older_checkpoints():
 def test_worker_refuses_a_ps_with_another_rule(ps_opt, w_opt):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, ps_opt, cfg)
     try:
         w = Worker(cluster, 0, spec, w_opt, cfg)
@@ -441,32 +395,14 @@ def test_worker_refuses_a_ps_with_another_rule(ps_opt, w_opt):
         ps.close()
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_cli_adagrad_da_one_ps_two_worker_processes():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "300", "--learning_rate", "0.5", "--optimizer", "adagrad_da"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in (1, 0)]
-    outs = [_finish(w, 120) for w in ws]
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in (1, 0)]
+        outs = [t.finish(w, 120) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
     assert ps.returncode == 0, outp

@@ -1,12 +1,9 @@
 """Momentum (with and without Nesterov), Adagrad and RMSProp on the parameter server, cpu backend: the TF1
 `training_ops` formulas step by step (parameters and both slot buffers), their defaults and flags, slot
 initialisation, the ps / worker and checkpoint agreement on the optimizer, and a multi-process CLI run."""
-import os
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
@@ -17,10 +14,9 @@ from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, OptimizerConfig
 from dist_mnist_b200.parallel.ps import ParameterServer
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster, train_loop
+from dist_mnist_b200.session import InProcessCluster, free_port, train_loop
 from dist_mnist_b200.utils import ckpt, data
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 RULES = {
     "momentum": OptimizerConfig("momentum", 1e-2),
@@ -29,12 +25,6 @@ RULES = {
     "rmsprop": OptimizerConfig("rmsprop", 1e-3),
     "rmsprop_mom": OptimizerConfig("rmsprop", 1e-3, momentum=0.9),
 }
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
 
 
 @pytest.mark.parametrize("apply_mode", ["per_push", "merged"])
@@ -154,8 +144,7 @@ def test_slot_initialisation(kind, m0, v0):
 def test_worker_refuses_a_ps_with_another_optimizer(ps_kind, w_kind):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, OptimizerConfig(ps_kind, 1e-3), cfg)
     try:
         w = Worker(cluster, 0, spec, OptimizerConfig(w_kind, 1e-3), cfg)
@@ -206,32 +195,14 @@ def test_adam_checkpoint_is_refused_by_an_rmsprop_run():
         assert ckpt.restore_latest(cl.worker, d) == 10      # Adam <-> SGD restores as before
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_cli_rmsprop_one_ps_two_worker_processes():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "400", "--learning_rate", "0.001", "--optimizer", "rmsprop"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in (1, 0)]
-    outs = [_finish(w, 120) for w in ws]
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in (1, 0)]
+        outs = [t.finish(w, 120) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
         assert o.splitlines()[:2] == ["job name : worker", f"task index : {1 if w is ws[0] else 0}"]

@@ -3,26 +3,21 @@ TF1 `training_ops` formulas pinned by hand-computed one-element values and cross
 defaults, validation and flags, slot initialisation, lock-step runs (parameters and both slot buffers after every step,
 also under a learning-rate schedule and with moving averages), the exact zeros of a large l1, the ps / worker and
 checkpoint agreement on the optimizer, and a multi-process CLI run."""
-import os
-import socket
-import subprocess
-import sys
 import tempfile
 
+import _harness
 import pytest
 import torch
 
-from bench_tools.gpu_e2e import ref_ema, ref_slots, ref_step, tf1_apply
+from bench_tools.gpu_e2e import tf1_apply
 from dist_mnist_b200 import cli
 from dist_mnist_b200.cluster import ClusterSpec
 from dist_mnist_b200.models import mlp
 from dist_mnist_b200.parallel.config import EngineConfig, LrSchedule, OptimizerConfig
 from dist_mnist_b200.parallel.ps import ParameterServer
 from dist_mnist_b200.parallel.worker import Worker
-from dist_mnist_b200.session import InProcessCluster, train_loop
+from dist_mnist_b200.session import InProcessCluster, free_port, train_loop
 from dist_mnist_b200.utils import ckpt, data
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # every rule and branch: l1 > 0 and == 0, lr_power -0.5 and -0.25, shrinkage on and off
 RULES = {
@@ -40,12 +35,6 @@ RULES = {
     "proximal_sgd_l1": OptimizerConfig("proximal_sgd", 0.05, l1_regularization_strength=1e-3,
                                        l2_regularization_strength=1e-2),
 }
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
 
 
 def _one(x):
@@ -222,46 +211,11 @@ def test_slot_initialisation(kind, m0, v0):
                 assert torch.equal(t, torch.full_like(t, want)), (region, k)
 
 
-def _lockstep(opt, nps, apply_mode, steps=8, ema=False):
-    """`steps` lock-step cpu-backend steps against the fp32 reference, with the tolerances of
-    tests/test_optimizers_cpu.py::test_lockstep_trajectory_matches_tf1_formulas; returns (got, reference) params."""
-    spec = mlp.book_model(100)
-    cfg = EngineConfig(backend="cpu", apply_mode=apply_mode)
-    ds = data.synthetic_mnist(512, seed=2)
-    it = data.BatchIterator(ds, seed=0)
-    params = mlp.init_params(spec, seed=5)
-    rp = {k: v.clone() for k, v in params.items()}
-    re = {k: v.clone() for k, v in params.items()}
-    rm, rv = ref_slots(opt, params)
-    t = 0
-    with InProcessCluster(spec, opt, cfg, batch_size=32, num_ps=nps, params=params) as cl:
-        w = cl.worker
-        for i in range(steps):
-            x, y = it.next_batch(32)
-            r = w.step(x, y)
-            w.wait_applied()
-            lref, t = ref_step(spec, rp, rm, rv, t, x, y, opt, lr=opt.lr_at(i))
-            assert r.loss == pytest.approx(lref, rel=1e-4)
-            assert r.seq == i + 1
-            got, gm, gv = w.read_variables(), w.read_variables("adam_m"), w.read_variables("adam_v")
-            for k in got:
-                assert torch.allclose(got[k], rp[k], rtol=1e-4, atol=1e-6), (i, k)
-                assert torch.allclose(gm[k], rm[k], rtol=1e-4, atol=1e-7), (i, k)
-                assert torch.allclose(gv[k], rv[k], rtol=1e-4, atol=1e-7), (i, k)
-            if ema:
-                ref_ema(opt, rp, re, i + 1)
-                ge = w.read_variables("ema")
-                for k in ge:
-                    assert torch.allclose(ge[k], re[k], rtol=1e-4, atol=1e-6), (i, k)
-        assert w.read_global_step() == steps
-    return got, rp
-
-
 @pytest.mark.parametrize("apply_mode", ["per_push", "merged"])
 @pytest.mark.parametrize("nps", [1, 2])
 @pytest.mark.parametrize("rule", list(RULES))
 def test_lockstep_trajectory_matches_tf1_formulas(rule, nps, apply_mode):
-    _lockstep(RULES[rule], nps, apply_mode)
+    _harness.cpu_optimizer_lockstep(RULES[rule], nps, apply_mode)
 
 
 @pytest.mark.parametrize("rule,apply_mode", [("ftrl_pow", "per_push"), ("proximal_adagrad_l1", "merged"),
@@ -271,14 +225,14 @@ def test_lockstep_under_a_learning_rate_schedule(rule, apply_mode):
 
     opt = dataclasses.replace(RULES[rule], schedule=LrSchedule("exponential_decay", decay_steps=2, decay_rate=0.5))
     assert len({opt.lr_at(i) for i in range(8)}) == 8
-    _lockstep(opt, 2, apply_mode)
+    _harness.cpu_optimizer_lockstep(opt, 2, apply_mode)
 
 
 @pytest.mark.parametrize("rule", ["ftrl_v2", "proximal_sgd_l1", "adadelta_rho"])
 def test_lockstep_with_moving_averages(rule):
     import dataclasses
 
-    _lockstep(dataclasses.replace(RULES[rule], moving_average_decay=0.9), 1, "per_push", ema=True)
+    _harness.cpu_optimizer_lockstep(dataclasses.replace(RULES[rule], moving_average_decay=0.9), 1, "per_push", ema=True)
 
 
 @pytest.mark.parametrize("kind", ["proximal_adagrad", "ftrl"])
@@ -286,7 +240,7 @@ def test_large_l1_leaves_the_same_exact_zeros_as_the_reference(kind):
     """A large l1 sets most of hid_w to exact zeros (the proximal step's soft threshold; FTRL's |linear| <= l1), and they
     sit where the reference's are, element for element."""
     opt = OptimizerConfig(kind, 0.05, l1_regularization_strength=0.05 if kind == "ftrl" else 0.5)
-    got, ref = _lockstep(opt, 2, "per_push", steps=6)
+    got, ref = _harness.cpu_optimizer_lockstep(opt, 2, "per_push", steps=6)
     zg, zr = got["hid_w"] == 0, ref["hid_w"] == 0
     assert zr.float().mean() > 0.5, float(zr.float().mean())
     assert torch.equal(zg, zr), int((zg != zr).sum())
@@ -297,8 +251,7 @@ def test_large_l1_leaves_the_same_exact_zeros_as_the_reference(kind):
 def test_worker_refuses_a_ps_with_another_optimizer(ps_kind, w_kind):
     spec = mlp.book_model(32)
     cfg = EngineConfig(backend="cpu")
-    ports = [_free_port(), _free_port()]
-    cluster = ClusterSpec((f"127.0.0.1:{ports[0]}",), (f"127.0.0.1:{ports[1]}",))
+    cluster = ClusterSpec((f"127.0.0.1:{free_port()}",), (f"127.0.0.1:{free_port()}",))
     ps = ParameterServer(cluster, 0, spec, OptimizerConfig(ps_kind, 1e-3), cfg)
     try:
         w = Worker(cluster, 0, spec, OptimizerConfig(w_kind, 1e-3), cfg)
@@ -369,32 +322,14 @@ def test_checkpoints_of_other_kinds_are_refused_and_older_ones_restore():
             ckpt.restore_latest(cl.worker, d2)
 
 
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, os.path.join(ROOT, "distributed_server-basic.py"), "--job_name", job, "--task_index",
-           str(idx), "--ps_hosts", ps_hosts, "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_cli_ftrl_one_ps_two_worker_processes():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "400", "--learning_rate", "0.5", "--optimizer", "ftrl"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ws = [_spawn("worker", i, ps_hosts, worker_hosts, common) for i in (1, 0)]
-    outs = [_finish(w, 120) for w in ws]
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ws = [t.spawn("worker", i, common) for i in (1, 0)]
+        outs = [t.finish(w, 120) for w in ws]
+        outp = t.finish(ps, 60)
     for w, o in zip(ws, outs):
         assert w.returncode == 0, o
         assert o.splitlines()[:2] == ["job name : worker", f"task index : {1 if w is ws[0] else 0}"]

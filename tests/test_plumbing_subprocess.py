@@ -1,52 +1,28 @@
 """The README recipe of the reference (1 ps + 2 workers as separate OS processes on 127.0.0.1 ports) on the CPU
 backend: real processes, TCP rendezvous, POSIX-shm peer memory. BASELINE.json config 1 / SURVEY §4 item 2."""
 import os
-import socket
 import subprocess
 import sys
 import time
 
+import _harness
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SCRIPT = os.path.join(ROOT, "distributed_server-basic.py")
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(job, idx, ps_hosts, worker_hosts, extra=()):
-    cmd = [sys.executable, SCRIPT, "--job_name", job, "--task_index", str(idx), "--ps_hosts", ps_hosts,
-           "--worker_hosts", worker_hosts, "--backend", "cpu", *extra]
-    env = dict(os.environ, PYTHONPATH=ROOT, PYTHONUNBUFFERED="1")
-    return subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, cwd=ROOT)
-
-
-def _finish(p, timeout):
-    try:
-        out, _ = p.communicate(timeout=timeout)
-    except subprocess.TimeoutExpired:
-        p.kill()
-        out, _ = p.communicate()
-        pytest.fail(f"process timed out; output so far:\n{out}")
-    return out
-
-
 @pytest.mark.timeout(180)
 def test_one_ps_two_workers_processes():
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "300", "--learning_rate", "0.001"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    time.sleep(0.5)
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common)      # non-chief first: must wait for the chief's init
-    time.sleep(0.5)
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    out0, out1 = _finish(w0, 120), _finish(w1, 120)
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        time.sleep(0.5)
+        w1 = t.spawn("worker", 1, common)      # non-chief first: must wait for the chief's init
+        time.sleep(0.5)
+        w0 = t.spawn("worker", 0, common)
+        out0, out1 = t.finish(w0, 120), t.finish(w1, 120)
+        outp = t.finish(ps, 60)
     assert w0.returncode == 0, out0
     assert w1.returncode == 0, out1
     assert ps.returncode == 0, outp
@@ -64,17 +40,14 @@ def test_one_ps_two_workers_processes():
 def test_ps_blocks_forever_like_server_join():
     """Reference ps never exits (server.join(), DS:83): without --ps_exit_when_done it must still be alive after
     the only worker has finished."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()}"
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, ["--train_steps", "40"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, ["--train_steps", "40", "--log_every", "20"])
-    out0 = _finish(w0, 90)
-    assert w0.returncode == 0, out0
-    assert "Train step 20, loss:" in out0 and "Train step 40, loss:" in out0
-    time.sleep(1.0)
-    assert ps.poll() is None, "ps task exited although the reference's ps blocks forever"
-    ps.kill()
-    ps.communicate()
+    with _harness.Tasks(n_workers=1) as t:
+        ps = t.spawn("ps", 0, ["--train_steps", "40"])
+        w0 = t.spawn("worker", 0, ["--train_steps", "40", "--log_every", "20"])
+        out0 = t.finish(w0, 90)
+        assert w0.returncode == 0, out0
+        assert "Train step 20, loss:" in out0 and "Train step 40, loss:" in out0
+        time.sleep(1.0)
+        assert ps.poll() is None, "ps task exited although the reference's ps blocks forever"
 
 
 def test_bad_invocations():
@@ -93,18 +66,17 @@ def test_worker_crash_is_detected_and_training_continues():
     """Failure detection (SURVEY §5): worker 1 crashes mid-run (fault injection); the ps declares it dead after
     `--worker_timeout` seconds without a heartbeat, worker 0 trains on to the target global step, and the ps
     (asked to exit when done) does not wait for the dead worker forever."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "600", "--learning_rate", "0.001"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done", "--worker_timeout", "3"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common + ["--inject_fault", "50"])
-    out1 = _finish(w1, 120)
-    assert w1.returncode == 42 and "[fault injection] worker 1 dies" in out1, out1
-    out0 = _finish(w0, 150)
-    assert w0.returncode == 0, out0
-    assert "Train step 600, loss:" in out0 or "Train step 500, loss:" in out0, out0
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done", "--worker_timeout", "3"])
+        w0 = t.spawn("worker", 0, common)
+        w1 = t.spawn("worker", 1, common + ["--inject_fault", "50"])
+        out1 = t.finish(w1, 120)
+        assert w1.returncode == 42 and "[fault injection] worker 1 dies" in out1, out1
+        out0 = t.finish(w0, 150)
+        assert w0.returncode == 0, out0
+        assert "Train step 600, loss:" in out0 or "Train step 500, loss:" in out0, out0
+        outp = t.finish(ps, 60)
     assert ps.returncode == 0, outp
     assert "worker 1 presumed dead" in outp, outp
 
@@ -114,18 +86,17 @@ def test_crashed_worker_can_be_restarted_and_rejoins():
     """Elastic recovery (the reference's `_RecoverableSession`, SURVEY §3.4 / §5): worker 1 crashes, is started
     again with the same task index, the ps re-admits it (new incarnation: fresh push sequence and inbox) and it
     trains on with worker 0 until the shared global step reaches the target."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "2500", "--learning_rate", "0.001", "--log_every", "500"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done", "--worker_timeout", "30"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common + ["--inject_fault", "30"])
-    out1 = _finish(w1, 120)
-    assert w1.returncode == 42, out1
-    w1b = _spawn("worker", 1, ps_hosts, worker_hosts, common + ["--metrics_file", os.devnull, "--log_steps_per_sec"])
-    out1b = _finish(w1b, 200)
-    out0 = _finish(w0, 200)
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done", "--worker_timeout", "30"])
+        w0 = t.spawn("worker", 0, common)
+        w1 = t.spawn("worker", 1, common + ["--inject_fault", "30"])
+        out1 = t.finish(w1, 120)
+        assert w1.returncode == 42, out1
+        w1b = t.spawn("worker", 1, common + ["--metrics_file", os.devnull, "--log_steps_per_sec"])
+        out1b = t.finish(w1b, 200)
+        out0 = t.finish(w0, 200)
+        outp = t.finish(ps, 60)
     assert w1b.returncode == 0, out1b
     assert w0.returncode == 0, out0
     assert ps.returncode == 0, outp
@@ -140,18 +111,17 @@ def test_restarted_chief_does_not_reinitialize_live_variables():
     """Round-1 advisor finding: a restarted chief (worker 0) used to run the initialisers again on the live ps shards
     (parameters and Adam slots reset while global_step and the per-item step counts kept running, loss jumped from
     ~4e-5 to 0.08). It must see that the variables are live and simply rejoin."""
-    ps_hosts = f"127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "4000", "--learning_rate", "0.001", "--log_every", "100", "--chunk_sleep", "0.1"]
-    ps = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common + ["--inject_fault", "200"])
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common)
-    out0 = _finish(w0, 120)
-    assert w0.returncode == 42, out0
-    w0b = _spawn("worker", 0, ps_hosts, worker_hosts, common + ["--metrics_file", os.devnull, "--log_steps_per_sec"])
-    out0b = _finish(w0b, 240)
-    out1 = _finish(w1, 240)
-    outp = _finish(ps, 60)
+    with _harness.Tasks() as t:
+        ps = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        w0 = t.spawn("worker", 0, common + ["--inject_fault", "200"])
+        w1 = t.spawn("worker", 1, common)
+        out0 = t.finish(w0, 120)
+        assert w0.returncode == 42, out0
+        w0b = t.spawn("worker", 0, common + ["--metrics_file", os.devnull, "--log_steps_per_sec"])
+        out0b = t.finish(w0b, 240)
+        out1 = t.finish(w1, 240)
+        outp = t.finish(ps, 60)
     assert w0b.returncode == 0, out0b
     assert w1.returncode == 0, out1
     assert ps.returncode == 0, outp
@@ -195,16 +165,15 @@ def test_two_ps_row_split_two_workers_processes():
     """`--ps_hosts` is a list in the reference (DS:73-77); with `--sharding row_split` the hidden weight itself is
     split over both ps processes, so every push of every worker goes to two shards. The exit lines give the counters:
     the shard that owns the step counter must have seen exactly the sum of the workers' steps."""
-    ps_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
-    worker_hosts = f"127.0.0.1:{_free_port()},127.0.0.1:{_free_port()}"
     common = ["--train_steps", "240", "--learning_rate", "0.001", "--sharding", "row_split"]
-    ps0 = _spawn("ps", 0, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    ps1 = _spawn("ps", 1, ps_hosts, worker_hosts, common + ["--ps_exit_when_done"])
-    time.sleep(0.5)
-    w1 = _spawn("worker", 1, ps_hosts, worker_hosts, common)
-    w0 = _spawn("worker", 0, ps_hosts, worker_hosts, common)
-    out0, out1 = _finish(w0, 120), _finish(w1, 120)
-    outp0, outp1 = _finish(ps0, 60), _finish(ps1, 60)
+    with _harness.Tasks(n_ps=2) as t:
+        ps0 = t.spawn("ps", 0, common + ["--ps_exit_when_done"])
+        ps1 = t.spawn("ps", 1, common + ["--ps_exit_when_done"])
+        time.sleep(0.5)
+        w1 = t.spawn("worker", 1, common)
+        w0 = t.spawn("worker", 0, common)
+        out0, out1 = t.finish(w0, 120), t.finish(w1, 120)
+        outp0, outp1 = t.finish(ps0, 60), t.finish(ps1, 60)
     for p, o in ((w0, out0), (w1, out1), (ps0, outp0), (ps1, outp1)):
         assert p.returncode == 0, o
     done = [int(l.split("local_steps=")[1].split()[0].rstrip(",")) for l in (out0 + out1).splitlines() if "local_steps=" in l]
